@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- decoded audio-seconds/sec of the synthesis back-end, every BASELINE.json config in ONE line.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 Headline (`value`, `roofline`, `e2e`, `cpu_baseline`): BASELINE config 2 -- MP3 MPEG-1 44.1 kHz stereo, 8192 frames
 (64 streams x 128 consecutive frames) per GPU.  `value` is measured with inputs resident in HBM; `e2e` goes through the
@@ -15,13 +15,22 @@ table-blob broadcast at init (weak scaling); every rank checks a sample of its P
 `--impl reference` times the CPU restatement of the reference's own scalar path (oracle/, built with -march=native on
 this box) on all host threads -- the Rust toolchain does not exist here, see DESIGN.md.  Its inputs come from the
 oracle's own tables: that arm never maps the product library.
+
+`--dump-outputs DIR` writes what the last timed step of each config computed, as float32 .npy files: mp3_pcm.npy (the
+headline, every other frame of the 8192-frame batch: 4096 x 2 x 1152, 38 MB) and, unless --no-configs, a fixed seeded
+sample of 512 frames / packets of aac_pcm.npy and vorbis_pcm.npy and of 256 of each codec of the mixed corpus
+(mixed_mp3_pcm.npy, mixed_aac_pcm.npy, mixed_vorbis_pcm.npy), about 53 MB in all.  The inputs are seeded, so two builds run with the same arguments can be
+compared output for output.  The tree itself is never written: the -march=native oracle goes to a temporary directory.
 """
 import argparse
+import atexit
 import ctypes
 import json
 import os
+import shutil
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -33,13 +42,14 @@ sys.path.insert(0, ROOT)
 N_STREAMS = 64
 FRAMES_PER_STREAM = 128
 N_FRAMES = N_STREAMS * FRAMES_PER_STREAM
-N_BUFFER_SETS = 4  # rotating input/output sets: 4 x ~150 MB > 126 MB L2
+N_BUFFER_SETS = 4  # rotating input/output sets: 4 x ~150 MB, far beyond the 50 MB L2 of an H100
 WORKLOAD = "MP3 MPEG-1 Layer III 44.1kHz stereo, batch=8192 frames (64 streams x 128 frames), synthetic spectra"
 # config 5: 65 536 streams over 8 GPUs = 8192 per GPU; 50 % MP3 / 30 % AAC-LC / 20 % Vorbis, MIXED_FRAMES units per stream
 MIXED_STREAMS_PER_GPU = 8192
 MIXED_SPLIT = (4096, 2458, 1638)
 MIXED_FRAMES = 8
 METRIC = "decoded audio-seconds/sec (44.1kHz stereo)"
+DUMP_SEED = 20240601  # which frames / packets --dump-outputs samples: fixed, so that two builds dump the same ones
 
 
 def _dist_env():
@@ -82,11 +92,14 @@ class ClockSampler(threading.Thread):
 # ---- CPU arm: the oracle (C++ restatement of the reference's scalar path), built for THIS box ---------------------------
 
 def _load_oracle_native():
-    """Builds oracle/ with -march=native ON THIS BOX (the CPU baseline must use this host's ISA)."""
+    """Builds oracle/ with -march=native ON THIS BOX (the CPU baseline must use this host's ISA), into a temporary
+    directory: the tree may be read-only."""
     from tests import _oracle
-    out = os.path.join(ROOT, "oracle", "_build", "liboracle_native.so")
+    tmp = tempfile.mkdtemp(prefix="symgpu-oracle-")
+    atexit.register(shutil.rmtree, tmp, True)
+    out = os.path.join(tmp, "liboracle_native.so")
     try:
-        _oracle.build(arch="-march=native", out="_build/liboracle_native.so")
+        _oracle.build(arch="-march=native", out=out)
         return _oracle.load(out), "-march=native"
     except Exception:
         return _oracle.load(), "-march=x86-64-v3"
@@ -312,6 +325,15 @@ def run_ours(args):
         barrier()
         return float(np.mean([a.elapsed_time(b) for a, b in evs])), e_first.elapsed_time(e_last)
 
+    def dump(name, out, n):
+        """Saves a fixed, seeded sample of n units (first axis) of a device output as DIR/<name>.npy, float32."""
+        if not args.dump_outputs or rank != 0:
+            return
+        idx = np.sort(np.random.default_rng(DUMP_SEED).choice(out.shape[0], min(n, out.shape[0]), replace=False))
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        sample = out[torch.from_numpy(idx).to(out.device)].cpu().numpy().astype(np.float32)
+        np.save(os.path.join(args.dump_outputs, name + ".npy"), sample)
+
     def time_host(call, n):
         """2 warm-up calls, then n calls timed one by one on the host clock (each returns after the result is back in
         host memory).  (total seconds, median seconds)"""
@@ -329,15 +351,11 @@ def run_ours(args):
     if os.path.exists(peaks_path):
         peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+        peak, peak_src = 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s)"
 
-    def roofline(algo_bytes, kernel_ms, traffic_key=None):
+    def roofline(algo_bytes, kernel_ms):
         ach = algo_bytes / (kernel_ms * 1e-3) / 1e9
-        traffic = None
-        summary = os.path.join(ROOT, "profiles", "r02_ncu_dram_traffic.json")  # per-launch dram bytes of the committed ncu captures
-        if traffic_key and os.path.exists(summary):
-            traffic = json.load(open(summary)).get(traffic_key)
-        return {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": traffic,
+        return {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
                 "peak_source": peak_src, "algorithmic_bytes_per_launch": algo_bytes, "kernel_ms": kernel_ms}
 
     # ---- headline: MP3 config 2 -----------------------------------------------------------------
@@ -359,6 +377,15 @@ def run_ours(args):
         u_t, s_t, p_t = sets[i % N_BUFFER_SETS]
         eng.mp3_synth_dev(u_t, s_t, runs, p_t)
 
+    # what the numbers were measured on: card name and the power limit it runs under
+    device_info = {"name": torch.cuda.get_device_name(dev), "power_limit_w": None}
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(local_rank), "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=10).stdout.strip()
+        device_info["power_limit_w"] = float(out)
+    except (OSError, ValueError, subprocess.SubprocessError):
+        pass
+
     sampler = ClockSampler(local_rank)
     sampler.start()
     launches0 = eng.launch_count
@@ -366,6 +393,11 @@ def run_ours(args):
     avg_kernel_ms, total_ms = time_device(step, args.steps, args.warmup)
     wall = time.perf_counter() - t0
     launches = eng.launch_count - launches0 - args.warmup
+    if args.dump_outputs and rank == 0:
+        # the PCM of the last timed step, before the untimed launches below overwrite the buffer sets
+        last = sets[(args.warmup + args.steps - 1) % N_BUFFER_SETS][2]
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "mp3_pcm.npy"), last[::2].cpu().numpy().astype(np.float32))
     # The clock sampler polls nvidia-smi (a few hundred ms per query, and its driver calls stall CUDA API calls for tens of
     # ms): it covers the device-timed region above and is stopped before the host-timed regions below.  A short timed
     # region may end before three queries have returned: the same launches are then kept going, untimed, until they have.
@@ -438,6 +470,7 @@ def run_ours(args):
                    torch.empty((len(au), 2, 1024), dtype=torch.float32, device=dev)) for _ in range(N_BUFFER_SETS)]
         k_ms, t_ms = time_device(lambda i: eng.aac_synth_dev(a_sets[i % N_BUFFER_SETS][0], a_sets[i % N_BUFFER_SETS][1], len(at),
                                                              a_sets[i % N_BUFFER_SETS][2], ar, a_sets[i % N_BUFFER_SETS][3]), c_steps, 3)
+        dump("aac_pcm", a_sets[(3 + c_steps - 1) % N_BUFFER_SETS][3], 512)  # the buffer of the last timed step
         del a_sets
         au_pin, at_pin, ac_pin = pin(au.view(np.uint8).reshape(-1)), pin(at.view(np.uint8).reshape(-1)), pin(ac)
         ap_pin = torch.empty((len(au), 2, 1024), dtype=torch.float32).pin_memory()
@@ -448,7 +481,7 @@ def run_ours(args):
         cfg_static["aac"] = {"workload": f"AAC-LC 48kHz stereo, batch={len(au)} frames (64 streams x 128), TNS in 20% of channel-frames "
                                          f"({len(at)} filters), all four window sequences",
                              "audio_s_per_step": len(au) * 1024 / 48000.0, "algo": len(au) * workloads.AAC_ALGO_BYTES_PER_FRAME,
-                             "h2d": au.nbytes + at.nbytes + ac.nbytes, "d2h": len(au) * 8192, "traffic_key": "aac"}
+                             "h2d": au.nbytes + at.nbytes + ac.nbytes, "d2h": len(au) * 8192}
 
         # config 4: Vorbis
         wl = wls["vorbis"]
@@ -460,6 +493,7 @@ def run_ours(args):
         k_ms, t_ms = time_device(lambda i: eng.vorbis_synth_dev(v_sets[i % N_BUFFER_SETS][0], v_sets[i % N_BUFFER_SETS][1],
                                                                 v_sets[i % N_BUFFER_SETS][2], wl["runs"], slot,
                                                                 v_sets[i % N_BUFFER_SETS][3]), c_steps, 3)
+        dump("vorbis_pcm", v_sets[(3 + c_steps - 1) % N_BUFFER_SETS][3], 512)
         del v_sets
         vr_pin, vy_pin = pin(wl["residue"]), pin(wl["floor_y"])
         vp_pin = torch.empty((len(wl["units"]), 2, slot), dtype=torch.float32).pin_memory()
@@ -470,7 +504,7 @@ def run_ours(args):
                                             f"(64 streams x 128, {100 * long_share:.0f}% long)",
                                 "audio_s_per_step": float(wl["out_len"].sum()) / 44100.0, "algo": _vorbis_algo_bytes(wl),
                                 "h2d": wl["units"].nbytes + wl["floor_y"].nbytes + wl["residue"].nbytes,
-                                "d2h": len(wl["units"]) * 2 * slot * 4, "traffic_key": "vorbis"}
+                                "d2h": len(wl["units"]) * 2 * slot * 4}
 
         # config 5: this rank's 8192 streams of the 65 536-stream corpus (stream i -> GPU i mod 8), three launches per step
         (mu, ms_, mr), (xu, xt, xc, xr), mwl = wls["mixed"]
@@ -489,6 +523,9 @@ def run_ours(args):
             eng.aac_synth_dev(d_xu, d_xt, len(xt), d_xc, xr, d_xp)
             eng.vorbis_synth_dev(d_vu, d_vy, d_vr, mwl["runs"], mwl["slot"], d_vp)
         k_ms, t_ms = time_device(mixed_step, min(c_steps, 20), 3)
+        dump("mixed_mp3_pcm", d_mp, 256)
+        dump("mixed_aac_pcm", d_xp, 256)
+        dump("mixed_vorbis_pcm", d_vp, 256)
         del d_mu, d_ms, d_mp, d_xu, d_xt, d_xc, d_xp, d_vu, d_vy, d_vr, d_vp
         m_pins = [pin(mu.view(np.uint8).reshape(-1)), pin(ms_), torch.empty((len(mu), 2, 1152), dtype=torch.float32).pin_memory(),
                   pin(xc), torch.empty((len(xu), 2, 1024), dtype=torch.float32).pin_memory(),
@@ -533,14 +570,14 @@ def run_ours(args):
             "ms_per_step": total_ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "f32", "data": "synthetic",
             "config": {"workload": WORKLOAD, "frames_per_gpu": N_FRAMES, "parallelism": f"streams sharded over {world} GPU(s)",
-                       "l2": f"rotating {N_BUFFER_SETS} input/output buffer sets ({N_BUFFER_SETS * 151} MB) > 126 MB L2",
+                       "l2": f"rotating {N_BUFFER_SETS} input/output buffer sets ({N_BUFFER_SETS * 151} MB) > 50 MB L2",
                        "fma": "disabled (bit-exact parity with the reference)",
-                       "kernel": os.environ.get("SYMGPU_MP3_KERNEL", "auto (per launch plan; this batch of 256-granule runs: mp3_synth_kernel<16,16,0,1>, "
-                                                                     "the first-generation kernel with the packed window phase)")},
-            "roofline": dict(roofline(algo_bytes, avg_kernel_ms, "mp3"),
-                             note="FMA is off for parity, so the kernel is FP32-pipe bound, not HBM bound: the no-FMA floor for this "
-                                  "batch is ~31 us (1.1e9 f32 lane-ops at the measured 35.9e12/s) vs 23 us at the HBM peak; traffic "
-                                  "(when not null) is dram bytes per launch from the ncu capture committed in profiles/"),
+                       "kernel": os.environ.get("SYMGPU_MP3_KERNEL", "auto (per launch plan; this batch of 256-granule runs: mp3_synth_kernel<16,16,0>, "
+                                                                     "the first-generation kernel)")},
+            "device": device_info,
+            "roofline": dict(roofline(algo_bytes, avg_kernel_ms),
+                             note="FMA is off for parity (1.1e9 f32 lane-ops per step without it), so the kernel may be bound by "
+                                  "the FP32 pipe rather than by HBM"),
             "e2e": {"value": world * audio_per_step * e2e_steps / e2e_s, "unit": "audio-s/s",
                     "h2d_bytes_per_step": N_FRAMES * (256 + 9216), "d2h_bytes_per_step": N_FRAMES * 9216,
                     "ms_per_step": 1e3 * e2e_s / e2e_steps, "ms_per_step_median": 1e3 * e2e_med, "checksum": checksum},
@@ -595,7 +632,7 @@ def run_ours(args):
                 else:
                     c["value"] = world * audio / (step_ms * 1e-3)
                     c["kernel_ms"] = k_ms
-                    c["roofline"] = roofline(st["algo"], k_ms, st.get("traffic_key"))
+                    c["roofline"] = roofline(st["algo"], k_ms)
                 if "streams_this_job" in st:
                     c["streams"] = st["streams_this_job"]
                 c["unit"] = "audio-s/s"
@@ -617,6 +654,9 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-configs", action="store_true", help="only the MP3 headline (profiling runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the PCM of each config's last timed step (the headline's every other frame, a seeded sample of the "
+                         "others) to DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     if args.impl == "reference":

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Secondary measurements: BASELINE configs[2] (AAC-LC 48 kHz stereo, 8192 frames) and configs[3]
-(Vorbis 44.1 kHz stereo long/short mix, 8192 packets) on one B200, device-resident inputs.
+(Vorbis 44.1 kHz stereo long/short mix, 8192 packets) on one GPU, device-resident inputs.
 Prints one JSON line per codec with the same roofline arithmetic as bench.py (the headline metric
 and the driver contract live in bench.py; this script feeds profiles/ and DESIGN.md)."""
 import argparse
@@ -152,7 +152,7 @@ def main():
         ms = _time_steps(eng, step, args.steps, args.warmup)
         audio = (workloads.mp3_audio_seconds(n_mp3 * Fm) + n_aac * Fm * 1024 / 48000.0 + float(wl["out_len"].sum()) / 44100.0)
         print(json.dumps({"codec": "mixed", "workload": "4096 streams x 16 frames on one context: 2048 MP3 + 1229 AAC-LC + 819 Vorbis "
-                          "(SURVEY config 5 at 1/16 scale; 0.57 GB in + 0.57 GB out per step, far beyond the 126 MB L2)",
+                          "(SURVEY config 5 at 1/16 scale; 0.57 GB in + 0.57 GB out per step, far beyond the 50 MB L2 of an H100)",
                           "value": audio / (ms * 1e-3), "unit": "audio-s/s", "step_ms": ms, "audio_s_per_step": audio}), flush=True)
     if args.codec in ("aac", "both", "all"):
         units, tns, coeffs, runs = workloads.aac_batch(S, F, tns_prob=args.tns)

@@ -1,5 +1,5 @@
 /*
- * symgpu.h -- C ABI of libsymgpu.so, the B200 (sm_100a) batched audio-synthesis engine that
+ * symgpu.h -- C ABI of libsymgpu.so, the H100 (sm_90a) batched audio-synthesis engine that
  * replaces the f32 DSP back-end of Symphonia's MP3 / AAC-LC / Vorbis decoders.
  *
  * The seam this ABI sits on is the point inside each reference decoder where the serial
@@ -54,10 +54,11 @@ typedef struct symgpu_ctx symgpu_ctx; /* opaque */
 
 /* Creates a context on CUDA device `device` (cudaSetDevice ordinal), builds every lookup table
  * on the host with libm (see DESIGN.md "tables") and uploads them.  Fails with SYMGPU_ERR_CUDA
- * when no usable sm_100 device is present: there is NO CPU fallback behind this ABI.
+ * when no CUDA device is present, and with SYMGPU_ERR_UNSUPPORTED when the device is not sm_90 (the kernels are
+ * sm_90a code): there is NO CPU fallback behind this ABI.
  * The calling thread is bound to the CPUs of the device's NUMA node (sysfs numa_node of the PCI device, intersected
  * with the thread's current affinity), so that pinned host buffers it allocates afterwards are node-local by first
- * touch -- one rank per GPU on a two-socket B200 node otherwise pushes half of its PCIe traffic across the socket link.
+ * touch -- one rank per GPU on a two-socket node otherwise pushes half of its PCIe traffic across the socket link.
  * SYMGPU_NUMA_BIND=0 in the environment switches this off. */
 symgpu_status symgpu_ctx_create(int device, symgpu_ctx** out);
 /* NUMA node of CUDA device `device` (-1 if the platform does not say); binds the calling thread to that node's CPUs and
@@ -666,8 +667,7 @@ symgpu_status symgpu_mp3_entropy_decode_cpu(const uint8_t* data, size_t n, const
                                             symgpu_mp3_gc* units, int16_t* quant, uint32_t* frame_of, size_t* n_good,
                                             symgpu_mp3_frame_info* info, uint32_t* n_rounds);
 
-/* ---- the device path of the front-end.  EXPERIMENTAL in this revision: compiled for sm_100a, not yet run on a GPU
- * (tests/test_mp3_entropy_gpu.py is opt-in, SYMGPU_TEST_ENTROPY=1). ------------------------------------------------ */
+/* ---- the device path of the front-end (tests/test_mp3_entropy_gpu.py) --------------------------------------------- */
 /* One thread per job, the same decode functions as symgpu_mp3_entropy_run_cpu.  All pointers are device memory;
  * d_failed[n_jobs / 4] must be zeroed by the caller; asynchronous on the context stream. */
 symgpu_status symgpu_mp3_entropy_dev(symgpu_ctx* ctx, const uint8_t* d_md, size_t md_len, const symgpu_mp3_gc_job* d_jobs, size_t n_jobs,

@@ -1,4 +1,4 @@
-"""symphonia_b200 -- B200 (sm_100a) batched audio-synthesis engine behind Symphonia's decoder seam.
+"""symphonia_b200 -- H100 (sm_90a) batched audio-synthesis engine behind Symphonia's decoder seam.
 
 The product is `libsymgpu.so` (CUDA kernels + C ABI, see include/symgpu.h).  This package is the
 thin host-side harness: a ctypes binding (`_native`), an `Engine` wrapper that moves numpy / torch

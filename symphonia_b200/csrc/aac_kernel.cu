@@ -1,4 +1,4 @@
-// AAC-LC synthesis for sm_100a: TNS (aac/ics/tns.rs:149-199) then the filterbank of Dsp::synth
+// AAC-LC synthesis for sm_90a: TNS (aac/ics/tns.rs:149-199) then the filterbank of Dsp::synth
 // (aac/dsp.rs:57-158): 1024-point or 8 x 128-point IMDCT, sine / KBD windows, the four window
 // sequences, overlap-add through the per-channel `delay` line.
 //
@@ -58,7 +58,7 @@ __device__ __forceinline__ void tns_lines(float* col, int cnt, int m0, float (&h
     // compile time: no register moves between lines (the shifting form below spends ORDER of its ~3.3 ORDER instructions per
     // line on them).  Same operations on the same operands in the same order.
     constexpr int L = ORDER >= 4 ? ORDER : ORDER == 3 ? 6 : 4;
-#ifndef SYMGPU_TNS_NO_RING // (A/B switch of tools/gpu_calls/r02_gpu_ab.sh)
+#ifndef SYMGPU_TNS_NO_RING // (A/B switch: TNS history in shared memory instead of the register ring)
     if (k + L <= cnt) {
         float c[ORDER];
 #pragma unroll
@@ -308,7 +308,6 @@ constexpr int kAacKWarp = kAacChunkFramesWarp; // frames per chunk, ONE warp per
 #define SYMGPU_AAC_PRE_UNROLL 2
 #endif
 constexpr int kAacPreUnroll = SYMGPU_AAC_PRE_UNROLL; // pre-twiddle iterations (4 spectrum loads each) in flight per lane; 2 / 4 / 8
-                                                     // measured on one box: 105.9-106.2 us each (tools/gpu_calls/r02_gpu_ab.sh) -- no effect
 constexpr int kAacKZ = kAacChunkFramesZ;       // the same with frame slots in the Z layout
 struct alignas(16) AacFrameSmem {
     float out[2048];          // spectrum (first 1024 floats) until the pre-twiddle has consumed it, then pcm_long
@@ -671,10 +670,10 @@ int aac_kernel_variant() {
     return mode;
 }
 bool aac_warp_per_frame() { return aac_kernel_variant() != 0; }
-// Frames per chunk of the Z kernel, i.e. 16, 10 or 8 warps per CTA at 2, 3 or 4 CTAs per SM.  Measured on one box: long runs
-// (8192 frames = 128 stream-channels x 128) 106 / 114 / 116 us with 15 / 9 / 7; short runs (the mixed corpus: 8-16 frames per
-// stream and call, a chunk plus its state slot fills 9 of the 16 warps) 1.166 / 1.115 / 1.130 ms per step.  So the plan takes 9
-// when the runs are short and 15 otherwise; SYMGPU_AAC_Z_FRAMES = 15 | 9 | 7 pins it.
+// Frames per chunk of the Z kernel, i.e. 16, 10 or 8 warps per CTA at 2, 3 or 4 CTAs per SM.  Long runs fill the large
+// chunks; short runs (the mixed corpus: 8-16 frames per stream and call, a chunk plus its state slot fills 9 of the 16 warps)
+// leave warps of a large chunk idle.  So the plan takes 9 when the runs are short and 15 otherwise; SYMGPU_AAC_Z_FRAMES =
+// 15 | 9 | 7 pins it.
 int aac_z_frames(uint32_t mean_run_frames) {
     static int pinned = -1;
     if (pinned < 0) {

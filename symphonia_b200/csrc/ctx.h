@@ -21,7 +21,7 @@ struct symgpu_ctx {
     uint64_t launches = 0;
     symgpu_async_mp3* async_mp3 = nullptr;
     int numa_node = -1; // node the creating thread was bound to (-1: platform does not say, -2: binding switched off)
-    // Layer III kernel choice (SYMGPU_MP3_KERNEL): 0 auto (by plan shape: long runs -> first generation with the packed window,
+    // Layer III kernel choice (SYMGPU_MP3_KERNEL): 0 auto (by plan shape: long runs -> first generation,
     // short runs -> second generation), 1 always the first generation, 2 always the second
     int mp3_kernel_mode = 0;
     // tables
@@ -53,9 +53,8 @@ struct symgpu_ctx {
     // copy pipeline of the host entry points: H2D on copy_in, kernels on `stream`, D2H on copy_out
     static constexpr int kMaxSlices = 32;
     // pinned (device-mapped) host buffers handed straight to the kernels: 0 never (default), 1 output only (PCM stores cross
-    // PCIe from the kernel, no D2H copy), 2 input too (TMA reads across PCIe).  Measured on a B200 (profiles/r02l): 8192 MP3 frames
-    // take 2.20 ms staged through the copy pipeline, 2.36 ms with both directions zero-copy, 3.2 ms with output only -- SM stores to
-    // host memory reach ~25 GB/s against the copy engines' ~50 -- so the staged pipeline stays the default.  SYMGPU_ZERO_COPY
+    // PCIe from the kernel, no D2H copy), 2 input too (TMA reads across PCIe).  SM stores to host memory
+    // are slower than the copy engines, so the staged pipeline is the default.  SYMGPU_ZERO_COPY
     int zero_copy = 0;
     bool zero_copy_small = true; // host batches below the pipeline threshold with mapped buffers: one launch on the caller's memory
     int h2d_ahead = 2; // slices whose H2D copy is queued before the host's descriptor check and planning (SYMGPU_H2D_AHEAD)
@@ -63,7 +62,7 @@ struct symgpu_ctx {
     cudaStream_t copy_in = nullptr, copy_out = nullptr;
     cudaStream_t copy_in2 = nullptr, copy_out2 = nullptr; // odd slices (SYMGPU_COPY_STREAMS=2): the next copy is already queued on
                                                           // another engine when one ends, so the link does not idle between slices
-    int copy_streams = 1; // 2 was measured slower (2.6 ms against 2.27 ms per step): copies of one direction on two streams delay each other
+    int copy_streams = 1; // 2: copies of one direction on two streams can delay each other
     cudaEvent_t ev_in[kMaxSlices] = {}, ev_k[kMaxSlices] = {};
     cudaEvent_t ev_units = nullptr;
     // ---- AAC / Vorbis ----

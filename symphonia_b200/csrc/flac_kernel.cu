@@ -1,4 +1,4 @@
-// FLAC integer restoration for sm_100a (SURVEY §8f N4): what FlacDecoder::decode_inner does after the Rice stage.
+// FLAC integer restoration for sm_90a (SURVEY §8f N4): what FlacDecoder::decode_inner does after the Rice stage.
 //   fixed_predict / lpc_predict   symphonia-bundle-flac/src/decoder.rs:663-752
 //   samples_shl                   decoder.rs:387-394
 //   decorrelate_*                 decoder.rs:32-82

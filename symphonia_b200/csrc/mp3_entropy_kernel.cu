@@ -1,5 +1,4 @@
-// Device side of the MP3 entropy front-end (SURVEY §8f N1, EXPERIMENTAL: written in a round whose GPU budget was spent,
-// compiled for sm_100a but not yet run -- tests/test_mp3_entropy_gpu.py is opt-in until it has been).
+// Device side of the MP3 entropy front-end (SURVEY §8f N1; parity in tests/test_mp3_entropy_gpu.py).
 //
 // One thread decodes one granule-channel with the very functions the CPU front-end runs (mp3_entropy.h), from the
 // compacted main-data stream and the job table symgpu_mp3_entropy_plan builds from side information alone.  For 8192

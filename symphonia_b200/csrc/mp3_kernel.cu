@@ -1,4 +1,4 @@
-// Fused MPEG Layer III synthesis kernel for sm_100a:
+// Fused MPEG Layer III synthesis kernel for sm_90a:
 //   requantize -> joint stereo -> reorder -> antialias -> IMDCT-36/12 + window + overlap-add
 //   -> frequency inversion -> DCT-32 -> 512-tap polyphase window  (layer3/mod.rs:421-477)
 // in ONE launch, PCM written straight to HBM.  No intermediate ever leaves the SM.
@@ -9,14 +9,13 @@
 // HBM; any other tile recomputes a 2-granule halo (the overlap of granule g-1 needs IMDCT of g-1;
 // the 15 history slots need the time samples of g-1, which need the overlap of g-2).  The grid is
 // PERSISTENT: one CTA of NW warps per SM walks tiles blockIdx, blockIdx+grid, ... with all its
-// warps in the same phase (several phases live on one SM thrash the instruction cache: measured
-// +30% time with 2 CTAs/SM).  The spectra of the next tile are fetched by TMA bulk copies
+// warps in the same phase (several phases live on one SM thrash the instruction cache, as
+// with 2 CTAs/SM).  The spectra of the next tile are fetched by TMA bulk copies
 // (cp.async.bulk -> mbarrier) while the current tile is in its DCT / window phases.
 //
 // Bit-exactness rules: compiled with -fmad=false; every expression keeps the reference's operand
-// order; tables come from the host (tables.cpp).  ptxas 12.9 contracts mul.rn.f32x2 + add.rn.f32x2
-// into FFMA2 even with --fmad=false, so packed f32x2 arithmetic is NOT used on mul->add chains;
-// tests/test_build.py greps the SASS of this file for FFMA/FFMA2 and fails on any hit.
+// order; tables come from the host (tables.cpp); tests/test_build_and_abi.py greps the SASS for
+// FFMA and fails on any hit.
 #include <cuda_runtime.h>
 
 #include <cstdint>
@@ -259,23 +258,9 @@ __device__ __forceinline__ float2 lds64(uint32_t addr) {
 }
 
 
-// ---- packed f32x2 arithmetic for the (ch0, ch1) pairs of the window phase (round 2, see mp3_kernel_v2.cu for the rules:
-// a packed sum is fma(a, ONE, b) with ONE a kernel argument, because ptxas contracts mul.f32x2 + add.f32x2) ----------------
-__device__ __forceinline__ float2 pk_mul(float2 a, float s) {
-    float2 r;
-    asm("{.reg .b64 ra, rb, rc; mov.b64 ra, {%2,%3}; mov.b64 rb, {%4,%4}; mul.rn.f32x2 rc, ra, rb; mov.b64 {%0,%1}, rc;}"
-        : "=f"(r.x), "=f"(r.y)
-        : "f"(a.x), "f"(a.y), "f"(s));
-    return r;
-}
-__device__ __forceinline__ float2 pk_add(float2 a, float2 b, float one) { // a * 1 + b
-    float2 r;
-    asm("{.reg .b64 ra, rb, rc, rd; mov.b64 ra, {%2,%3}; mov.b64 rb, {%4,%4}; mov.b64 rc, {%5,%6}; fma.rn.f32x2 rd, ra, rb, rc; "
-        "mov.b64 {%0,%1}, rd;}"
-        : "=f"(r.x), "=f"(r.y)
-        : "f"(a.x), "f"(a.y), "f"(one), "f"(b.x), "f"(b.y));
-    return r;
-}
+// ---- (ch0, ch1) pair arithmetic of the window phase: one correctly rounded scalar operation per channel, never contracted
+__device__ __forceinline__ float2 pk_mul(float2 a, float s) { return make_float2(__fmul_rn(a.x, s), __fmul_rn(a.y, s)); }
+__device__ __forceinline__ float2 pk_add(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 
 // Polyphase window of `total` consecutive time slots whose DCT vectors sit in XT rows row0 ..  // PHASE: D window
 // (with the 15 rows before row0 holding the history).  lane = PCM sample index i; each warp walks a
@@ -287,10 +272,10 @@ __device__ __forceinline__ float2 pk_add(float2 a, float2 b, float one) { // a *
 // batch-wide sequence number of the first slot: slots of a frame are contiguous in a PCM plane
 // (plane[gr*576 + t*32 + i]) and frames are SYMGPU_MP3_FRAME_FLOATS apart.
 // TWO_JUMPS: a block of 16 slots may cross two frame boundaries (Layer I: 12 slots per frame).
-template <bool TWO_JUMPS = false, bool PACKED = false>
+template <bool TWO_JUMPS = false>
 __device__ __forceinline__ void window_phase(const float* xt, int row0, int begin, int end, int lane,
                                              const float* __restrict__ synth_d, float* __restrict__ pcm, int slot_seq0,
-                                             int slots_per_frame, bool stereo, float one = 1.0f) {
+                                             int slots_per_frame, bool stereo) {
     const int col_lo = lane < 16 ? 16 + lane : (lane == 16 ? 32 : 48 - lane);
     const int col_hi = lane <= 16 ? 16 - lane : lane - 16;
     float dlo[8], dhi[8];
@@ -326,31 +311,16 @@ __device__ __forceinline__ void window_phase(const float* xt, int row0, int begi
             if (u < cnt) {
                 wl[u] = lds64(a_lo + u * kRowBytes);
                 wh[u] = lds64(a_hi + u * kRowBytes);
-                float o0 = 0.0f, o1 = 0.0f;
-                if constexpr (PACKED) {
-                    float2 acc = make_float2(0.0f, 0.0f);
+                float2 acc = make_float2(0.0f, 0.0f);
 #pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        acc = pk_add(pk_mul(wl[(u - 2 * j) & 15], dlo[j]), acc, one);
-                        acc = pk_add(pk_mul(wh[(u - 2 * j - 1) & 15], dhi[j]), acc, one);
-                    }
-                    o0 = acc.x;
-                    o1 = acc.y;
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const float2 v0 = wl[(u - 2 * j) & 15];
-                        const float2 v1 = wh[(u - 2 * j - 1) & 15];
-                        o0 += v0.x * dlo[j];
-                        o1 += v0.y * dlo[j];
-                        o0 += v1.x * dhi[j];
-                        o1 += v1.y * dhi[j];
-                    }
+                for (int j = 0; j < 8; ++j) {
+                    acc = pk_add(pk_mul(wl[(u - 2 * j) & 15], dlo[j]), acc);
+                    acc = pk_add(pk_mul(wh[(u - 2 * j - 1) & 15], dhi[j]), acc);
                 }
                 float* o = (u < kj ? out0 : out1) + u * 32;
                 if (TWO_JUMPS && u >= kj + slots_per_frame) o += frame_jump;
-                o[off1] = o1;
-                o[0] = o0;
+                o[off1] = acc.y;
+                o[0] = acc.x;
             }
         }
         a_lo += 16 * kRowBytes;
@@ -377,7 +347,7 @@ struct Mp3Smem {
 
 // MULTI = false: every group of the plan is a single tile (the shape of large batches); the loops over the
 // pieces of a group then fold away at compile time.
-template <int T, int NW, bool MULTI, bool PK = false>
+template <int T, int NW, bool MULTI>
 __global__ void __launch_bounds__(NW * 32, NW <= 8 ? 2 : 1) mp3_synth_kernel(Mp3Args a) {
     static_assert(NW >= T, "one warp per granule job (a tile with a halo holds NW - 2 granules)");
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -865,7 +835,7 @@ __global__ void __launch_bounds__(NW * 32, NW <= 8 ? 2 : 1) mp3_synth_kernel(Mp3
                 if (b < e) {
                     const int shift = t.gpf == 2 ? 1 : 0;
                     const int gseq = ((int)t.first_frame << shift) + t.first_gr;
-                    window_phase<false, PK>(xt, 18 * (regions + 1), b, e, lane, tab->synth_d, a.pcm, gseq * 18, 18 << shift, t.n_ch == 2, a.one);
+                    window_phase(xt, 18 * (regions + 1), b, e, lane, tab->synth_d, a.pcm, gseq * 18, 18 << shift, t.n_ch == 2);
                 }
                 first += cnt;
                 regions += t.n_granules + 1;
@@ -1090,29 +1060,13 @@ int mp3_grid_size(cudaError_t* err) {
     return e == cudaSuccess ? grid_for_device[dev & 63] : 0;
 }
 
-static bool g_v1_packed_window = false;
-void mp3_v1_set_packed_window(bool on) { g_v1_packed_window = on; }
-
 cudaError_t mp3_launch(const Mp3Args& a, cudaStream_t stream) {
     constexpr size_t smem = sizeof(Mp3Smem<kMp3TileGranules, kMp3Warps>);
     cudaError_t e = cudaSuccess;
     const int max_grid = mp3_grid_size(&e);
     if (e != cudaSuccess) return e;
     if (a.n_ctas <= 0 || a.n_ctas > max_grid) return cudaErrorInvalidConfiguration;
-    if (g_v1_packed_window) {
-        static bool configured = false;
-        if (!configured) {
-            e = cudaFuncSetAttribute(mp3_synth_kernel<kMp3TileGranules, kMp3Warps, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            if (e == cudaSuccess)
-                e = cudaFuncSetAttribute(mp3_synth_kernel<kMp3TileGranules, kMp3Warps, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            if (e != cudaSuccess) return e;
-            configured = true;
-        }
-        if (a.multi_tile_groups)
-            mp3_synth_kernel<kMp3TileGranules, kMp3Warps, true, true><<<a.n_ctas, kMp3Warps * 32, smem, stream>>>(a);
-        else
-            mp3_synth_kernel<kMp3TileGranules, kMp3Warps, false, true><<<a.n_ctas, kMp3Warps * 32, smem, stream>>>(a);
-    } else if (a.multi_tile_groups)
+    if (a.multi_tile_groups)
         mp3_synth_kernel<kMp3TileGranules, kMp3Warps, true><<<a.n_ctas, kMp3Warps * 32, smem, stream>>>(a);
     else
         mp3_synth_kernel<kMp3TileGranules, kMp3Warps, false><<<a.n_ctas, kMp3Warps * 32, smem, stream>>>(a);

@@ -71,7 +71,6 @@ struct Mp3Args {
     uint32_t* gen;          // [n_streams] state generation; buffer (gen & 1) is current
     unsigned* done;         // retired-CTA counter (self-resetting)
     const Mp3Tables* tab;
-    float one;              // 1.0f: multiplicand of the packed sums of the window phase (opaque to ptxas)
 };
 
 // MPEG Layer I / II polyphase synthesis (mpa12_synth_kernel): tiles are whole frames of one stream, `n_granules`
@@ -94,14 +93,13 @@ int mpa12_tile_frames(int n_slots); // frames per tile
 
 cudaError_t mp3_upload_const(const Mp3Tables& t, cudaStream_t stream);
 cudaError_t mp3_launch(const Mp3Args& a, cudaStream_t stream);
-void mp3_v1_set_packed_window(bool on); // experiment: channel-pair packed FMUL2 / FFMA2 in the window phase of the first-generation kernel
 int mp3_tile_granules();
 int mp3_halo_tile_granules(); // limit for a tile that recomputes its halo (two warps go to the halo granules)
 int mp3_cta_warps();           // warps per CTA = granule jobs per group
 // Persistent grid size of the kernel on the current device (SM count x resident CTAs), <= 0 on error.
 int mp3_grid_size(cudaError_t* err);
 
-// ---- second-generation Layer III kernel (mp3_kernel_v2.cu): warp-autonomous, channel-pair packed FP32 ----
+// ---- second-generation Layer III kernel (mp3_kernel_v2.cu): warp-autonomous, channel pairs in float2 ----
 // A warp owns a SHARE of the batch's granules (a list of Mp3Tile segments, walked in order); share s runs on
 // warp s / grid of CTA s % grid.  Tile flags: kTileLoadState (the segment starts its run: state from HBM),
 // kTileStoreState (it ends its run: state to HBM), kTileCarryIn / kTileCarryOut (the segment continues / is
@@ -123,7 +121,6 @@ struct Mp3V2Args {
     uint32_t* gen;          // [n_streams] state generation; buffer (gen & 1) is current
     unsigned* done;         // retired-CTA counter (self-resetting)
     const Mp3Tables* tab;
-    float one, mone;        // 1.0f, -1.0f: multiplicands of the packed sums (opaque to ptxas, see mp3_kernel_v2.cu)
 };
 cudaError_t mp3v2_upload_const(const Mp3Tables& t, cudaStream_t stream);
 cudaError_t mp3v2_launch(const Mp3V2Args& a, int n_ctas, cudaStream_t stream, bool short_runs);

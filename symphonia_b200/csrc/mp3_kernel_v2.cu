@@ -1,10 +1,9 @@
-// Fused MPEG Layer III synthesis kernel for sm_100a, second generation ("v2"):
+// Fused MPEG Layer III synthesis kernel for sm_90a, second generation ("v2"):
 //   requantize -> joint stereo -> reorder -> antialias -> IMDCT-36/12 + window + overlap-add
 //   -> frequency inversion -> DCT-32 -> 512-tap polyphase window  (layer3/mod.rs:421-477)
 // in ONE launch, PCM written straight to HBM.
 //
-// What changed against mp3_kernel.cu (round 1: 138 us for 8192 frames, 0.17 of the HBM peak, 50 % issue
-// utilisation, 13-18 % of the time in CTA-wide barriers, 107 KB of instructions per tile):
+// What changed against mp3_kernel.cu (CTA-wide barriers between phases, a large instruction footprint per tile):
 //
 //  * WARP-AUTONOMOUS.  A warp owns a SHARE: a contiguous piece of the batch's granules in run order.  It walks
 //    its granules one at a time through every phase with nothing but __syncwarp() -- no CTA barrier, no
@@ -12,17 +11,14 @@
 //    (18 float2 per lane), the last 15 DCT vectors stay in the warp's two-region XT ring in shared memory,
 //    the next granule's spectra arrive by a per-warp TMA bulk copy (cp.async.bulk -> mbarrier) issued as
 //    soon as the current granule's lines are in registers.  12 warps per SM (3 per scheduler, 168
-//    registers, no spills), each in its own phase, share the issue slots; a stall of one warp is filled by
+//    registers; under sm_90a the granule loop spills a few words -- tile loads, the TMA issue, the call of the
+//    out-of-line mixed-block helper -- and that helper passes its operands through local memory by design), each in its own phase, share the issue slots; a stall of one warp is filled by
 //    the others instead of being multiplied by a barrier.
-//  * CHANNEL-PAIR PACKED FP32.  Every value on the path exists once per channel, so lane data is held as
-//    float2 (ch0, ch1) and the arithmetic is Blackwell's packed FMUL2 / FFMA2: half the issue slots of the
-//    scalar code.  Bit-exactness: ptxas 12.9 contracts mul.rn.f32x2 + add.rn.f32x2 into FFMA2 even with
-//    --fmad=false, so this file NEVER emits add.f32x2 / sub.f32x2.  A packed sum is fma(a, ONE, b) and a packed
-//    difference fma(b, MINUS_ONE, a) with ONE / MINUS_ONE kernel arguments the assembler cannot fold
-//    (x*1 is exact, so the FMA rounds exactly once, on the sum); products are mul.rn.f32x2, which has
-//    nothing to fuse with.  tests/test_build_and_abi.py holds the SASS to that: no scalar FFMA, no FADD2, and
-//    as many FFMA2 / FMUL2 as the PTX has fma.rn.f32x2 / mul.rn.f32x2.
-//  * One instruction stream of ~30 KB for the whole granule loop (one IMDCT-36 body for both channels, one
+//  * CHANNEL PAIRS.  Every value on the path exists once per channel, so lane data is held as float2
+//    (ch0, ch1): one body of code serves both channels.  Hopper has no packed FP32 arithmetic, so each pair
+//    operation is two scalar __fmul_rn / __fadd_rn / __fsub_rn, which the compiler never contracts into an FMA
+//    (bit-exactness); tests/test_build_and_abi.py holds the SASS to that: no FFMA anywhere.
+//  * One instruction stream for the whole granule loop (one IMDCT-36 body for both channels, one
 //    DCT-32 body, one window body), so twelve warps in different phases still fit the instruction caches.
 //
 // A share that starts inside a run recomputes a 2-granule halo (hybrid of g-2 for its overlap, hybrid + DCT
@@ -86,27 +82,12 @@ constexpr int kPitch = 33;            // float2 per XT row: 32 sub-bands + one a
 constexpr uint32_t kRowBytes = kPitch * 8;
 constexpr float kFrac1Sqrt2 = 0.707106781186547524400844362104849039f;
 
-// ---- packed f32x2 arithmetic (see the header: no add.f32x2 / sub.f32x2 ever) ---------------------  // PHASE: packed ops
+// ---- channel-pair arithmetic: one correctly rounded scalar operation per channel, never contracted ----  // PHASE: pair ops
 struct Ops {
-    float one, mone; // 1.0f and -1.0f from the kernel arguments: opaque to ptxas
-    __device__ __forceinline__ f2 mul(f2 a, f2 b) const {
-        f2 r;
-        asm("{.reg .b64 ra, rb, rc; mov.b64 ra, {%2,%3}; mov.b64 rb, {%4,%5}; mul.rn.f32x2 rc, ra, rb; mov.b64 {%0,%1}, rc;}"
-            : "=f"(r.x), "=f"(r.y)
-            : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-        return r;
-    }
+    __device__ __forceinline__ f2 mul(f2 a, f2 b) const { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
     __device__ __forceinline__ f2 mul(f2 a, float s) const { return mul(a, make_float2(s, s)); }
-    __device__ __forceinline__ f2 fma(f2 a, f2 b, f2 c) const {
-        f2 r;
-        asm("{.reg .b64 ra, rb, rc, rd; mov.b64 ra, {%2,%3}; mov.b64 rb, {%4,%5}; mov.b64 rc, {%6,%7}; fma.rn.f32x2 rd, ra, rb, rc; "
-            "mov.b64 {%0,%1}, rd;}"
-            : "=f"(r.x), "=f"(r.y)
-            : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y), "f"(c.x), "f"(c.y));
-        return r;
-    }
-    __device__ __forceinline__ f2 add(f2 a, f2 b) const { return fma(a, make_float2(one, one), b); }   // a*1 + b
-    __device__ __forceinline__ f2 sub(f2 a, f2 b) const { return fma(b, make_float2(mone, mone), a); } // b*(-1) + a
+    __device__ __forceinline__ f2 add(f2 a, f2 b) const { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+    __device__ __forceinline__ f2 sub(f2 a, f2 b) const { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
 };
 
 struct WarpSmem {
@@ -234,9 +215,8 @@ __device__ __forceinline__ void imdct12x3(const Ops& o, const f2 (&x)[18], f2 (&
 // A sub-band in which one channel is long and the other short (independent block types outside joint stereo;
 // rare): both transforms, component-wise choice.  Kept out of line with its operands in local memory so that
 // its register needs do not shape the granule loop.
-__device__ __noinline__ void hybrid_mixed(float one, float mone, const f2* xin, int wsel0, int wsel1, int cat0, int cat1, f2* fout,
-                                          f2* sout) {
-    const Ops o{one, mone};
+__device__ __noinline__ void hybrid_mixed(const f2* xin, int wsel0, int wsel1, int cat0, int cat1, f2* fout, f2* sout) {
+    const Ops o{};
     f2 x[18], fa[18], sa[18], fb[18], sb[18];
 #pragma unroll
     for (int i = 0; i < 18; ++i) x[i] = xin[i];
@@ -409,7 +389,7 @@ __global__ void __launch_bounds__(NW * 32, (NW <= 6 ? 12 / NW : 1)) mp3v2_synth_
     };
     WarpSmem& ws = sm.w[warp];
     const Mp3Tables* __restrict__ tab = a.tab;
-    const Ops o{a.one, a.mone};
+    const Ops o{};
 
     if (lane == 0) {
         mbar_init(&ws.bar, 1);
@@ -843,7 +823,7 @@ __global__ void __launch_bounds__(NW * 32, (NW <= 6 ? 12 / NW : 1)) mp3v2_synth_
                 f2 lx[18], lf[18], ls[18];
 #pragma unroll
                 for (int i = 0; i < 18; ++i) lx[i] = x[i];
-                hybrid_mixed(a.one, a.mone, lx, wsel0, wsel1, cat[0], cat[1], lf, ls);
+                hybrid_mixed(lx, wsel0, wsel1, cat[0], cat[1], lf, ls);
 #pragma unroll
                 for (int i = 0; i < 18; ++i) {
                     first[i] = lf[i];

@@ -139,7 +139,14 @@ cudaError_t dequant_launch(const int16_t* q, float* spectra, size_t n, const flo
     if (n == 0) return cudaSuccess;
     if (n % 8) return cudaErrorInvalidValue;
     const size_t n8 = n / 8;
-    const unsigned grid = (unsigned)((n8 + 255) / 256 < 148u * 16u ? (n8 + 255) / 256 : 148u * 16u);
+    static int sms = 0;
+    if (!sms) {
+        int dev = 0;
+        cudaGetDevice(&dev);
+        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    }
+    const size_t cap = (size_t)sms * 16;
+    const unsigned grid = (unsigned)((n8 + 255) / 256 < cap ? (n8 + 255) / 256 : cap);
     dequant_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const int4*>(q), reinterpret_cast<float4*>(spectra), n8, pow43);
     return cudaGetLastError();
 }

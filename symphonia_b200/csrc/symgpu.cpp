@@ -258,9 +258,8 @@ symgpu_status build_plan(symgpu_ctx* ctx, const symgpu_mp3_run* runs, uint32_t n
                          bool whole_batch = true) {
     cudaError_t ce = cudaSuccess;
     // Which kernel: the second generation (one warp per share, state in registers) wins where runs are short -- the serving
-    // shape, a frame or two per stream: 143 us against 219 us for 8192 one-frame streams -- the first generation (CTA-wide
-    // tiles of 16 consecutive granules, one halo per CTA chain) with the packed window phase where runs are long: 128 us
-    // against 135 us for 64 streams x 128 frames (profiles/r02_mp3_variants_log.txt).
+    // shape, a frame or two per stream -- the first generation (CTA-wide tiles of 16 consecutive granules, one halo per CTA
+    // chain) where runs are long (64 streams x 128 frames).
     bool v2 = ctx->mp3_kernel_mode == 2;
     if (ctx->mp3_kernel_mode == 0) {
         uint64_t gran = 0, n = 0;
@@ -292,13 +291,13 @@ cudaError_t launch_plan(symgpu_ctx* ctx, const Mp3Tile* d_plan, int hdr, int n_t
         if (ce != cudaSuccess) return ce;
         const int n_shares = n_ctas; // the v2 plan counts shares
         const Mp3V2Args a{units, spectra, pcm, reinterpret_cast<const uint32_t*>(d_plan), d_plan + hdr, n_tiles, n_shares,
-                          ctx->d_mp3_states, ctx->d_mp3_gen, ctx->d_mp3_gen + ctx->n_mp3_streams, ctx->d_mp3_tab, 1.0f, -1.0f};
+                          ctx->d_mp3_states, ctx->d_mp3_gen, ctx->d_mp3_gen + ctx->n_mp3_streams, ctx->d_mp3_tab};
         // many short run segments per share = the serving shape (a frame or two per stream)
         const bool short_runs = n_tiles >= 2 * n_shares;
         return mp3v2_launch(a, std::min(n_sm * mp3v2_ctas_per_sm(), n_shares), stream, short_runs);
     }
     const Mp3Args a{units, spectra, pcm, reinterpret_cast<const uint32_t*>(d_plan), d_plan + hdr, n_tiles, n_ctas, multi ? 1 : 0,
-                    ctx->d_mp3_states, ctx->d_mp3_gen, ctx->d_mp3_gen + ctx->n_mp3_streams, ctx->d_mp3_tab, 1.0f};
+                    ctx->d_mp3_states, ctx->d_mp3_gen, ctx->d_mp3_gen + ctx->n_mp3_streams, ctx->d_mp3_tab};
     return mp3_launch(a, stream);
 }
 
@@ -344,9 +343,8 @@ symgpu_status ensure_plan(symgpu_ctx* ctx, const symgpu_mp3_run* runs, uint32_t 
 
 
 // ---- NUMA placement ------------------------------------------------------------------------------------------------
-// A B200 node has its GPUs behind two sockets; a rank whose thread (and therefore its first-touched pinned buffers)
-// sits on the far socket pays for every H2D / D2H byte twice on the inter-socket link, and eight ranks doing so at once
-// is what bent round 1's end-to-end scaling (0.62 at 8 GPUs).  Parses "0-3,8,10-11" style lists.
+// An eight-GPU node has its GPUs behind two sockets; a rank whose thread (and therefore its first-touched pinned buffers)
+// sits on the far socket pays for every H2D / D2H byte twice on the inter-socket link.  Parses "0-3,8,10-11" style lists.
 static bool parse_cpulist(const char* text, cpu_set_t* set) {
     CPU_ZERO(set);
     int n = 0;
@@ -498,8 +496,9 @@ symgpu_status symgpu_ctx_create(int device, symgpu_ctx** out) {
         return SYMGPU_ERR_CUDA;
     }
     cudaDeviceProp prop{};
-    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess || prop.major < 10) {
-        std::fprintf(stderr, "symgpu: device %d is not sm_100-class; kernels are built for sm_100a only\n", device);
+    // sm_90a code runs on compute capability 9.0 only (the "a" features do not carry forward to later architectures)
+    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess || prop.major != 9 || prop.minor != 0) {
+        std::fprintf(stderr, "symgpu: device %d is not sm_90 (H100-class); kernels are built for sm_90a only\n", device);
         return SYMGPU_ERR_UNSUPPORTED;
     }
     symgpu_ctx* ctx = new (std::nothrow) symgpu_ctx();
@@ -520,13 +519,9 @@ symgpu_status symgpu_ctx_create(int device, symgpu_ctx** out) {
         const int v = std::atoi(env);
         if (v >= 1 && v <= symgpu_ctx::kMaxSlices) ctx->n_slices = v;
     }
-    // SYMGPU_MP3_KERNEL=v1 selects the first-generation Layer III kernel (mp3_kernel.cu), kept for comparison
-    // SYMGPU_MP3_KERNEL = auto (default) | v1 (first generation, scalar window) | v1p (first generation, packed window) | v2
-    mp3_v1_set_packed_window(true);
-    if (const char* env = std::getenv("SYMGPU_MP3_KERNEL")) {
-        ctx->mp3_kernel_mode = std::strncmp(env, "v1", 2) == 0 ? 1 : std::strcmp(env, "v2") == 0 ? 2 : 0;
-        mp3_v1_set_packed_window(std::strcmp(env, "v1") != 0);
-    }
+    // SYMGPU_MP3_KERNEL = auto (default) | v1 (first generation, mp3_kernel.cu) | v2 (second generation, mp3_kernel_v2.cu)
+    if (const char* env = std::getenv("SYMGPU_MP3_KERNEL"))
+        ctx->mp3_kernel_mode = std::strcmp(env, "v1") == 0 ? 1 : std::strcmp(env, "v2") == 0 ? 2 : 0;
     if (const char* env = std::getenv("SYMGPU_MP3_V2_VARIANT")) { // "<warps>:<mode>", experiments
         int nw = 0, mode = 0;
         if (std::sscanf(env, "%d:%d", &nw, &mode) != 2 || !mp3v2_set_variant(nw, mode)) {
@@ -654,8 +649,8 @@ constexpr uint32_t kPipelineMinFrames = 512; // smaller host batches: no slice p
 static inline float* d_spec_base(char* stage_base) { return reinterpret_cast<float*>(stage_base); }
 
 
-// symgpu_mp3_units_check over the runs in four parts on as many threads (the 64-byte descriptors of 8192 frames take ~190 us on
-// one thread, which is 9 % of an end-to-end step).
+// symgpu_mp3_units_check over the runs in four parts on as many threads (the 64-byte descriptors of 8192 frames are a noticeable
+// share of an end-to-end step on one thread).
 static symgpu_status units_check_mt(const symgpu_mp3_gc* units, const symgpu_mp3_run* runs, uint32_t n_runs, uint32_t n_frames) {
     if (n_frames < 1024 || n_runs < 4) return symgpu_mp3_units_check(units, runs, n_runs, n_frames);
     symgpu_status chk[4] = {SYMGPU_OK, SYMGPU_OK, SYMGPU_OK, SYMGPU_OK};
@@ -683,8 +678,7 @@ static symgpu_status mp3_synth_host_impl(symgpu_ctx* ctx, const symgpu_mp3_gc* u
     const size_t sample_bytes = format < 0 ? sizeof(float) : symgpu_sample_bytes(format);
     if (sample_bytes == 0) return SYMGPU_ERR_ARG;
     if (n_frames == 0) return SYMGPU_OK;
-    // The runs' geometry is checked now (cheap); the 64-byte descriptors of every granule-channel (~200 us of host time
-    // for 8192 frames) are checked while the first H2D copies are already on their way.
+    // The runs' geometry is checked now (cheap); the 64-byte descriptors of every granule-channel are checked while the first H2D copies are already on their way.
     for (uint32_t r = 0; r < n_runs; ++r) {
         const int gpf = runs[r].granules_per_frame ? runs[r].granules_per_frame : 2;
         const int n_ch = runs[r].channels ? runs[r].channels : 2;
@@ -699,8 +693,8 @@ static symgpu_status mp3_synth_host_impl(symgpu_ctx* ctx, const symgpu_mp3_gc* u
     // addressing), the synthesis kernel takes them as they are: its TMA bulk copies pull the next granule's spectra across PCIe
     // one granule (or tile) ahead of the arithmetic and its coalesced 128-byte PCM stores go straight to host memory.  H2D
     // traffic, arithmetic and D2H traffic overlap inside ONE launch -- no staging copy, no slice pipeline, no copy-engine
-    // scheduling between them.  Opt-in (SYMGPU_ZERO_COPY=2): measured 2.36 ms per 8192-frame step against 2.20 ms for the
-    // staged pipeline below (profiles/r02l_*), bit-identical output (tests/test_mp3_parity_gpu.py).
+    // scheduling between them.  Opt-in (SYMGPU_ZERO_COPY=2); bit-identical output to the staged pipeline below
+    // (tests/test_mp3_parity_gpu.py).
     // Small batches (a single packet is the extreme: config 1) take this path by default when the buffers allow it: one launch and
     // one synchronisation instead of two or three copy set-ups around them (SYMGPU_ZERO_COPY=0 switches it off).
     const bool small_auto = ctx->zero_copy_small && n_frames < kPipelineMinFrames;
@@ -719,7 +713,7 @@ static symgpu_status mp3_synth_host_impl(symgpu_ctx* ctx, const symgpu_mp3_gc* u
         void* d_s = d_u ? mapped(spectra) : nullptr;
         void* d_o = d_s ? mapped(out) : nullptr;
         if (d_o) {
-            // descriptors are checked before anything runs on them (four host threads: ~50 us for 8192 frames)
+            // descriptors are checked before anything runs on them (four host threads)
             {
                 const symgpu_status c = units_check_mt(units, runs, n_runs, n_frames);
                 if (c != SYMGPU_OK) return c;
@@ -821,7 +815,7 @@ static symgpu_status mp3_synth_host_impl(symgpu_ctx* ctx, const symgpu_mp3_gc* u
     uint32_t r = 0;
     // Both PCIe directions carry about the same bytes, so the run is as long as the D2H chain, which cannot start
     // before the first slice is in and cannot end before the last slice is out: the slices taper at both ends
-    // (weights 0.25, 0.5, 1, ..., 1, 0.5, 0.25); every extra slice costs two copy set-ups (~20 us each).
+    // (weights 0.25, 0.5, 1, ..., 1, 0.5, 0.25); every extra slice costs two copy set-ups.
     double w_total = 0.0, w_acc = 0.0;
     auto weight = [&](int i) {
         const int edge = std::min(i, n_slices - 1 - i);
@@ -843,7 +837,7 @@ static symgpu_status mp3_synth_host_impl(symgpu_ctx* ctx, const symgpu_mp3_gc* u
     }
     // 1. the H2D copies of the first `ahead` slices are queued at once, so that the copy engine has work while the host checks
     //    the descriptors and plans the launches.  The rest is queued slice by slice BEHIND the D2H copy of an earlier slice:
-    //    queueing every H2D copy up front was measured to serialise the two directions (2.9 ms instead of 2.2 ms per step).
+    //    queueing every H2D copy up front serialises the two directions.
     // (with the output written by the kernels there are no D2H copies to interleave with: everything is queued at once)
     const size_t ahead = out_mapped ? slices.size() : std::min<size_t>(slices.size(), (size_t)std::max(1, ctx->h2d_ahead));
     // SYMGPU_E2E_TRACE=1: timing events around every copy and launch of the pipeline, printed after the call (diagnostics only)

@@ -3,7 +3,7 @@
 //
 // The reference's decoders are one object per stream, one decode() call per packet (codecs/audio.rs:251-298), made by
 // the registry (registry.rs:260-269); a server runs hundreds of them on as many threads.  One launch per packet wastes
-// the GPU (a 148-SM kernel for one frame), so the context gathers what the decoders of all threads have submitted into
+// the GPU (a kernel sized for every SM, for one frame), so the context gathers what the decoders of all threads have submitted into
 // ONE batch: a frame is copied into pinned staging memory under a mutex (submit), and the first thread that waits for a
 // ticket of the oldest unfinished batch closes it and runs it for everybody (wait) -- group commit: while that batch is
 // on the device the other threads keep submitting into the next one.  Batches run in order, so the frames of a stream are

@@ -1,4 +1,4 @@
-// Vorbis synthesis for sm_100a (codec-vorbis/src/lib.rs:250-315):
+// Vorbis synthesis for sm_90a (codec-vorbis/src/lib.rs:250-315):
 //   floor-1 curve (floor.rs:568-653, :776-825)  ->  inverse coupling (lib.rs:252-278)
 //   -> floor * residue (lib.rs:282-292) -> IMDCT -> power-sine window + overlap-add (dsp.rs:68-145)
 //
@@ -76,7 +76,7 @@ __device__ __forceinline__ void floor1_build(const symgpu_vorbis_floor1& s, cons
     const int range = mult == 1 ? 256 : mult == 2 ? 128 : mult == 3 ? 86 : 64;
     int16_t* final_y = out.final_y;
     // my posts: i = lane, lane + 32, lane + 64  (ordering the posts by level on the host, so that a level touches fewer of the
-    // three slots, was measured: 139.5 -> 138.9 us, not worth the table)
+    // three slots, gains too little to be worth the table)
     int px[3], plo[3], phi[3], pxlo[3], pxhi[3], pval[3], plvl[3];
 #pragma unroll
     for (int k = 0; k < 3; ++k) {

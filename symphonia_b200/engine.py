@@ -31,7 +31,7 @@ class Engine:
         st = self._lib.symgpu_ctx_create(int(device), ctypes.byref(self._ctx))
         if st != 0:
             self._ctx = None
-            raise SymgpuError(st, "symgpu_ctx_create failed: a B200-class CUDA device is required; "
+            raise SymgpuError(st, "symgpu_ctx_create failed: an H100-class (sm_90) CUDA device is required; "
                                   "there is no CPU fallback")
         self.device = int(device)
 

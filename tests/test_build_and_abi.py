@@ -42,41 +42,23 @@ def _sass_by_function(lib_path):
 
 
 def test_no_fused_multiply_add_in_sass():
-    """Bit-exact parity needs every product and every sum rounded on its own.  Scalar code: -fmad=false, so no FFMA /
-    DFMA anywhere.  Packed f32x2 code (mp3_kernel_v2.cu): ptxas contracts mul.f32x2 + add.f32x2 even with --fmad=false,
-    so that file writes no packed add / sub at all; its sums are fma(a, ONE, b) with ONE a kernel argument.  Held here:
-    no FADD2 in the SASS, no add / sub .f32x2 in the PTX, and as many FFMA2 / FMUL2 as the PTX has
-    fma.rn.f32x2 / mul.rn.f32x2 at least -- a contraction would lower the FMUL2 count."""
+    """Bit-exact parity needs every product and every sum rounded on its own: -fmad=false, and the channel-pair
+    arithmetic of the MP3 kernels is written as separate __fmul_rn / __fadd_rn / __fsub_rn per channel.  Held here:
+    the library is sm_90a code only, with no FFMA / DFMA (scalar or packed) in any kernel, and the MP3 kernels keep
+    their products and sums as FMUL / FADD."""
     import symphonia_b200 as sb
     if not shutil.which("cuobjdump"):
         pytest.skip("cuobjdump not available")
     sass, funcs = _sass_by_function(sb.lib_path())
-    assert "sm_100a" in sass or "SM100" in sass.upper()
-    hits = re.findall(r"\b(FFMA|DFMA)\b", sass)
+    archs = set(re.findall(r"arch = (sm_\w+)", sass))
+    assert archs == {"sm_90a"}, f"kernels built for {sorted(archs)}, not sm_90a only"
+    hits = re.findall(r"\b(FFMA|DFMA|FFMA2)\b", sass)
     assert not hits, f"{len(hits)} fused multiply-adds in the kernels: bit-exact parity would break"
-    assert not re.findall(r"\bFADD2\b", sass), "packed adds are contracted by ptxas: the kernels must not contain any"
     assert re.search(r"\bFMUL\b", sass) and re.search(r"\bFADD\b", sass)
-    packed = {k: v for k, v in funcs.items() if re.search(r"\bFFMA2\b", v)}
-    # the second-generation kernel, its out-of-line mixed-block helper, and the window phase of the first-generation kernel
-    assert packed and all("mp3v2" in k or "hybrid_mixed" in k or "mp3_synth_kernel" in k for k in packed), \
-        f"FFMA2 outside the packed MP3 kernels: {list(packed)}"
-    ptx_path = os.path.join(os.path.dirname(sb.lib_path()), "csrc", "mp3_kernel_v2.ptx")
-    assert os.path.exists(ptx_path), "the build writes the PTX of the packed kernel next to its source"
-    ptx = open(ptx_path).read()
-    assert not re.findall(r"\b(add|sub)(\.\w+)*\.f32x2\b", ptx), "a packed add / sub would be contracted into FFMA2"
-    n_fma_ptx = len(re.findall(r"\bfma\.rn\.f32x2\b", ptx))
-    n_mul_ptx = len(re.findall(r"\bmul\.rn\.f32x2\b", ptx))
-    v2_funcs = {k: v for k, v in funcs.items() if "mp3v2" in k or "hybrid_mixed" in k}
-    n_fma_sass = sum(len(re.findall(r"\bFFMA2\b", v)) for v in v2_funcs.values())
-    n_mul_sass = sum(len(re.findall(r"\bFMUL2\b", v)) for v in v2_funcs.values())
-    # first-generation kernel, packed window: a product and a sum per tap pair, nothing contracted away
-    for k, v in funcs.items():
-        if "mp3_synth_kernel" in k and re.search(r"\bFFMA2\b", v):
-            assert len(re.findall(r"\bFMUL2\b", v)) >= len(re.findall(r"\bFFMA2\b", v)) >= 256, k
-    assert n_fma_ptx > 500 and n_mul_ptx > 500
-    # ptxas may duplicate a block (more instructions than the PTX), never drop a product
-    assert n_mul_sass >= n_mul_ptx, f"FMUL2 {n_mul_sass} < mul.rn.f32x2 {n_mul_ptx}: a product was contracted away"
-    assert n_fma_sass >= n_fma_ptx, f"FFMA2 {n_fma_sass} < fma.rn.f32x2 {n_fma_ptx}"
+    mp3 = {k: v for k, v in funcs.items() if "mp3v2" in k or "hybrid_mixed" in k or "mp3_synth_kernel" in k}
+    assert mp3, "the MP3 synthesis kernels are missing from the library"
+    for k, v in mp3.items():
+        assert re.search(r"\bFMUL\b", v) and re.search(r"\bFADD\b", v), k
 
 
 def test_tables_match_oracle(oracle):

@@ -1,11 +1,6 @@
 """GPU parity of the FLAC integer restoration (SURVEY §8f N4): identical to the oracle, and -- the property the
-format exists for -- identical to the PCM the residuals were computed from.
-
-OPT-IN (SYMGPU_TEST_FLAC=1).  Status at the end of round 1: the one GPU run of this file found every sub-frame type
-bit-exact (CONSTANT, VERBATIM, FIXED orders 0 / 2 / 3 / 4, LPC orders 1..32, all channel assignments, wasted bits)
-except FIXED order 1, whose coefficient set-up was miscompiled (see flac_kernel.cu); the set-up was rewritten, but
-the round's GPU budget was spent before the re-run, so the kernel is not claimed as verified and this file does
-not run by default."""
+format exists for -- identical to the PCM the residuals were computed from.  Covers every sub-frame type (CONSTANT,
+VERBATIM, FIXED orders 0..4, LPC orders 1..32), all channel assignments and wasted bits."""
 import os
 
 import numpy as np

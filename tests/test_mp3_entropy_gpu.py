@@ -1,10 +1,7 @@
 """The device front-end (SURVEY §8f N1 on the GPU): `symgpu_mp3_decode_files_host` -- side-information pass on the CPU,
 Huffman decode of every granule-channel by one thread each, then the synthesis kernel -- against the oracle's synthesis
-of what the CPU front-end decodes from the same bytes.
-
-OPT-IN (SYMGPU_TEST_ENTROPY=1): the kernel was written after the round's GPU budget was spent; it compiles for sm_100a
-and runs the same decode functions the CPU tests cover (symphonia_b200/csrc/mp3_entropy.h), but it has not run on a
-device yet, so it is not part of the default GPU suite."""
+of what the CPU front-end decodes from the same bytes.  The kernel runs the same decode
+functions the CPU tests cover (symphonia_b200/csrc/mp3_entropy.h)."""
 import os
 
 import numpy as np

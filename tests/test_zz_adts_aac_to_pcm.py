@@ -1,7 +1,7 @@
 """ADTS file bytes -> frames -> raw_data_blocks -> AAC-LC entropy front-end -> synthesis -> interleaved samples
 (`symphonia_b200.decode.adts_aac_plan` / `decode_adts_aac`).  The CPU test runs everything up to the launch, renders the plan with
 the synthesis and output-stage oracles and compares with an expectation built from the stream WRITER's ground truth; the GPU test
-(opt-in until it has run on a B200 once: SYMGPU_TEST_AAC_CHAIN=1, tools/next_round_gpu.sh) compares `decode_adts_aac` with the
+compares `decode_adts_aac` with the
 rendered plan byte for byte."""
 import os
 

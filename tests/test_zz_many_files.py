@@ -1,7 +1,7 @@
 """Many files at once (`symphonia_b200.decode.plan_files` / `decode_files`): MPEG audio (Layers I-III), ADTS AAC-LC and Ogg Vorbis files
 planned on host threads and merged into ONE synthesis batch per codec, every file a stream of its own.  CPU test: the merged
 batches rendered by the synthesis and output oracles equal every file rendered alone (index re-basing of TNS records, floor tables,
-runs, spans; residues re-padded to a common slot).  GPU test (opt-in until it has run on a B200 once: SYMGPU_TEST_MANY_FILES=1):
+runs, spans; residues re-padded to a common slot).  GPU test:
 `decode_files` equals the same rendering byte for byte."""
 import os
 

@@ -1,7 +1,7 @@
 """Vorbis-in-Ogg file bytes -> pages -> packets -> headers -> entropy front-end -> synthesis -> trimmed interleaved samples
 (`symphonia_b200.decode.ogg_vorbis_plan` / `decode_ogg_vorbis`).  The CPU test runs everything up to the launch, renders the plan
 with the synthesis and output-stage oracles and compares with an expectation built from the stream WRITER's ground truth (which
-never saw a bit reader); the GPU test (opt-in until it has run on a B200 once: SYMGPU_TEST_VORBIS_CHAIN=1, tools/next_round_gpu.sh)
+never saw a bit reader); the GPU test
 compares `decode_ogg_vorbis` with the rendered plan byte for byte."""
 import os
 

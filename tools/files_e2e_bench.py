@@ -3,8 +3,7 @@
 of MP3, ADTS AAC-LC and Ogg Vorbis files through `symphonia_b200.decode.decode_files` -- front-ends on host threads, one synthesis
 launch per codec, output stage per file -- host wall clock around the whole call, and the plan (CPU) share on its own.
 
-NOT part of the driver contract (bench.py is); written in round 1 after the GPU budget was spent, for the first GPU call of round 2
-(`tools/next_round_gpu.sh`).  `--plan-only` runs the CPU half without a GPU.  One JSON line."""
+NOT part of the headline measurement (bench.py is).  `--plan-only` runs the CPU half without a GPU.  One JSON line."""
 import argparse
 import json
 import os

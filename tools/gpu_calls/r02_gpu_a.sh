@@ -10,8 +10,6 @@ nvidia-smi --query-gpu=name,clocks.sm,clocks.max.sm,power.draw --format=csv > $o
 timeout 900 python -m pytest tests/test_mp3_parity_gpu.py -m gpu -x -q 2>&1 | tail -25 | tee $out/${tag}_pytest_mp3.txt
 # 2. the whole GPU suite, no -x
 timeout 1500 python -m pytest tests -m gpu -q 2>&1 | tail -60 | tee $out/${tag}_pytest_gpu.txt
-# 3. packed FP32 issue rates
-nvcc -gencode arch=compute_100a,code=sm_100a -O3 -fmad=false -o /tmp/fp32_issue tools/microbench/fp32_issue.cu 2>/dev/null && /tmp/fp32_issue | tee $out/${tag}_fp32_issue.txt
 # 4. A/B bench
 timeout 400 python bench.py --steps 20 --warmup 5 > $out/${tag}_bench_v2.json 2>$out/${tag}_bench_v2.err
 SYMGPU_MP3_KERNEL=v1 timeout 400 python bench.py --steps 20 --warmup 5 --no-cpu-baseline > $out/${tag}_bench_v1.json 2>$out/${tag}_bench_v1.err

@@ -18,7 +18,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 def sass_lines(so, stem, kernel):
     tmp = tempfile.mkdtemp()
     subprocess.check_call(["cuobjdump", "-xelf", "all", os.path.abspath(so)], cwd=tmp, stdout=subprocess.DEVNULL)
-    sass = subprocess.run(["nvdisasm", "-g", "-c", os.path.join(tmp, stem + ".sm_100a.cubin")], capture_output=True, text=True).stdout
+    sass = subprocess.run(["nvdisasm", "-g", "-c", os.path.join(tmp, stem + ".sm_90a.cubin")], capture_output=True, text=True).stdout
     out, cur, infn = [], 0, False
     for ln in sass.splitlines():
         if ln.strip().startswith(".section") and ".text." in ln:

@@ -14,7 +14,7 @@ sys.path.insert(0, ROOT)
 import symphonia_b200 as sb  # noqa: E402
 from symphonia_b200 import workloads  # noqa: E402
 
-variants = sys.argv[1:] or ["v1", "v1p", "auto", "12:33", "12:81"]
+variants = sys.argv[1:] or ["v1", "auto", "12:33", "12:81"]
 dev = torch.device("cuda", 0)
 S, F = 64, 128
 shapes = {"bench": (S, F), "serving": (8192, 1)}
@@ -24,7 +24,7 @@ ref = {}
 for shape, (s_, f_) in shapes.items():
     units, spectra, runs = workloads.mp3_batch(s_, f_, seed=workloads.SEED_BASE + 1)
     for v in variants:
-        if v in ("v1", "v1p", "auto"):
+        if v in ("v1", "auto"):
             os.environ["SYMGPU_MP3_KERNEL"] = v
         else:
             os.environ["SYMGPU_MP3_KERNEL"] = "v2"

@@ -19,7 +19,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 def line_of_each_instruction(so, variant=None):
     tmp = tempfile.mkdtemp()
     subprocess.check_call(["cuobjdump", "-xelf", "all", os.path.abspath(so)], cwd=tmp, stdout=subprocess.DEVNULL)
-    sass = subprocess.run(["nvdisasm", "-g", "-c", os.path.join(tmp, "mp3_kernel.sm_100a.cubin")],
+    sass = subprocess.run(["nvdisasm", "-g", "-c", os.path.join(tmp, "mp3_kernel.sm_90a.cubin")],
                           capture_output=True, text=True).stdout
     out, cur, infn = [], 0, False
     for ln in sass.splitlines():
@@ -52,11 +52,9 @@ def main():
     rows = list(csv.reader(io.StringIO(txt)))
     # the kernel has a single-tile-group and a multi-tile-group instantiation (last template argument)
     name = next((r[1] for r in rows if r and r[0] == "Kernel Name"), "")
-    # "mp3_synth_kernel<16, 16, 0, 1>" -> the mangled template argument list ILi16ELi16ELb0ELb1EE
+    # "mp3_synth_kernel<16, 16, 0>" -> the mangled template argument list ILi16ELi16ELb0EE
     targs = re.sub(r"\((int|bool)\)", "", re.search(r"<([^>]*)>", name).group(1)).replace(" ", "").split(",")
     variant = "I" + "".join(f"Li{a}E" for a in targs[:2]) + "".join("Lb1E" if a in ("1", "true") else "Lb0E" for a in targs[2:]) + "E"
-    if len(targs) == 3:
-        variant = variant[:-1] + "Lb0EE"  # the defaulted PK argument
     lines = line_of_each_instruction(so, variant)
     hdr_i = next(i for i, r in enumerate(rows) if r and r[0] == "Address")
     hdr = rows[hdr_i]
