@@ -22,9 +22,13 @@
  *
  * Threading (AudioDecoder: Send + Sync, symphonia-core/src/codecs/audio.rs:251): a context owns
  * one CUDA stream; calls on one context must be serialised by the caller (the trait's &mut self
- * already guarantees that per decoder).  Different contexts may be used concurrently.  The exception is
- * symgpu_mp3_submit / symgpu_mp3_submit_quantized / symgpu_mp3_wait: any number of decoder threads may call
- * them on ONE context at the same time, and the context gathers their frames into shared launches.
+ * already guarantees that per decoder).  Different contexts may be used concurrently.  The exceptions are the
+ * per-packet submission calls and the stream-slot calls a decoder makes while others decode:
+ *   symgpu_{mp3,aac,mpa12,vorbis}_submit, symgpu_mp3_submit_quantized, symgpu_{mp3,aac,mpa12,vorbis}_wait,
+ *   symgpu_{mp3,aac,vorbis}_stream_reset, symgpu_vorbis_stream_configure, symgpu_async_stats, symgpu_mp3_async_stats.
+ * Any number of decoder threads may call these on ONE context at the same time, of any codec: the context
+ * gathers their packets into shared launches and serialises every launch and slot update on one lock.  They
+ * must not run concurrently with the other entry points of the same context (allocation, batch calls).
  */
 #ifndef SYMGPU_H
 #define SYMGPU_H
@@ -180,8 +184,8 @@ symgpu_status symgpu_mp3_synth_dev(symgpu_ctx* ctx, const symgpu_mp3_gc* units,
 /* ---- MP3: asynchronous, thread-safe submission (many single-stream decoders sharing one context) ------------------- *
  * The reference creates one decoder per stream (registry.rs:260-269) and calls decode() once per packet
  * (codecs/audio.rs:251-298); a server runs many of them on as many threads.  These three entry points may be called
- * concurrently from any number of threads on ONE context (every other entry point of a context still wants one caller at
- * a time, and must not run concurrently with these).  submit copies one frame into the context's pinned staging batch
+ * concurrently from any number of threads on ONE context, together with the other thread-safe calls of the list at the top of
+ * this file (every other entry point of a context still wants one caller at a time, and must not run concurrently with these).  submit copies one frame into the context's pinned staging batch
  * and returns a ticket; wait returns that frame's PCM.  The first thread that waits for a ticket of the oldest
  * unfinished batch closes the batch and runs it -- one copy in, ONE launch, one copy out -- for every thread that has a
  * frame in it; the others sleep until it is done, while new submissions gather in the next batch.  Frames of a stream
@@ -202,6 +206,20 @@ symgpu_status symgpu_mp3_submit_quantized(symgpu_ctx* ctx, uint32_t stream, cons
 symgpu_status symgpu_mp3_wait(symgpu_ctx* ctx, symgpu_ticket ticket, float* pcm);
 /* Launch batches run so far through submit / wait and the frames they held (frames / batches = achieved batching). */
 void symgpu_mp3_async_stats(const symgpu_ctx* ctx, uint64_t* batches, uint64_t* frames);
+/* The same for the queue of any codec (symgpu_mp3_async_stats = SYMGPU_CODEC_MP3).  Layer I and Layer II frames have
+ * queues of their own: a launch takes one time-slot count.  SYMGPU_ERR_ARG for a null context or an unknown codec. */
+typedef enum symgpu_codec {
+    SYMGPU_CODEC_MP3 = 0,    /* Layer III: symgpu_mp3_submit / _submit_quantized                  */
+    SYMGPU_CODEC_MP1 = 1,    /* Layer I:   symgpu_mpa12_submit with n_slots 12                     */
+    SYMGPU_CODEC_MP2 = 2,    /* Layer II:  symgpu_mpa12_submit with n_slots 36                     */
+    SYMGPU_CODEC_AAC = 3,    /* symgpu_aac_submit                                                  */
+    SYMGPU_CODEC_VORBIS = 4  /* symgpu_vorbis_submit                                               */
+} symgpu_codec;
+symgpu_status symgpu_async_stats(const symgpu_ctx* ctx, int codec, uint64_t* batches, uint64_t* frames);
+/* The submission calls of the other codecs (declared with their codec below) follow the same rules: a ticket belongs to
+ * the codec that issued it (its `reserved` field says which; pass tickets back unchanged), a malformed packet is refused
+ * at submission (SYMGPU_ERR_DECODE) and never enters a batch, a stream occurs at most once per batch, batches of a codec
+ * run in order, and a ticket redeemed twice, or by the wait call of another codec, is SYMGPU_ERR_ARG. */
 
 /* ---- AAC-LC filterbank --------------------------------------------------------------------- */
 
@@ -253,6 +271,12 @@ symgpu_status symgpu_aac_synth_host(symgpu_ctx* ctx, const symgpu_aac_unit* unit
 symgpu_status symgpu_aac_synth_dev(symgpu_ctx* ctx, const symgpu_aac_unit* units, const symgpu_aac_tns* tns,
                                    uint32_t n_tns, const float* coeffs, const symgpu_aac_run* runs,
                                    uint32_t n_runs, uint32_t n_frames, float* pcm);
+/* One frame of `stream` into the context's shared batch (thread-safe, see symgpu_mp3_submit): units [2], tns [n_tns] with
+ * the units' tns_first counted from the start of THIS `tns` array, coeffs [2][1024], channels 1 | 2 (0 means 2).  The units
+ * are checked with symgpu_aac_units_check.  wait: pcm [2][1024] of the ticket's frame. */
+symgpu_status symgpu_aac_submit(symgpu_ctx* ctx, uint32_t stream, const symgpu_aac_unit* units, const symgpu_aac_tns* tns,
+                                uint32_t n_tns, const float* coeffs, uint8_t channels, symgpu_ticket* ticket);
+symgpu_status symgpu_aac_wait(symgpu_ctx* ctx, symgpu_ticket ticket, float* pcm);
 
 /* ---- Vorbis synthesis ---------------------------------------------------------------------- */
 
@@ -314,6 +338,28 @@ symgpu_status symgpu_vorbis_synth_host(symgpu_ctx* ctx, const symgpu_vorbis_unit
 symgpu_status symgpu_vorbis_synth_dev(symgpu_ctx* ctx, const symgpu_vorbis_unit* units, const uint16_t* floor_y,
                                       const float* residue, const symgpu_vorbis_run* runs, uint32_t n_runs,
                                       uint32_t n_packets, uint32_t slot, float* pcm);
+
+/* ---- Vorbis stream slots configured one at a time, and thread-safe submission ------------------------------------- *
+ * streams_alloc reserves n_streams slots, none configured yet (it replaces whatever streams_set / floors_set registered;
+ * a later streams_set or floors_set drops the slots again).  Slot s owns floor setups [64 s, 64 s + 64): a Vorbis setup
+ * has at most 64 floors, and unit->floor is 16 bits with 0xffff for "unused", hence at most SYMGPU_VORBIS_MAX_SLOTS slots.
+ * configure checks the record as streams_set does and the floors with symgpu_vorbis_floors_check, writes them into the
+ * slot, zeroes the slot's overlap state and returns *floor_base = 64 * stream -- the floor_base to hand to
+ * symgpu_vorbis_fe_decode, so that unit->floor indexes the slot's own setups. */
+#define SYMGPU_VORBIS_SLOT_FLOORS 64
+#define SYMGPU_VORBIS_MAX_SLOTS 1023
+symgpu_status symgpu_vorbis_streams_alloc(symgpu_ctx* ctx, uint32_t n_streams);
+symgpu_status symgpu_vorbis_stream_configure(symgpu_ctx* ctx, uint32_t stream, const symgpu_vorbis_stream* config,
+                                             const symgpu_vorbis_floor1* floors, uint32_t n_floors, uint32_t* floor_base);
+/* One packet of a configured slot into the context's shared batch (thread-safe, see symgpu_mp3_submit): unit, floor_y [2][65],
+ * residue [2][slot] with slot >= the stream's blocksize_1 / 2.  Refused with SYMGPU_ERR_DECODE: a block flag, previous block
+ * flag or do_not_decode flag other than 0 / 1, or a used floor outside the slot's configured setups (or on a channel the
+ * stream does not have).  A batch's rows are as long as the largest blocksize_1 / 2 of the configured slots.
+ * wait: pcm [2][slot] with the `slot` given at submission, of which the first (prev_n + n) / 4 samples are the packet's
+ * output, zeros behind. */
+symgpu_status symgpu_vorbis_submit(symgpu_ctx* ctx, uint32_t stream, const symgpu_vorbis_unit* unit, const uint16_t* floor_y,
+                                   const float* residue, uint32_t slot, symgpu_ticket* ticket);
+symgpu_status symgpu_vorbis_wait(symgpu_ctx* ctx, symgpu_ticket ticket, float* pcm);
 
 /* ---- Vorbis with more than two channels / several coupling steps ------------------------------------------------------ *
  * The reference maps up to 8 channels (codec-vorbis/src/lib.rs:771-788) and applies every coupling step of the packet's
@@ -431,6 +477,12 @@ symgpu_status symgpu_mpa12_synth_host(symgpu_ctx* ctx, const float* subbands, co
                                       uint32_t n_frames, uint32_t n_slots, float* pcm);
 symgpu_status symgpu_mpa12_synth_dev(symgpu_ctx* ctx, const float* subbands, const symgpu_mpa12_run* runs, uint32_t n_runs,
                                      uint32_t n_frames, uint32_t n_slots, float* pcm);
+/* One frame of `stream` (a Layer III state slot) into the context's shared batch of its layer (thread-safe, see
+ * symgpu_mp3_submit): subbands [2][32][n_slots], n_slots 12 | 36, channels 1 | 2.  wait: pcm [2][1152], of which plane(ch)
+ * [0 .. 32 * n_slots) is the frame's output and the rest zero. */
+symgpu_status symgpu_mpa12_submit(symgpu_ctx* ctx, uint32_t stream, const float* subbands, uint32_t n_slots, uint8_t channels,
+                                  symgpu_ticket* ticket);
+symgpu_status symgpu_mpa12_wait(symgpu_ctx* ctx, symgpu_ticket ticket, float* pcm);
 
 /* ===================================================================================================
  * FLAC (SURVEY 8f N4): what FlacDecoder::decode_inner does after the Rice residuals are decoded --

@@ -121,12 +121,13 @@ class CodecRegistry {
     std::map<uint32_t, AudioDecoderFactory[3]> slots_;
 };
 
-// A context shared by GPU decoders (one CUDA stream).  Stream-state slots are handed out from a free list under a mutex.
-// MPEG Layer III decoders of ANY number of threads may share one context: their decode() goes through the thread-safe
-// symgpu_mp3_submit / symgpu_mp3_wait pair, which gathers the packets of all threads into shared launches.  The other decoders
-// (Layer I / II, AAC, Vorbis) still want one calling thread per context (codecs/audio.rs "Send + Sync": one call at a time).
+// A context shared by GPU decoders (one CUDA stream).  Stream-state slots are handed out from a free list under a mutex; every
+// decoder of the registry takes one, whatever its codec (a Vorbis decoder too: its slot holds the stream's configuration and
+// floor setups).  Every decoder of the registry may run on any thread: decode() goes through the thread-safe submit / wait pair
+// of its codec, which gathers the packets of all threads into shared launches, and reset() through the thread-safe slot resets.
 class GpuContext {
   public:
+    // max_streams: decoders open at once.  Vorbis decoders can use the first min(max_streams, SYMGPU_VORBIS_MAX_SLOTS) slots.
     static Result<std::shared_ptr<GpuContext>> create(int device, uint32_t max_streams) {
         symgpu_ctx* c = nullptr;
         symgpu_status st = symgpu_ctx_create(device, &c);
@@ -134,6 +135,7 @@ class GpuContext {
         std::shared_ptr<GpuContext> g(new GpuContext(c, max_streams, device));
         st = symgpu_mp3_streams_alloc(c, max_streams);
         if (st == SYMGPU_OK) st = symgpu_aac_streams_alloc(c, max_streams);
+        if (st == SYMGPU_OK) st = symgpu_vorbis_streams_alloc(c, std::min<uint32_t>(max_streams, SYMGPU_VORBIS_MAX_SLOTS));
         if (st != SYMGPU_OK) return {nullptr, map_status(st)};
         return {g, {}};
     }
@@ -263,9 +265,9 @@ class GpuMpaDecoder final : public AudioDecoder {
             if (!have_spec_) have_spec_ = true, spec_rate_ = info.sample_rate, spec_channels_ = info.channels;
             else if (spec_rate_ != info.sample_rate || spec_channels_ != info.channels)
                 return {{}, {ErrorKind::DecodeError, "mpa: invalid audio buffer signal spec for packet"}};
-            symgpu_mpa12_run run{};
-            run.stream = stream_, run.n_frames = 1, run.channels = info.channels;
-            st = symgpu_mpa12_synth_host(gpu_->raw(), sub_, &run, 1, 1, (uint32_t)n_slots, pcm_.data());
+            symgpu_ticket ticket;  // batched with the Layer I / II packets other decoders of this context have in flight
+            st = symgpu_mpa12_submit(gpu_->raw(), stream_, sub_, (uint32_t)n_slots, info.channels, &ticket);
+            if (st == SYMGPU_OK) st = symgpu_mpa12_wait(gpu_->raw(), ticket, pcm_.data());
             frames = 32 * (size_t)n_slots;
         }
         if (st != SYMGPU_OK) return {{}, map_status(st)};
@@ -348,9 +350,9 @@ class GpuAacDecoder final : public AudioDecoder {
         uint32_t n_tns = 0;
         symgpu_status st = symgpu_aac_fe_decode(fe_, packet.data, packet.len, 0, units, tns_, &n_tns, coeffs_.data());
         if (st != SYMGPU_OK) return {{}, map_status(st)};
-        symgpu_aac_run run{};
-        run.stream = stream_, run.first_frame = 0, run.n_frames = 1, run.channels = (uint8_t)params_.channels;
-        st = symgpu_aac_synth_host(gpu_->raw(), units, n_tns ? tns_ : nullptr, n_tns, coeffs_.data(), &run, 1, 1, pcm_.data());
+        symgpu_ticket ticket;  // batched with the AAC packets other decoders of this context have in flight
+        st = symgpu_aac_submit(gpu_->raw(), stream_, units, n_tns ? tns_ : nullptr, n_tns, coeffs_.data(), (uint8_t)params_.channels, &ticket);
+        if (st == SYMGPU_OK) st = symgpu_aac_wait(gpu_->raw(), ticket, pcm_.data());
         if (st != SYMGPU_OK) return {{}, map_status(st)};
         frames_ = 1024;  // the reference's AAC decoder trims nothing (mod.rs:231-255)
         return {last_decoded(), {}};
@@ -378,8 +380,8 @@ class GpuAacDecoder final : public AudioDecoder {
 
 // Vorbis decoder whose floor synthesis, inverse coupling, IMDCT and overlap-add run on the GPU (mirrors VorbisDecoder,
 // symphonia-codec-vorbis/src/lib.rs:48-420).  Extra data = the identification packet followed by the setup packet, as the Ogg
-// mapping hands them over (mappings/vorbis.rs:196-214).  The library registers Vorbis streams and floor tables per context, all
-// at once, so this decoder owns a context of its own on the shared context's device.
+// mapping hands them over (mappings/vorbis.rs:196-214).  The decoder takes a stream slot of the shared context and configures it
+// with the stream's block sizes and floor setups; its packets are batched with those of every other decoder of the context.
 class GpuVorbisDecoder final : public AudioDecoder {
   public:
     static Result<std::unique_ptr<AudioDecoder>> try_new(std::shared_ptr<GpuContext> gpu, const AudioCodecParameters& p,
@@ -389,29 +391,32 @@ class GpuVorbisDecoder final : public AudioDecoder {
         symgpu_vorbis_fe* fe = nullptr;
         symgpu_status st = symgpu_vorbis_fe_create(p.extra_data.data(), 30, p.extra_data.data() + 30, p.extra_data.size() - 30, &fe);
         if (st != SYMGPU_OK) return {nullptr, map_status(st)};
-        symgpu_vorbis_stream stream{};
-        std::vector<symgpu_vorbis_floor1> floors(64);
+        symgpu_vorbis_stream config{};
+        std::vector<symgpu_vorbis_floor1> floors(SYMGPU_VORBIS_SLOT_FLOORS);
         uint32_t n_floors = 0;
-        symgpu_vorbis_fe_config(fe, &stream, floors.data(), &n_floors);
-        symgpu_ctx* ctx = nullptr;
-        st = symgpu_ctx_create(gpu->device(), &ctx);
-        if (st == SYMGPU_OK) st = symgpu_vorbis_streams_set(ctx, &stream, 1);
-        if (st == SYMGPU_OK && n_floors) st = symgpu_vorbis_floors_set(ctx, floors.data(), n_floors);
-        if (st != SYMGPU_OK) {
+        symgpu_vorbis_fe_config(fe, &config, floors.data(), &n_floors);
+        const int slot = gpu->acquire_stream();
+        if (slot < 0) {
             symgpu_vorbis_fe_destroy(fe);
-            if (ctx) symgpu_ctx_destroy(ctx);
+            return {nullptr, {ErrorKind::LimitError, "symgpu: no free stream slot"}};
+        }
+        uint32_t floor_base = 0;
+        st = symgpu_vorbis_stream_configure(gpu->raw(), (uint32_t)slot, &config, floors.data(), n_floors, &floor_base);
+        if (st != SYMGPU_OK) {
+            gpu->release_stream(slot);
+            symgpu_vorbis_fe_destroy(fe);
             return {nullptr, map_status(st)};
         }
         AudioCodecParameters params = p;
-        params.channels = stream.channels;
-        return {std::unique_ptr<AudioDecoder>(new GpuVorbisDecoder(ctx, std::move(params), o, fe, stream)), {}};
+        params.channels = config.channels;
+        return {std::unique_ptr<AudioDecoder>(new GpuVorbisDecoder(std::move(gpu), std::move(params), o, fe, config, (uint32_t)slot, floor_base)), {}};
     }
     ~GpuVorbisDecoder() override {
+        gpu_->release_stream((int)stream_);
         symgpu_vorbis_fe_destroy(fe_);
-        symgpu_ctx_destroy(ctx_);
     }
     void reset() override {  // lib.rs:336-338 -> dsp.rs:26-32: overlap cleared, no previous block
-        symgpu_vorbis_stream_reset(ctx_, 0);
+        symgpu_vorbis_stream_reset(gpu_->raw(), stream_);
         symgpu_vorbis_fe_reset(fe_);
         have_prev_ = false;
         frames_ = 0;
@@ -420,14 +425,14 @@ class GpuVorbisDecoder final : public AudioDecoder {
     Result<AudioBufferRef> decode(const Packet& packet) override {
         frames_ = first_ = 0;
         symgpu_vorbis_unit unit;
-        symgpu_status st = symgpu_vorbis_fe_decode(fe_, packet.data, packet.len, slot_, 0, &unit, floor_y_, residue_.data());
+        symgpu_status st = symgpu_vorbis_fe_decode(fe_, packet.data, packet.len, slot_, floor_base_, &unit, floor_y_, residue_.data());
         if (st != SYMGPU_OK) return {{}, map_status(st)};
-        symgpu_vorbis_run run{};
-        run.stream = 0, run.first_packet = 0, run.n_packets = 1;
-        st = symgpu_vorbis_synth_host(ctx_, &unit, floor_y_, residue_.data(), &run, 1, 1, slot_, pcm_.data());
+        symgpu_ticket ticket;  // batched with the Vorbis packets other decoders of this context have in flight
+        st = symgpu_vorbis_submit(gpu_->raw(), stream_, &unit, floor_y_, residue_.data(), slot_, &ticket);
+        if (st == SYMGPU_OK) st = symgpu_vorbis_wait(gpu_->raw(), ticket, pcm_.data());
         if (st != SYMGPU_OK) return {{}, map_status(st)};
-        const size_t prev_n = size_t(1) << (unit.prev_block_flag ? stream_.bs1_exp : stream_.bs0_exp);
-        const size_t n = size_t(1) << (unit.block_flag ? stream_.bs1_exp : stream_.bs0_exp);
+        const size_t prev_n = size_t(1) << (unit.prev_block_flag ? config_.bs1_exp : config_.bs0_exp);
+        const size_t n = size_t(1) << (unit.block_flag ? config_.bs1_exp : config_.bs0_exp);
         frames_ = (prev_n + n) / 4;
         if (opts_.gapless) {  // lib.rs:316-326
             if (!have_prev_) {
@@ -451,15 +456,17 @@ class GpuVorbisDecoder final : public AudioDecoder {
     }
 
   private:
-    GpuVorbisDecoder(symgpu_ctx* ctx, AudioCodecParameters p, AudioDecoderOptions o, symgpu_vorbis_fe* fe, symgpu_vorbis_stream stream)
-        : ctx_(ctx), params_(std::move(p)), opts_(o), fe_(fe), stream_(stream), slot_((1u << stream.bs1_exp) >> 1),
-          residue_(2 * size_t(slot_), 0.0f), pcm_(2 * size_t(slot_), 0.0f) {}
-    symgpu_ctx* ctx_;
+    GpuVorbisDecoder(std::shared_ptr<GpuContext> gpu, AudioCodecParameters p, AudioDecoderOptions o, symgpu_vorbis_fe* fe,
+                     symgpu_vorbis_stream config, uint32_t stream, uint32_t floor_base)
+        : gpu_(std::move(gpu)), params_(std::move(p)), opts_(o), fe_(fe), config_(config), stream_(stream), floor_base_(floor_base),
+          slot_((1u << config.bs1_exp) >> 1), residue_(2 * size_t(slot_), 0.0f), pcm_(2 * size_t(slot_), 0.0f) {}
+    std::shared_ptr<GpuContext> gpu_;
     AudioCodecParameters params_;
     AudioDecoderOptions opts_;
     symgpu_vorbis_fe* fe_;
-    symgpu_vorbis_stream stream_;
-    uint32_t slot_;
+    symgpu_vorbis_stream config_;
+    uint32_t stream_, floor_base_;
+    uint32_t slot_;  // floats per channel of the residue / PCM buffers: blocksize_1 / 2
     uint16_t floor_y_[2 * 65];
     std::vector<float> residue_, pcm_;
     size_t frames_ = 0, first_ = 0;

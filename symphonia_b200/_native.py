@@ -105,6 +105,14 @@ assert VORBIS_SETUP_INFO_DTYPE.itemsize == 160
 assert PIECE_DTYPE.itemsize == 16 and OGG_PACKET_DTYPE.itemsize == 40 and VORBIS_IDENT_DTYPE.itemsize == 8
 AAC_ONLY_LONG, AAC_LONG_START, AAC_EIGHT_SHORT, AAC_LONG_STOP = 0, 1, 2, 3
 
+# `symgpu_ticket` (thread-safe submission) and the queues of symgpu_async_stats (`symgpu_codec`)
+class Ticket(ctypes.Structure):
+    _fields_ = [("batch", ctypes.c_uint64), ("slot", ctypes.c_uint32), ("reserved", ctypes.c_uint32)]
+
+
+CODEC_MP3, CODEC_MP1, CODEC_MP2, CODEC_AAC, CODEC_VORBIS = 0, 1, 2, 3, 4
+VORBIS_SLOT_FLOORS = 64
+
 MP3_LONG, MP3_START, MP3_SHORT, MP3_END = 0, 1, 2, 3
 F_MIXED, F_SCALEFAC_SCALE, F_PREFLAG, F_SFC_LSB = 1, 2, 4, 8
 F_MID_SIDE, F_INTENSITY, F_MPEG1, F_MUTE = 16, 32, 64, 128
@@ -282,6 +290,26 @@ def lib():
     L.symgpu_vorbis_fe_decode_packets_jobs.argtypes = [vp, sz, vp, sz, vp, sz, vp, sz, u32, u32, vp, vp, vp, vp, ctypes.POINTER(sz), u32]
     L.symgpu_aac_fe_tables.restype = None
     L.symgpu_aac_fe_tables.argtypes = [vp, vp, vp]
+    # thread-safe submission (ctypes releases the GIL around these calls, so Python threads can share one context)
+    pt, u8 = ctypes.POINTER(Ticket), ctypes.c_uint8
+    L.symgpu_mp3_submit.restype = ctypes.c_int
+    L.symgpu_mp3_submit.argtypes = [vp, u32, vp, vp, u8, u8, pt]
+    L.symgpu_aac_submit.restype = ctypes.c_int
+    L.symgpu_aac_submit.argtypes = [vp, u32, vp, vp, u32, vp, u8, pt]
+    L.symgpu_mpa12_submit.restype = ctypes.c_int
+    L.symgpu_mpa12_submit.argtypes = [vp, u32, vp, u32, u8, pt]
+    L.symgpu_vorbis_submit.restype = ctypes.c_int
+    L.symgpu_vorbis_submit.argtypes = [vp, u32, vp, vp, vp, u32, pt]
+    for name in ("symgpu_mp3_wait", "symgpu_aac_wait", "symgpu_mpa12_wait", "symgpu_vorbis_wait"):
+        fn = getattr(L, name)
+        fn.restype = ctypes.c_int
+        fn.argtypes = [vp, Ticket, vp]
+    L.symgpu_async_stats.restype = ctypes.c_int
+    L.symgpu_async_stats.argtypes = [vp, ctypes.c_int, ctypes.POINTER(ctypes.c_uint64), ctypes.POINTER(ctypes.c_uint64)]
+    L.symgpu_vorbis_streams_alloc.restype = ctypes.c_int
+    L.symgpu_vorbis_streams_alloc.argtypes = [vp, u32]
+    L.symgpu_vorbis_stream_configure.restype = ctypes.c_int
+    L.symgpu_vorbis_stream_configure.argtypes = [vp, u32, vp, vp, u32, ctypes.POINTER(u32)]
     _LIB = L
     return L
 

@@ -2,8 +2,10 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <atomic>
 #include <cstdio>
 #include <cstring>
+#include <mutex>
 #include <vector>
 
 #include "../../include/symgpu.h"
@@ -11,15 +13,19 @@
 #include "mp3_kernel.h"
 #include "tables.h"
 
-struct symgpu_async_mp3;                       // symgpu_async.cpp: batches gathered from many submitting threads
-void symgpu_async_mp3_destroy(symgpu_async_mp3*);
+struct symgpu_async;                           // symgpu_async.cpp: batches gathered from many submitting threads
+symgpu_async* symgpu_async_create();
+void symgpu_async_destroy(symgpu_async*);
 
 struct symgpu_ctx {
     int device = 0;
     cudaStream_t stream = nullptr;
     char cuda_err[256] = {0};
     uint64_t launches = 0;
-    symgpu_async_mp3* async_mp3 = nullptr;
+    symgpu_async* async = nullptr; // one submission queue per codec
+    // Held by every batch leader of every codec around its host-entry-point call, and by the stream-slot calls decoders make
+    // while other threads decode (resets, Vorbis slot configuration): they share d_stage, the plan / chunk caches and the stream.
+    std::mutex launch_m;
     int numa_node = -1; // node the creating thread was bound to (-1: platform does not say, -2: binding switched off)
     // Layer III kernel choice (SYMGPU_MP3_KERNEL): 0 auto (by plan shape: long runs -> first generation,
     // short runs -> second generation), 1 always the first generation, 2 always the second
@@ -96,6 +102,10 @@ struct symgpu_ctx {
     void* d_vorbis_mc_scratch = nullptr; // per-pair unit records + stream of every packet
     size_t vorbis_mc_scratch_cap = 0;
     uint32_t vorbis_cfg_epoch = 0;   // bumped by streams_set: chunk sizes depend on the stream block sizes
+    // slots of symgpu_vorbis_streams_alloc: floor setups configured per slot (empty when the streams came from streams_set);
+    // a slot is configured when its record's bs1_exp is non-zero
+    std::vector<uint8_t> vorbis_slot_floors;
+    std::atomic<uint32_t> vorbis_row{0}; // largest blocksize_1 / 2 among the configured slots: the row of a submission batch
 };
 
 namespace symgpu_detail {

@@ -504,6 +504,11 @@ symgpu_status symgpu_ctx_create(int device, symgpu_ctx** out) {
     symgpu_ctx* ctx = new (std::nothrow) symgpu_ctx();
     if (!ctx) return SYMGPU_ERR_LIMIT;
     ctx->device = device;
+    ctx->async = symgpu_async_create();
+    if (!ctx->async) {
+        delete ctx;
+        return SYMGPU_ERR_LIMIT;
+    }
     // SYMGPU_ZERO_COPY = 0 never (default) | 1 output only | 2 input and output
     if (const char* env = std::getenv("SYMGPU_COPY_STREAMS")) ctx->copy_streams = std::atoi(env) >= 2 ? 2 : 1;
     if (const char* env = std::getenv("SYMGPU_ZERO_COPY")) {
@@ -526,6 +531,7 @@ symgpu_status symgpu_ctx_create(int device, symgpu_ctx** out) {
         int nw = 0, mode = 0;
         if (std::sscanf(env, "%d:%d", &nw, &mode) != 2 || !mp3v2_set_variant(nw, mode)) {
             std::fprintf(stderr, "symgpu: SYMGPU_MP3_V2_VARIANT=%s is not a built variant\n", env);
+            symgpu_async_destroy(ctx->async);
             delete ctx;
             return SYMGPU_ERR_ARG;
         }
@@ -556,7 +562,7 @@ void symgpu_ctx_destroy(symgpu_ctx* ctx) {
     if (!ctx) return;
     DeviceGuard guard(ctx->device);
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
-    symgpu_async_mp3_destroy(ctx->async_mp3);
+    symgpu_async_destroy(ctx->async);
     if (ctx->d_mp3_tab) cudaFree(ctx->d_mp3_tab);
     if (ctx->d_mp3_states) cudaFree(ctx->d_mp3_states);
     if (ctx->d_mp3_gen) cudaFree(ctx->d_mp3_gen);
@@ -624,6 +630,7 @@ symgpu_status symgpu_mp3_streams_alloc(symgpu_ctx* ctx, uint32_t n_streams) {
 symgpu_status symgpu_mp3_stream_reset(symgpu_ctx* ctx, uint32_t stream) {
     if (!ctx) return SYMGPU_ERR_ARG;
     if (stream >= ctx->n_mp3_streams) return SYMGPU_ERR_LIMIT;
+    std::lock_guard<std::mutex> g(ctx->launch_m); // decoders reset their slot while other threads' batches run
     DeviceGuard guard(ctx->device);
     CU(ctx, cudaMemsetAsync(ctx->d_mp3_states + (size_t)stream * 2, 0, 2 * sizeof(Mp3StreamState), ctx->stream));
     return SYMGPU_OK;

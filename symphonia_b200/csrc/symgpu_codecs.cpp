@@ -65,6 +65,37 @@ symgpu_status ensure_codec_tables(symgpu_ctx* ctx) {
     return SYMGPU_OK;
 }
 
+// Replaces the Vorbis stream records, overlap states and generation counters with zeroed ones for n streams (records are left
+// for the caller to fill).  Drops the slots of symgpu_vorbis_streams_alloc and the multichannel registration.
+symgpu_status vorbis_streams_realloc(symgpu_ctx* ctx, uint32_t n_streams) {
+    DeviceGuard guard(ctx->device);
+    CU(ctx, cudaStreamSynchronize(ctx->stream));
+    symgpu_status st = ensure_codec_tables(ctx);
+    if (st != SYMGPU_OK) return st;
+    if (ctx->d_vorbis_streams) cudaFree(ctx->d_vorbis_streams);
+    if (ctx->d_vorbis_states) cudaFree(ctx->d_vorbis_states);
+    if (ctx->d_vorbis_gen) cudaFree(ctx->d_vorbis_gen);
+    ctx->d_vorbis_streams = nullptr;
+    ctx->d_vorbis_states = nullptr;
+    ctx->d_vorbis_gen = nullptr;
+    ctx->n_vorbis_streams = 0;
+    ctx->h_vorbis_streams.clear();
+    ctx->vorbis_slot_floors.clear();
+    ctx->vorbis_row = 0;
+    CU(ctx, cudaMalloc(&ctx->d_vorbis_streams, (size_t)n_streams * sizeof(symgpu_vorbis_stream)));
+    CU(ctx, cudaMemset(ctx->d_vorbis_streams, 0, (size_t)n_streams * sizeof(symgpu_vorbis_stream)));
+    const size_t bytes = (size_t)n_streams * 2 * kVorbisStateFloats * sizeof(float);
+    CU(ctx, cudaMalloc(&ctx->d_vorbis_states, bytes));
+    CU(ctx, cudaMemset(ctx->d_vorbis_states, 0, bytes));
+    CU(ctx, cudaMalloc(&ctx->d_vorbis_gen, ((size_t)n_streams + 1) * sizeof(uint32_t)));
+    CU(ctx, cudaMemset(ctx->d_vorbis_gen, 0, ((size_t)n_streams + 1) * sizeof(uint32_t)));
+    ctx->n_vorbis_mc_streams = 0; // (symgpu_vorbis_mc_streams_set sets it again after symgpu_vorbis_streams_set)
+    ctx->vorbis_cfg_epoch = (ctx->vorbis_cfg_epoch + 1) & 0xffu;
+    ctx->chunk_key.clear();
+    ctx->n_vorbis_streams = n_streams;
+    return SYMGPU_OK;
+}
+
 } // namespace
 
 extern "C" {
@@ -95,6 +126,7 @@ symgpu_status symgpu_aac_streams_alloc(symgpu_ctx* ctx, uint32_t n_streams) {
 symgpu_status symgpu_aac_stream_reset(symgpu_ctx* ctx, uint32_t stream) {
     if (!ctx) return SYMGPU_ERR_ARG;
     if (stream >= ctx->n_aac_streams) return SYMGPU_ERR_LIMIT;
+    std::lock_guard<std::mutex> g(ctx->launch_m); // decoders reset their slot while other threads' batches run
     DeviceGuard guard(ctx->device);
     CU(ctx, cudaMemsetAsync(ctx->d_aac_states + (size_t)stream * 4096, 0, 4096 * sizeof(float), ctx->stream));
     return SYMGPU_OK;
@@ -298,29 +330,64 @@ symgpu_status symgpu_vorbis_streams_set(symgpu_ctx* ctx, const symgpu_vorbis_str
         if (s.channels < 1 || s.channels > 2) return SYMGPU_ERR_UNSUPPORTED;
         if (s.coupled && s.channels != 2) return SYMGPU_ERR_ARG;
     }
-    DeviceGuard guard(ctx->device);
-    CU(ctx, cudaStreamSynchronize(ctx->stream));
-    symgpu_status st = ensure_codec_tables(ctx);
+    symgpu_status st = vorbis_streams_realloc(ctx, n_streams);
     if (st != SYMGPU_OK) return st;
-    if (ctx->d_vorbis_streams) cudaFree(ctx->d_vorbis_streams);
-    if (ctx->d_vorbis_states) cudaFree(ctx->d_vorbis_states);
-    if (ctx->d_vorbis_gen) cudaFree(ctx->d_vorbis_gen);
-    ctx->d_vorbis_streams = nullptr;
-    ctx->d_vorbis_states = nullptr;
-    ctx->d_vorbis_gen = nullptr;
-    ctx->n_vorbis_streams = 0;
-    CU(ctx, cudaMalloc(&ctx->d_vorbis_streams, (size_t)n_streams * sizeof *streams));
     CU(ctx, cudaMemcpy(ctx->d_vorbis_streams, streams, (size_t)n_streams * sizeof *streams, cudaMemcpyHostToDevice));
-    const size_t bytes = (size_t)n_streams * 2 * kVorbisStateFloats * sizeof(float);
-    CU(ctx, cudaMalloc(&ctx->d_vorbis_states, bytes));
-    CU(ctx, cudaMemset(ctx->d_vorbis_states, 0, bytes));
-    CU(ctx, cudaMalloc(&ctx->d_vorbis_gen, ((size_t)n_streams + 1) * sizeof(uint32_t)));
-    CU(ctx, cudaMemset(ctx->d_vorbis_gen, 0, ((size_t)n_streams + 1) * sizeof(uint32_t)));
     ctx->h_vorbis_streams.assign(streams, streams + n_streams);
-    ctx->n_vorbis_mc_streams = 0; // (symgpu_vorbis_mc_streams_set sets it again after this call)
-    ctx->vorbis_cfg_epoch = (ctx->vorbis_cfg_epoch + 1) & 0xffu;
+    return SYMGPU_OK;
+}
+
+symgpu_status symgpu_vorbis_streams_alloc(symgpu_ctx* ctx, uint32_t n_streams) {
+    if (!ctx || n_streams == 0) return SYMGPU_ERR_ARG;
+    if (n_streams > SYMGPU_VORBIS_MAX_SLOTS) return SYMGPU_ERR_LIMIT;
+    symgpu_status st = vorbis_streams_realloc(ctx, n_streams);
+    if (st != SYMGPU_OK) return st;
+    const size_t n_floors = (size_t)n_streams * SYMGPU_VORBIS_SLOT_FLOORS;
+    if (ctx->d_vorbis_floors) cudaFree(ctx->d_vorbis_floors);
+    if (ctx->d_vorbis_floor_aux) cudaFree(ctx->d_vorbis_floor_aux);
+    ctx->d_vorbis_floors = nullptr;
+    ctx->d_vorbis_floor_aux = nullptr;
+    ctx->n_vorbis_floors = 0;
+    CU(ctx, cudaMalloc(&ctx->d_vorbis_floors, n_floors * sizeof(symgpu_vorbis_floor1)));
+    CU(ctx, cudaMemset(ctx->d_vorbis_floors, 0, n_floors * sizeof(symgpu_vorbis_floor1)));
+    CU(ctx, cudaMalloc(&ctx->d_vorbis_floor_aux, n_floors * sizeof(FloorAux)));
+    CU(ctx, cudaMemset(ctx->d_vorbis_floor_aux, 0, n_floors * sizeof(FloorAux)));
+    ctx->n_vorbis_floors = (uint32_t)n_floors;
+    ctx->h_vorbis_streams.assign(n_streams, symgpu_vorbis_stream{}); // bs1_exp 0: not configured
+    ctx->vorbis_slot_floors.assign(n_streams, 0);
+    ctx->vorbis_row = 0;
+    return SYMGPU_OK;
+}
+
+symgpu_status symgpu_vorbis_stream_configure(symgpu_ctx* ctx, uint32_t stream, const symgpu_vorbis_stream* config,
+                                             const symgpu_vorbis_floor1* floors, uint32_t n_floors, uint32_t* floor_base) {
+    if (!ctx || !config || !floor_base || (n_floors && !floors) || n_floors > SYMGPU_VORBIS_SLOT_FLOORS) return SYMGPU_ERR_ARG;
+    if (stream >= ctx->vorbis_slot_floors.size()) return SYMGPU_ERR_LIMIT;
+    const symgpu_vorbis_stream& s = *config;
+    if (s.bs0_exp < 6 || s.bs1_exp > 13 || s.bs0_exp > s.bs1_exp) return SYMGPU_ERR_ARG; // as symgpu_vorbis_streams_set
+    if (s.channels < 1 || s.channels > 2) return SYMGPU_ERR_UNSUPPORTED;
+    if (s.coupled && s.channels != 2) return SYMGPU_ERR_ARG;
+    std::vector<FloorAux> aux(n_floors);
+    if (n_floors) {
+        const symgpu_status chk = symgpu_vorbis_floors_levels(floors, n_floors, reinterpret_cast<uint8_t*>(aux.data()));
+        if (chk != SYMGPU_OK) return chk;
+    }
+    std::lock_guard<std::mutex> g(ctx->launch_m); // no batch is on the device while the slot changes
+    DeviceGuard guard(ctx->device);
+    const size_t base = (size_t)stream * SYMGPU_VORBIS_SLOT_FLOORS;
+    CU(ctx, cudaMemcpyAsync(ctx->d_vorbis_streams + stream, config, sizeof *config, cudaMemcpyHostToDevice, ctx->stream));
+    if (n_floors) {
+        CU(ctx, cudaMemcpyAsync(ctx->d_vorbis_floors + base, floors, n_floors * sizeof *floors, cudaMemcpyHostToDevice, ctx->stream));
+        CU(ctx, cudaMemcpyAsync(ctx->d_vorbis_floor_aux + base, aux.data(), n_floors * sizeof(FloorAux), cudaMemcpyHostToDevice, ctx->stream));
+    }
+    CU(ctx, cudaMemsetAsync(ctx->d_vorbis_states + (size_t)stream * 2 * kVorbisStateFloats, 0, 2 * kVorbisStateFloats * sizeof(float), ctx->stream));
+    CU(ctx, cudaStreamSynchronize(ctx->stream)); // `aux` is a local vector
+    ctx->h_vorbis_streams[stream] = s;
+    ctx->vorbis_slot_floors[stream] = (uint8_t)n_floors;
+    ctx->vorbis_row = std::max<uint32_t>(ctx->vorbis_row.load(), (1u << s.bs1_exp) >> 1);
+    ctx->vorbis_cfg_epoch = (ctx->vorbis_cfg_epoch + 1) & 0xffu; // chunk sizes depend on the stream block sizes
     ctx->chunk_key.clear();
-    ctx->n_vorbis_streams = n_streams;
+    *floor_base = (uint32_t)base;
     return SYMGPU_OK;
 }
 
@@ -344,12 +411,14 @@ symgpu_status symgpu_vorbis_floors_set(symgpu_ctx* ctx, const symgpu_vorbis_floo
     CU(ctx, cudaMalloc(&ctx->d_vorbis_floor_aux, (size_t)n_floors * sizeof(FloorAux)));
     CU(ctx, cudaMemcpy(ctx->d_vorbis_floor_aux, aux.data(), (size_t)n_floors * sizeof(FloorAux), cudaMemcpyHostToDevice));
     ctx->n_vorbis_floors = n_floors;
+    ctx->vorbis_slot_floors.clear(); // the slots' floor ranges are gone
     return SYMGPU_OK;
 }
 
 symgpu_status symgpu_vorbis_stream_reset(symgpu_ctx* ctx, uint32_t stream) {
     if (!ctx) return SYMGPU_ERR_ARG;
     if (stream >= ctx->n_vorbis_streams) return SYMGPU_ERR_LIMIT;
+    std::lock_guard<std::mutex> g(ctx->launch_m);
     DeviceGuard guard(ctx->device);
     CU(ctx, cudaMemsetAsync(ctx->d_vorbis_states + (size_t)stream * 2 * kVorbisStateFloats, 0,
                             2 * kVorbisStateFloats * sizeof(float), ctx->stream));
@@ -396,6 +465,7 @@ static symgpu_status vorbis_synth_dev_impl(symgpu_ctx* ctx, const symgpu_vorbis_
         if ((uint64_t)run.first_packet + run.n_packets > n_packets || run.reserved) return SYMGPU_ERR_ARG;
         if (reg(run.stream) >= ctx->n_vorbis_streams) return SYMGPU_ERR_LIMIT;
         const symgpu_vorbis_stream& cfg = ctx->h_vorbis_streams[reg(run.stream)];
+        if (cfg.bs1_exp == 0) return SYMGPU_ERR_ARG;                  // a slot of symgpu_vorbis_streams_alloc never configured
         if ((1u << (cfg.bs1_exp - 1)) > slot) return SYMGPU_ERR_ARG; // slot too small for this stream
         covered += run.n_packets;
         split_even(run.n_packets, per_chunk, [&](uint32_t lo, uint32_t hi, bool first, bool last) {

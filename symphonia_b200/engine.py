@@ -311,3 +311,84 @@ class Engine:
         self._check(self._lib.symgpu_vorbis_synth_dev(
             self._ctx, ctypes.c_void_p(units_t.data_ptr()), ctypes.c_void_p(floor_y_t.data_ptr()),
             ctypes.c_void_p(residue_t.data_ptr()), _np_ptr(runs), len(runs), n, int(slot), ctypes.c_void_p(pcm_t.data_ptr())))
+
+    # -- thread-safe submission: many decoder threads, one context, shared launches ---------------------------------------
+    # Every submit copies one frame into the context's open batch and returns a ticket; wait returns that frame's PCM, running
+    # the batch if no other thread has.  ctypes releases the GIL around both, so Python threads can share one Engine.
+    def _submit(self, fn, *args):
+        ticket = _native.Ticket()
+        self._check(fn(self._ctx, *args, ctypes.byref(ticket)))
+        return ticket
+
+    def _wait(self, fn, ticket, out):
+        self._check(fn(self._ctx, ticket, _np_ptr(out)))
+        return out
+
+    def mp3_submit(self, stream, units, spectra, granules_per_frame=2, channels=2):
+        """units [2,2] MP3_GC_DTYPE, spectra [2,2,576] f32 of one frame -> ticket."""
+        units = np.ascontiguousarray(units, dtype=MP3_GC_DTYPE)
+        spectra = np.ascontiguousarray(spectra, dtype=np.float32)
+        if units.size != 4 or spectra.size != 2304:
+            raise ValueError("one frame: units [2,2], spectra [2,2,576]")
+        return self._submit(self._lib.symgpu_mp3_submit, int(stream), _np_ptr(units), _np_ptr(spectra), int(granules_per_frame), int(channels))
+
+    def mp3_wait(self, ticket, out=None):
+        return self._wait(self._lib.symgpu_mp3_wait, ticket, np.empty((2, 1152), dtype=np.float32) if out is None else out)
+
+    def aac_submit(self, stream, units, tns, coeffs, channels=2):
+        """units [2] AAC_UNIT_DTYPE (tns_first counted from the start of `tns`), tns [T] AAC_TNS_DTYPE, coeffs [2,1024] f32 -> ticket."""
+        units = np.ascontiguousarray(units, dtype=AAC_UNIT_DTYPE)
+        tns = np.ascontiguousarray(tns, dtype=AAC_TNS_DTYPE)
+        coeffs = np.ascontiguousarray(coeffs, dtype=np.float32)
+        if units.size != 2 or coeffs.size != 2048:
+            raise ValueError("one frame: units [2], coeffs [2,1024]")
+        return self._submit(self._lib.symgpu_aac_submit, int(stream), _np_ptr(units), _np_ptr(tns) if len(tns) else None, len(tns),
+                            _np_ptr(coeffs), int(channels))
+
+    def aac_wait(self, ticket, out=None):
+        """pcm [2,1024] of the ticket's frame."""
+        return self._wait(self._lib.symgpu_aac_wait, ticket, np.empty((2, 1024), dtype=np.float32) if out is None else out)
+
+    def mpa12_submit(self, stream, subbands, channels=2):
+        """subbands [2,32,n_slots] f32 of one Layer I (n_slots 12) or Layer II (36) frame; `stream` is an MP3 state slot -> ticket."""
+        subbands = np.ascontiguousarray(subbands, dtype=np.float32)
+        if subbands.shape[:2] != (2, 32) or subbands.ndim != 3:
+            raise ValueError("one frame: subbands [2,32,n_slots]")
+        return self._submit(self._lib.symgpu_mpa12_submit, int(stream), _np_ptr(subbands), subbands.shape[2], int(channels))
+
+    def mpa12_wait(self, ticket, out=None):
+        """pcm [2,1152]; plane(ch)[:32 * n_slots] is the frame's output."""
+        return self._wait(self._lib.symgpu_mpa12_wait, ticket, np.empty((2, 1152), dtype=np.float32) if out is None else out)
+
+    def vorbis_streams_alloc(self, n_streams):
+        """Reserves n Vorbis stream slots, configured one at a time with vorbis_stream_configure."""
+        self._check(self._lib.symgpu_vorbis_streams_alloc(self._ctx, int(n_streams)))
+
+    def vorbis_stream_configure(self, stream, config, floors):
+        """config: one VORBIS_STREAM_DTYPE record, floors [<= 64] VORBIS_FLOOR1_DTYPE -> floor_base (= 64 * stream): what a unit's
+        floor index of this stream is counted from."""
+        config = np.ascontiguousarray(config, dtype=VORBIS_STREAM_DTYPE).reshape(1)
+        floors = np.ascontiguousarray(floors, dtype=VORBIS_FLOOR1_DTYPE)
+        base = ctypes.c_uint32(0)
+        self._check(self._lib.symgpu_vorbis_stream_configure(self._ctx, int(stream), _np_ptr(config), _np_ptr(floors) if len(floors) else None,
+                                                             len(floors), ctypes.byref(base)))
+        return base.value
+
+    def vorbis_submit(self, stream, unit, floor_y, residue):
+        """unit VORBIS_UNIT_DTYPE (floors counted from the slot's floor_base), floor_y [2,65] u16, residue [2,slot] f32 -> ticket."""
+        unit = np.ascontiguousarray(unit, dtype=VORBIS_UNIT_DTYPE).reshape(1)
+        floor_y = np.ascontiguousarray(floor_y, dtype=np.uint16)
+        residue = np.ascontiguousarray(residue, dtype=np.float32)
+        if floor_y.size != 130 or residue.ndim != 2 or residue.shape[0] != 2:
+            raise ValueError("one packet: floor_y [2,65], residue [2,slot]")
+        return self._submit(self._lib.symgpu_vorbis_submit, int(stream), _np_ptr(unit), _np_ptr(floor_y), _np_ptr(residue), residue.shape[1])
+
+    def vorbis_wait(self, ticket, slot, out=None):
+        """pcm [2,slot] with the slot the packet was submitted with."""
+        return self._wait(self._lib.symgpu_vorbis_wait, ticket, np.empty((2, int(slot)), dtype=np.float32) if out is None else out)
+
+    def async_stats(self, codec):
+        """(launch batches, frames they held) of the queue of `codec` (_native.CODEC_*)."""
+        b, f = ctypes.c_uint64(0), ctypes.c_uint64(0)
+        self._check(self._lib.symgpu_async_stats(self._ctx, int(codec), ctypes.byref(b), ctypes.byref(f)))
+        return b.value, f.value
