@@ -809,6 +809,53 @@ typedef struct symgpu_flac_packet {        /* 24 bytes */
 symgpu_status symgpu_flac_index(const uint8_t* data, size_t n, symgpu_flac_stream_info* info, symgpu_flac_packet* packets, size_t cap,
                                 size_t* n_out);
 
+/* FLAC decoded on the device, many files per call: packets of file bytes -> interleaved int32 PCM.  One device thread per
+ * packet runs the front-end's own frame decoder (flac_entropy.h, the code behind symgpu_flac_fe_decode_packets), the
+ * restoration kernels of symgpu_flac_restore_* then run unchanged, and a last kernel writes each file's accepted frames, in
+ * stream order, as [frames][channels] into the file's region of `out` (channels a frame does not carry are 0).
+ *   jobs    one per packet; the jobs of one group are consecutive in the table, in stream order
+ *   groups  one per file
+ *   out     int32 [out_cap]: file g's output starts at groups[g].out_offset and holds group_frames[g] * channels samples
+ *   group_frames[g]  frames written for group g;  status[j]  one SYMGPU_FLAC_JOB_* per job
+ * A packet is refused in exactly the cases where symgpu_flac_fe_decode_packets refuses it with the group's stream facts.
+ * Nothing outside [offset, offset + len) of a job is read and nothing outside the file's region of `out` is written. */
+typedef struct symgpu_flac_job {    /* 24 bytes */
+    uint64_t offset;                /* first byte of the packet in `bytes`                                                      */
+    uint32_t len;                   /* its length in bytes                                                                      */
+    uint32_t group;                 /* index of its file in `groups`                                                            */
+    uint32_t slot;                  /* samples per channel it may decode: a larger block is SYMGPU_FLAC_JOB_NO_ROOM.  For a
+                                     * packet of symgpu_flac_index this is its `dur`, which comes from the same header.          */
+    uint32_t reserved;
+} symgpu_flac_job;
+typedef struct symgpu_flac_group {  /* 16 bytes */
+    uint64_t out_offset;            /* first int32 of the file's [frames][channels] output in `out`                              */
+    uint32_t max_block;             /* STREAMINFO block_max (0 = unknown)                                                        */
+    uint8_t bits_per_sample;        /* STREAMINFO (0 = unknown: a frame without its own is refused)                               */
+    uint8_t channels;               /* STREAMINFO channels, 1..8: the output's columns; a frame with more is refused             */
+    uint8_t reserved[2];
+} symgpu_flac_group;
+enum {
+    SYMGPU_FLAC_JOB_DECODED = 0,
+    SYMGPU_FLAC_JOB_REFUSED = 1,    /* the reference refuses the packet                                                          */
+    SYMGPU_FLAC_JOB_NO_ROOM = 2,    /* a valid header whose block is larger than the job's slot                                   */
+    SYMGPU_FLAC_JOB_INVALID = 3     /* device variant only: the job's bytes, group or slot lie outside the buffers it was given   */
+};
+/* Host variant: every pointer is host memory.  jobs and groups are validated completely before anything is launched:
+ * SYMGPU_ERR_ARG for a job outside `bytes`, a group index outside `groups`, the jobs of a group not consecutive, a group
+ * with channels outside 1..8 or bits_per_sample above 32, or an out_offset beyond out_cap; SYMGPU_ERR_LIMIT when a group's
+ * region (out_offset + channels * the sum of its slots) or all regions together exceed out_cap.  Stages through the context's
+ * staging buffer and returns when the results are in host memory; elements of `out` outside the written frames are left as
+ * they were.  One caller at a time per context, as every batch entry point. */
+symgpu_status symgpu_flac_decode_host(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_flac_job* jobs, size_t n_jobs,
+                                      const symgpu_flac_group* groups, size_t n_groups, int32_t* out, size_t out_cap, uint64_t* group_frames,
+                                      uint8_t* status);
+/* Device variant: every pointer is device memory; asynchronous on the context stream, no host round trip.  Not validated on the
+ * host; the kernels check each job's byte range, group index and slot against n_bytes, n_groups and out_cap, and give a job that
+ * fails SYMGPU_FLAC_JOB_INVALID.  Scratch of out_cap int32 plus about 1.2 KB per job comes from the context's staging buffer. */
+symgpu_status symgpu_flac_decode_dev(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_flac_job* jobs, size_t n_jobs,
+                                     const symgpu_flac_group* groups, size_t n_groups, int32_t* out, size_t out_cap, uint64_t* group_frames,
+                                     uint8_t* status);
+
 /* ===================================================================================================
  * Vorbis entropy front-end (SURVEY 8f N1): audio packets -> the batch format of symgpu_vorbis_synth_* (unit, floor-1 Y
  * values, residue vectors BEFORE inverse coupling).  CPU only; one object per stream (codebooks, setup, previous block).

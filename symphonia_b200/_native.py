@@ -97,6 +97,11 @@ FLAC_STREAM_INFO_DTYPE = np.dtype([("n_samples", "<u8"), ("first_frame_pos", "<u
                                    ("reserved", "u1"), ("md5", "u1", (16,)), ("reserved2", "u1", (4,))])
 FLAC_PACKET_DTYPE = np.dtype([("offset", "<u8"), ("ts", "<u8"), ("size", "<u4"), ("dur", "<u4")])
 assert FLAC_STREAM_INFO_DTYPE.itemsize == 56 and FLAC_PACKET_DTYPE.itemsize == 24
+# device FLAC decoding: `symgpu_flac_job` 24 bytes, `symgpu_flac_group` 16 bytes, per-job status values
+FLAC_JOB_DTYPE = np.dtype([("offset", "<u8"), ("len", "<u4"), ("group", "<u4"), ("slot", "<u4"), ("reserved", "<u4")])
+FLAC_GROUP_DTYPE = np.dtype([("out_offset", "<u8"), ("max_block", "<u4"), ("bits_per_sample", "u1"), ("channels", "u1"), ("reserved", "u1", (2,))])
+assert FLAC_JOB_DTYPE.itemsize == 24 and FLAC_GROUP_DTYPE.itemsize == 16
+FLAC_JOB_DECODED, FLAC_JOB_REFUSED, FLAC_JOB_NO_ROOM, FLAC_JOB_INVALID = 0, 1, 2, 3
 MP3_FILE_DTYPE = np.dtype([("data", "<u8"), ("n", "<u8"), ("packets", "<u8"), ("n_packets", "<u8"), ("stream", "<u4"), ("reserved", "<u4")])
 assert MP3_FILE_DTYPE.itemsize == 40
 VORBIS_SETUP_INFO_DTYPE = np.dtype([("n_codebooks", "<u4"), ("n_floors", "<u4"), ("n_residues", "<u4"), ("n_mappings", "<u4"), ("n_modes", "<u4"),
@@ -254,6 +259,10 @@ def lib():
     L.symgpu_flac_fe_decode_packets.argtypes = [vp, sz, vp, sz, u32, u32, u32, vp, vp, vp, vp, sz, vp, sz, psz, psz, psz]
     L.symgpu_flac_index.restype = ctypes.c_int
     L.symgpu_flac_index.argtypes = [vp, sz, vp, vp, sz, psz]
+    for name in ("symgpu_flac_decode_host", "symgpu_flac_decode_dev"):
+        fn = getattr(L, name)
+        fn.restype = ctypes.c_int
+        fn.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, sz, vp, vp]
     L.symgpu_vorbis_fe_create.restype = ctypes.c_int
     L.symgpu_vorbis_fe_create.argtypes = [vp, sz, vp, sz, ctypes.POINTER(vp)]
     L.symgpu_vorbis_fe_destroy.restype = None

@@ -1,233 +1,11 @@
 // FLAC front-end (include/symgpu.h "FLAC front-end", SURVEY §8f N1 for the FLAC row): frame header, sub-frame headers,
 // warm-up samples, quantised predictor coefficients and Rice-coded residuals -- everything FlacDecoder::decode_inner
 // reads from the bitstream (symphonia-bundle-flac/src/frame.rs, decoder.rs:139-640) -- into the descriptor tables and the
-// sample buffer of symgpu_flac_restore_*.  Prediction, wasted-bit shifts, decorrelation and scaling are NOT done here:
-// they are the data-parallel half (flac_kernel.cu / oracle_flac.cpp).  CPU only.
-#include <cstring>
-#include <vector>
-
+// sample buffer of symgpu_flac_restore_*.  The per-packet rules live in flac_entropy.h, shared with the device decoder
+// (flac_decode_kernel.cu); this loop packs the accepted packets densely.  Prediction, wasted-bit shifts, decorrelation
+// and scaling are NOT done here: they are the data-parallel half (flac_kernel.cu / oracle_flac.cpp).
 #include "../../include/symgpu.h"
-#include "mp3_entropy.h"  // Bits: the most-significant-bit-first reader
-
-namespace {
-
-using symgpu::mp3e::Bits;
-
-uint8_t crc8(const uint8_t* p, size_t n) {  // polynomial 0x07, initial value 0 (symphonia-core/src/checksum/crc8.rs:32-65)
-    uint8_t c = 0;
-    for (size_t i = 0; i < n; ++i) {
-        c ^= p[i];
-        for (int k = 0; k < 8; ++k) c = uint8_t(c & 0x80 ? (c << 1) ^ 0x07 : c << 1);
-    }
-    return c;
-}
-
-inline int32_t sign_extend(uint32_t v, unsigned bits) { return bits ? int32_t(v << (32 - bits)) >> (32 - bits) : 0; }
-
-struct Reader {  // bit reader with the two reads FLAC adds: up to 32 bits, and unary
-    Bits b;
-    Reader(const uint8_t* p, size_t n) : b(p, n) {}
-    bool read(unsigned width, uint32_t& v) {  // width <= 32
-        if (width <= 24) return b.read(width, v);
-        uint32_t hi, lo;
-        if (!b.read(width - 16, hi) || !b.read(16, lo)) return false;
-        v = hi << 16 | lo;
-        return true;
-    }
-    bool read_signed(unsigned width, int32_t& v) {
-        uint32_t u;
-        if (!read(width, u)) return false;
-        v = sign_extend(u, width);
-        return true;
-    }
-    bool unary(uint32_t& zeros) {  // zeros before the next 1 bit (bit.rs:642-671); the data ending first is an error
-        zeros = 0;
-        for (;;) {
-            if (b.left() == 0) return false;
-            const uint32_t w = b.window();
-            const size_t take = b.left() < 32 ? b.left() : 32;
-            if (w == 0) {
-                zeros += uint32_t(take), b.at += take;
-                continue;
-            }
-            const unsigned lead = unsigned(__builtin_clz(w));
-            if (lead >= take) {
-                zeros += uint32_t(take), b.at += take;
-                continue;
-            }
-            zeros += lead, b.at += lead + 1;
-            return true;
-        }
-    }
-};
-
-struct Header {
-    uint64_t sequence;
-    bool by_sample;
-    uint32_t block, rate, bps;  // rate / bps 0: not in the header
-    uint32_t channels;
-    uint8_t assignment;
-    size_t size;                // bytes, sync code to CRC-8 inclusive
-};
-
-// frame.rs:66-233.  0 ok, 1 decode error.
-int read_header(const uint8_t* p, size_t n, size_t at, Header& h) {
-    const size_t start = at;
-    auto need = [&](size_t k) { return at + k <= n; };
-    if (!need(4)) return 1;
-    const uint16_t sync = uint16_t(p[at] << 8 | p[at + 1]);
-    const uint16_t desc = uint16_t(p[at + 2] << 8 | p[at + 3]);
-    at += 4;
-    h.by_sample = sync & 1;
-    const uint32_t bs_enc = desc >> 12, sr_enc = (desc >> 8) & 15, ch_enc = (desc >> 4) & 15, bps_enc = (desc >> 1) & 7;
-    if (desc & 1) return 1;
-    // the sequence number, "extended UTF-8" (frame.rs:281-333)
-    {
-        if (!need(1)) return 1;
-        uint64_t v = p[at++];
-        int more;
-        if (v < 0x80) more = 0;
-        else if (v >= 0xc0 && v <= 0xdf) more = 1, v &= 0x1f;
-        else if (v >= 0xe0 && v <= 0xef) more = 2, v &= 0x0f;
-        else if (v >= 0xf0 && v <= 0xf7) more = 3, v &= 0x07;
-        else if (v >= 0xf8 && v <= 0xfb) more = 4, v &= 0x03;
-        else if (v >= 0xfc && v <= 0xfd) more = 5, v &= 0x01;
-        else if (v == 0xfe) more = 6, v = 0;
-        else return 1;  // 10xxxxxx or 0xff cannot start a sequence
-        for (int k = 0; k < more; ++k) {
-            if (!need(1)) return 1;
-            v = v << 6 | (p[at++] & 0x3f);
-        }
-        if (v > (h.by_sample ? 0x000fffffffffull : 0x7fffffffull)) return 1;
-        h.sequence = v;
-    }
-    if (bs_enc == 0) return 1;
-    else if (bs_enc == 1) h.block = 192;
-    else if (bs_enc <= 5) h.block = 576u << (bs_enc - 2);
-    else if (bs_enc == 6) {
-        if (!need(1)) return 1;
-        h.block = uint32_t(p[at++]) + 1;
-    } else if (bs_enc == 7) {
-        if (!need(2)) return 1;
-        const uint32_t v = uint32_t(p[at] << 8 | p[at + 1]);
-        at += 2;
-        if (v == 0xffff) return 1;
-        h.block = v + 1;
-    } else h.block = 256u << (bs_enc - 8);
-    static const uint32_t rates[12] = {0, 88200, 176400, 192000, 8000, 16000, 22050, 24000, 32000, 44100, 48000, 96000};
-    if (sr_enc < 12) h.rate = rates[sr_enc];
-    else if (sr_enc == 12) {
-        if (!need(1)) return 1;
-        h.rate = uint32_t(p[at++]) * 1000;
-    } else if (sr_enc == 15) return 1;
-    else {
-        if (!need(2)) return 1;
-        h.rate = uint32_t(p[at] << 8 | p[at + 1]) * (sr_enc == 14 ? 10 : 1);
-        at += 2;
-    }
-    if (sr_enc != 0 && (h.rate < 1 || h.rate > 655350)) return 1;
-    static const uint8_t widths[8] = {0, 8, 12, 255, 16, 20, 24, 32};
-    if (widths[bps_enc] == 255) return 1;
-    h.bps = widths[bps_enc];
-    if (ch_enc <= 7) h.channels = ch_enc + 1, h.assignment = SYMGPU_FLAC_INDEPENDENT;
-    else if (ch_enc == 8) h.channels = 2, h.assignment = SYMGPU_FLAC_LEFT_SIDE;
-    else if (ch_enc == 9) h.channels = 2, h.assignment = SYMGPU_FLAC_RIGHT_SIDE;
-    else if (ch_enc == 10) h.channels = 2, h.assignment = SYMGPU_FLAC_MID_SIDE;
-    else return 1;
-    if (!need(1)) return 1;
-    if (p[at] != crc8(p + start, at - start)) return 1;
-    ++at;
-    h.size = at - start;
-    return 0;
-}
-
-// decoder.rs:522-640: residuals of samples [prelude, n) into out.  0 ok, 1 decode error.
-int read_residual(Reader& r, uint32_t prelude, int32_t* out, uint32_t n) {
-    uint32_t method, order;
-    if (!r.read(2, method) || method > 1 || !r.read(4, order)) return 1;
-    const unsigned param_bits = method ? 5 : 4;
-    const uint32_t per = n >> order;
-    if (prelude > per || (uint64_t(per) << order) != n) return 1;
-    for (uint32_t part = 0; part < (1u << order); ++part) {
-        const uint32_t a = part ? part * per : prelude, b = (part + 1) * per;
-        uint32_t param;
-        if (!r.read(param_bits, param)) return 1;
-        if (param < (1u << param_bits) - 1) {
-            for (uint32_t i = a; i < b; ++i) {
-                uint32_t q, low = 0;
-                if (!r.unary(q) || !r.read(param, low)) return 1;
-                const uint32_t word = (param < 32 ? q << param : 0) | low;  // (q << param) wraps in the reference for q this large; not reachable in a sized packet
-                out[i] = int32_t(word >> 1) ^ -int32_t(word & 1);
-            }
-        } else {
-            uint32_t width;
-            if (!r.read(5, width)) return 1;
-            for (uint32_t i = a; i < b; ++i)
-                if (!r.read_signed(width, out[i])) return 1;
-        }
-    }
-    return 0;
-}
-
-// decoder.rs:340-520.  0 ok, 1 decode error, 2 unsupported.
-int read_subframe(Reader& r, uint32_t frame_bps, uint32_t n, symgpu_flac_subframe& sf, int32_t* out) {
-    uint32_t v;
-    if (!r.read(1, v) || v) return 1;
-    uint32_t type;
-    if (!r.read(6, type)) return 1;
-    uint32_t order = 0;
-    if (type == 0) sf.type = SYMGPU_FLAC_CONSTANT;
-    else if (type == 1) sf.type = SYMGPU_FLAC_VERBATIM;
-    else if (type >= 8 && type <= 15) {
-        order = type & 7;
-        if (order > 4) return 1;
-        sf.type = SYMGPU_FLAC_FIXED;
-    } else if (type >= 32) {
-        order = (type & 31) + 1;
-        sf.type = SYMGPU_FLAC_LPC;
-    } else return 1;
-    uint32_t wasted = 0;
-    if (!r.read(1, v)) return 1;
-    if (v) {
-        if (!r.unary(wasted)) return 1;
-        ++wasted;
-    }
-    if (wasted > frame_bps) return 1;
-    const uint32_t bps = frame_bps - wasted;
-    if (bps > 32) return 2;  // a 33-bit side channel: the reference's 32-bit reads cannot carry it either
-    sf.wasted = uint8_t(wasted), sf.order = uint8_t(order), sf.shift = 0;
-    std::memset(out, 0, sizeof(int32_t) * n);
-    switch (sf.type) {
-        case SYMGPU_FLAC_CONSTANT:
-            return r.read_signed(bps, out[0]) ? 0 : 1;
-        case SYMGPU_FLAC_VERBATIM:
-            for (uint32_t i = 0; i < n; ++i)
-                if (!r.read_signed(bps, out[i])) return 1;
-            return 0;
-        case SYMGPU_FLAC_FIXED:
-            if (order > n) return 1;
-            for (uint32_t i = 0; i < order; ++i)
-                if (!r.read_signed(bps, out[i])) return 1;
-            return read_residual(r, order, out, n);
-        default: {
-            if (order > n) return 1;
-            for (uint32_t i = 0; i < order; ++i)
-                if (!r.read_signed(bps, out[i])) return 1;
-            uint32_t precision;
-            int32_t shift;
-            if (!r.read(4, precision)) return 1;
-            if (++precision > 15) return 1;
-            if (!r.read_signed(5, shift)) return 1;
-            if (shift < 0) return 2;
-            sf.shift = uint8_t(shift);
-            for (uint32_t j = 0; j < order; ++j)  // coefficient j multiplies the sample j + 1 back (the reference stores them reversed)
-                if (!r.read_signed(precision, sf.coeffs[j])) return 1;
-            return read_residual(r, order, out, n);
-        }
-    }
-}
-
-}  // namespace
+#include "flac_entropy.h"
 
 extern "C" symgpu_status symgpu_flac_fe_decode_packets(const uint8_t* data, size_t n, const symgpu_piece* packets, size_t n_packets,
                                                        uint32_t stream_bps, uint32_t stream_channels, uint32_t max_block,
@@ -239,41 +17,14 @@ extern "C" symgpu_status symgpu_flac_fe_decode_packets(const uint8_t* data, size
     size_t good = 0, sub_at = 0, smp_at = 0;
     for (size_t i = 0; i < n_packets; ++i) {
         if (packets[i].offset > n || packets[i].len > n - packets[i].offset) return SYMGPU_ERR_ARG;
-        const uint8_t* p = data + packets[i].offset;
-        const size_t len = packets[i].len;
-        // frame.rs:66-79: a 14-bit sync code on a byte boundary, searched as 1111 1111 1111 10xx
-        size_t at = 0;
-        for (;; ++at) {
-            if (at + 2 > len) break;
-            if (p[at] == 0xff && (p[at + 1] & 0xfc) == 0xf8) break;
-        }
-        if (at + 2 > len) continue;
-        Header h{};
-        if (read_header(p, len, at, h)) continue;
-        const uint32_t bps = h.bps ? h.bps : stream_bps;
-        if (bps == 0 || bps > 32) continue;
-        if (max_block && h.block > max_block) continue;
-        if (stream_channels && h.channels > stream_channels) continue;
-        if (sub_at + h.channels > subs_cap || smp_at + size_t(h.channels) * h.block > samples_cap) return SYMGPU_ERR_LIMIT;
-        Reader r(p + at + h.size, len - at - h.size);
-        bool ok = true;
-        for (uint32_t c = 0; c < h.channels && ok; ++c) {
-            // the difference channel of a decorrelated pair carries one more bit (decoder.rs:193-225)
-            const bool side = (h.assignment == SYMGPU_FLAC_LEFT_SIDE && c == 1) || (h.assignment == SYMGPU_FLAC_MID_SIDE && c == 1) ||
-                              (h.assignment == SYMGPU_FLAC_RIGHT_SIDE && c == 0);
-            symgpu_flac_subframe& sf = subs[sub_at + c];
-            std::memset(&sf, 0, sizeof sf);
-            sf.offset = smp_at + size_t(c) * h.block, sf.n = h.block;
-            ok = read_subframe(r, bps + (side ? 1 : 0), h.block, sf, samples + sf.offset) == 0;
-        }
-        if (!ok) continue;
-        symgpu_flac_frame& f = frames[good];
-        std::memset(&f, 0, sizeof f);
-        f.first_subframe = uint32_t(sub_at), f.channels = uint8_t(h.channels), f.assignment = h.assignment, f.bits_per_sample = uint8_t(bps);
-        infos[good] = symgpu_flac_frame_info{};
-        infos[good].sequence = h.sequence, infos[good].block_size = h.block, infos[good].sample_rate = h.rate, infos[good].by_sample = h.by_sample;
+        const int r = symgpu::flace::decode_packet(data + packets[i].offset, packets[i].len, stream_bps, stream_channels, max_block, uint32_t(sub_at),
+                                                   subs + sub_at, subs_cap - sub_at, samples + smp_at, smp_at, samples_cap - smp_at, ~0u,
+                                                   frames + good, infos + good);
+        if (r == symgpu::flace::kNoRoom) return SYMGPU_ERR_LIMIT;
+        if (r != symgpu::flace::kDecoded) continue;
+        const uint32_t channels = frames[good].channels, block = infos[good].block_size;
         frame_of[good++] = uint32_t(i);
-        sub_at += h.channels, smp_at += size_t(h.channels) * h.block;
+        sub_at += channels, smp_at += size_t(channels) * block;
     }
     *n_good = good, *n_subs = sub_at, *n_samples = smp_at;
     return SYMGPU_OK;

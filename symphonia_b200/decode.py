@@ -426,3 +426,75 @@ def decode_flac(engine, data):
         return np.zeros((0, plan["channels"]), dtype=np.int32), plan["sample_rate"]
     restored = engine.flac_restore_host(plan["frames"], plan["subframes"], plan["samples"].copy())
     return flac_interleave(plan, restored), plan["sample_rate"]
+
+
+def flac_files_plan(files, threads=None, errors=None):
+    """Host half of decode_flac_files: every file indexed (symgpu_flac_index, on `threads` host threads), their bytes concatenated
+    once, one job per packet and one group per file.  Returns dict(data, jobs, groups, rates, out_cap, failed).  A file that cannot
+    be indexed (listed in `failed`) gets a group without jobs; its message goes to errors[i] when `errors` is a dict."""
+    import concurrent.futures
+    import os
+    messages = {}
+
+    def index(i):
+        try:
+            return packetizer.flac_index(files[i])
+        except Exception as e:  # noqa: BLE001 -- one bad file must not abort the batch; its message is kept
+            messages[i] = f"{type(e).__name__}: {e}"
+            return None
+    with concurrent.futures.ThreadPoolExecutor(max_workers=threads or os.cpu_count()) as pool:
+        ix = list(pool.map(index, range(len(files))))
+    if errors is not None:
+        errors.update(messages)
+    bufs = [np.frombuffer(f, dtype=np.uint8) if not isinstance(f, np.ndarray) else np.ascontiguousarray(f, dtype=np.uint8) for f in files]
+    good = [i for i in range(len(files)) if ix[i] is not None]
+    data = np.concatenate([bufs[i] for i in good]) if good else np.zeros(0, dtype=np.uint8)
+    groups = np.zeros(len(files), dtype=nat.FLAC_GROUP_DTYPE)
+    groups["channels"] = 1
+    rates = np.zeros(len(files), dtype=np.int64)
+    jobs, byte_at, out_at = [], 0, 0
+    for i in good:
+        info, packets = ix[i]
+        g = groups[i]
+        g["out_offset"], g["max_block"], g["bits_per_sample"], g["channels"] = out_at, int(info["block_max"]), int(info["bits_per_sample"]), int(info["channels"])
+        rates[i] = int(info["sample_rate"])
+        j = np.zeros(len(packets), dtype=nat.FLAC_JOB_DTYPE)
+        j["offset"], j["len"], j["group"], j["slot"] = packets["offset"] + byte_at, packets["size"], i, packets["dur"]
+        jobs.append(j)
+        byte_at += bufs[i].size
+        out_at += int(packets["dur"].astype(np.int64).sum()) * int(info["channels"])
+    failed = [i for i in range(len(files)) if ix[i] is None]
+    groups["out_offset"][failed] = out_at
+    jobs = np.concatenate(jobs) if jobs else np.zeros(0, dtype=nat.FLAC_JOB_DTYPE)
+    return dict(data=data, jobs=jobs, groups=groups, rates=rates, out_cap=out_at, failed=failed)
+
+
+def decode_flac_files(engine, files, threads=None, device=False, errors=None):
+    """[(samples [frames, channels] int32, sample_rate)] for a list of native FLAC files, each equal to decode_flac(engine, file):
+    the files are indexed on host threads, and ONE device call decodes every packet of every file -- frame headers and Rice
+    residuals in device code (one thread per packet), restoration and interleaving on the GPU.  device=True: the bytes go to the
+    device once and the samples are int32 CUDA tensors, views of one output tensor.  A file that cannot be indexed yields an empty
+    result with sample rate 0 (its message in errors[i] when `errors` is a dict)."""
+    plan = flac_files_plan(files, threads, errors)
+    groups, rates, cap = plan["groups"], plan["rates"], plan["out_cap"]
+    if device:
+        import torch
+        dev = torch.device("cuda", engine.device)
+        as_t = lambda a: torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(-1)).to(dev)  # noqa: E731
+        out = torch.empty(cap, dtype=torch.int32, device=dev)
+        frames_t = torch.empty(len(groups), dtype=torch.int64, device=dev)
+        status_t = torch.empty(len(plan["jobs"]), dtype=torch.uint8, device=dev)
+        data_t, jobs_t, groups_t = as_t(plan["data"]), as_t(plan["jobs"]), as_t(groups)
+        torch.cuda.current_stream(dev).synchronize()  # the copies above are on torch's stream, the decode on the engine's
+        engine.flac_decode_dev(data_t, jobs_t, groups_t, out, frames_t, status_t)
+        engine.sync()
+        group_frames = frames_t.cpu().numpy()
+    else:
+        out, group_frames, _ = engine.flac_decode_host(plan["data"], plan["jobs"], groups, cap)
+    result = []
+    for g in range(len(groups)):
+        ch, at, n = int(groups[g]["channels"]), int(groups[g]["out_offset"]), int(group_frames[g])
+        if g in plan["failed"]:
+            ch = 0
+        result.append((out[at:at + n * ch].reshape(n, ch), int(rates[g])))
+    return result

@@ -206,6 +206,39 @@ class Engine:
                                                       ctypes.c_void_p(subframes_t.data_ptr()), n_subframes,
                                                       ctypes.c_void_p(samples_t.data_ptr()), samples_t.numel()))
 
+    def flac_decode_host(self, data, jobs, groups, out_cap, out=None):
+        """Device FLAC decoding of many files in one call: `data` (bytes / uint8 array) holds the packets, jobs FLAC_JOB_DTYPE
+        (one per packet, a group's jobs consecutive in stream order), groups FLAC_GROUP_DTYPE (one per file).  Returns (out int32
+        [out_cap], group_frames uint64 [groups], status uint8 [jobs]); file g's PCM is out[out_offset:][:group_frames[g] * channels]
+        as [frames, channels]."""
+        from ._native import FLAC_GROUP_DTYPE, FLAC_JOB_DTYPE
+        a = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
+        jobs = np.ascontiguousarray(jobs, dtype=FLAC_JOB_DTYPE)
+        groups = np.ascontiguousarray(groups, dtype=FLAC_GROUP_DTYPE)
+        if out is None:
+            out = np.zeros(int(out_cap), dtype=np.int32)
+        assert out.dtype == np.int32 and out.flags.c_contiguous and out.size >= out_cap
+        group_frames = np.zeros(len(groups), dtype=np.uint64)
+        status = np.zeros(len(jobs), dtype=np.uint8)
+        self._check(self._lib.symgpu_flac_decode_host(self._ctx, _np_ptr(a) if a.size else None, a.size, _np_ptr(jobs) if len(jobs) else None, len(jobs),
+                                                      _np_ptr(groups) if len(groups) else None, len(groups), _np_ptr(out) if out_cap else None,
+                                                      int(out_cap), _np_ptr(group_frames) if len(groups) else None,
+                                                      _np_ptr(status) if len(jobs) else None))
+        return out, group_frames, status
+
+    def flac_decode_dev(self, data_t, jobs_t, groups_t, out_t, group_frames_t, status_t):
+        """Device-resident variant: torch CUDA tensors (uint8 bytes, jobs / groups as uint8 views of the records, int32 out, int64
+        group_frames, uint8 status); asynchronous on the engine's stream."""
+        from ._native import FLAC_GROUP_DTYPE, FLAC_JOB_DTYPE
+        ts = (data_t, jobs_t, groups_t, out_t, group_frames_t, status_t)
+        assert all(t.is_cuda and t.is_contiguous() for t in ts)
+        n_jobs = jobs_t.numel() * jobs_t.element_size() // FLAC_JOB_DTYPE.itemsize
+        n_groups = groups_t.numel() * groups_t.element_size() // FLAC_GROUP_DTYPE.itemsize
+        assert group_frames_t.numel() >= n_groups and group_frames_t.element_size() == 8 and status_t.numel() >= n_jobs
+        ptr = lambda t: ctypes.c_void_p(t.data_ptr()) if t.numel() else None  # noqa: E731
+        self._check(self._lib.symgpu_flac_decode_dev(self._ctx, ptr(data_t), data_t.numel(), ptr(jobs_t), n_jobs, ptr(groups_t), n_groups, ptr(out_t),
+                                                     out_t.numel(), ptr(group_frames_t), ptr(status_t)))
+
     # -- output stage -------------------------------------------------------------------------
     def pcm_pack_host(self, pcm, spans, channels, fmt, out_frames, plane_stride=0, frames=0, n_spans=None, out=None):
         """Trim + interleave + convert planar f32 `pcm` (any shape, flat indexing) into [out_frames, channels]
