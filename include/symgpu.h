@@ -758,6 +758,65 @@ symgpu_status symgpu_mpa12_fe_decode_packets(const uint8_t* data, size_t n, cons
  * ISO 11172-3 Table 3-B.4 (3, 5, 7, 9, 15, ... 65535 levels).  Returns 98 = the number of floats. */
 size_t symgpu_mpa12_constants(float* out, size_t cap);
 
+/* MPEG Layer I / II decoded on the device, many files per call: packets of file bytes -> interleaved samples of `format`.
+ * The packet rules are those of symgpu_mpa12_fe_decode_packets (mpa12_entropy.h, the same code): one device thread per packet
+ * reads the header and the side information, a warp per frame decodes its sample codewords at their closed-form bit
+ * positions, symgpu_mpa12_synth_dev synthesises every file as a stream (once per layer present), and the output stage of
+ * symgpu_pcm_pack_dev applies the packets' trims and converts.
+ *   jobs    one per packet (its byte range in `bytes` and the packetiser's trims)
+ *   groups  one per file: jobs [first_job, first_job + n_jobs) in stream order, all of one layer.  HOST memory in both variants
+ *           (the synthesis plan is made on the host before anything is decoded).
+ *   out     samples of `format`: file g's output starts at groups[g].out_offset (in samples) and holds results[g].frames frames
+ *           of results[g].channels interleaved samples; its region is 2 x n_jobs x (384 | 1152) samples.
+ *   results one per group;  status  one SYMGPU_MPA12_JOB_* per job (a job that no group names is left undecoded: REFUSED).
+ * A packet is refused in exactly the cases where symgpu_mpa12_fe_decode_packets refuses it for the file's layer: the first
+ * packet whose header parses and whose length matches fixes the file's (sample rate, channels).  Trims are clamped as the
+ * one-file decoder clamps them: trim_start <= per, trim_end <= per - trim_start, per = 384 (Layer I) or 1152 (Layer II).
+ * Each group synthesises in the Layer III state slot it names (symgpu_mp3_streams_alloc); the call resets those slots first,
+ * and their state after the call is unspecified.  The number of launches does not depend on the number of files. */
+typedef struct symgpu_mpa12_job {           /* 24 bytes */
+    uint64_t offset;                        /* first byte of the packet in `bytes`                                              */
+    uint32_t len;                           /* its length in bytes                                                              */
+    uint32_t trim_start;                    /* the packetiser's trims (symgpu_mpa_packet), saturated to 32 bits                  */
+    uint32_t trim_end;
+    uint32_t reserved;
+} symgpu_mpa12_job;
+typedef struct symgpu_mpa12_group {         /* 24 bytes */
+    uint64_t out_offset;                    /* first sample of the file's output in `out`; even                                  */
+    uint32_t first_job;
+    uint32_t n_jobs;
+    uint32_t slot;                          /* Layer III state slot, distinct per group, below the allocated count               */
+    uint8_t layer;                          /* 1 or 2                                                                           */
+    uint8_t reserved[3];
+} symgpu_mpa12_group;
+typedef struct symgpu_mpa12_group_result {  /* 24 bytes */
+    uint64_t frames;                        /* interleaved frames written to the file's region                                  */
+    uint32_t sample_rate;                   /* the signal specification: 0 / 0 when no packet fixed one                         */
+    uint32_t packets;                       /* packets decoded                                                                  */
+    uint8_t channels;
+    uint8_t reserved[7];
+} symgpu_mpa12_group_result;
+enum {
+    SYMGPU_MPA12_JOB_DECODED = 0,
+    SYMGPU_MPA12_JOB_REFUSED = 1,           /* the reference refuses the packet                                                  */
+    SYMGPU_MPA12_JOB_INVALID = 2            /* device variant only: the job's bytes lie outside `bytes`                          */
+};
+/* Host variant: every pointer is host memory.  Everything is validated before anything is launched: SYMGPU_ERR_ARG for a job
+ * outside `bytes`, a group whose jobs lie outside the table or overlap another group's, a layer other than 1 / 2, an odd
+ * out_offset, an unknown format, two groups naming one slot; SYMGPU_ERR_LIMIT for a slot at or above the allocated count or a
+ * region that does not fit in `out` (out_bytes).  Stages through the context's staging buffer and returns when the results
+ * are in host memory; samples of `out` outside the written frames are left as they were. */
+symgpu_status symgpu_mpa12_decode_host(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_mpa12_job* jobs, size_t n_jobs,
+                                       const symgpu_mpa12_group* groups, size_t n_groups, int format, void* out, size_t out_bytes,
+                                       symgpu_mpa12_group_result* results, uint8_t* status);
+/* Device variant: bytes, jobs, out, results and status are device memory, groups host memory; the groups are validated on the
+ * host as above, and the kernels check each job's byte range (SYMGPU_MPA12_JOB_INVALID).  Asynchronous on the context stream
+ * with no copy back to the host; it waits for earlier work on the stream where it uploads the group table and the synthesis
+ * plans.  Scratch of about 19 KB per job comes from the context's staging buffer. */
+symgpu_status symgpu_mpa12_decode_dev(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_mpa12_job* jobs, size_t n_jobs,
+                                      const symgpu_mpa12_group* groups, size_t n_groups, int format, void* out, size_t out_bytes,
+                                      symgpu_mpa12_group_result* results, uint8_t* status);
+
 /* ===================================================================================================
  * FLAC front-end (SURVEY 8f N1 for the FLAC row): a packet (one frame) becomes the descriptors and the residual /
  * warm-up / verbatim samples symgpu_flac_restore_* take.  CPU only, stateless.

@@ -10,7 +10,9 @@
 // skipped as junk, which frames are tags, how packets continue across pages, where the time stamps and trims come
 // from) are the reference's, cited at each function, and are checked bit for bit against oracle/packetizer_oracle.py.
 //
-// Header-only C++17, no dependencies, no device code.
+// Header-only C++17, no dependencies.  The MPEG frame-header functions are also device functions when the header is compiled by
+// nvcc (SYMGPU_PACKET_HD), so the Layer I / II device decoder parses headers with this very code; C++ compilers see plain inline
+// functions.
 #pragma once
 #include <algorithm>
 #include <cstddef>
@@ -19,6 +21,12 @@
 #include <map>
 #include <utility>
 #include <vector>
+
+#if defined(__CUDACC__)
+#define SYMGPU_PACKET_HD __host__ __device__
+#else
+#define SYMGPU_PACKET_HD
+#endif
 
 namespace symgpu {
 namespace packet {
@@ -37,7 +45,7 @@ struct Piece {
 };
 
 namespace detail {
-inline uint32_t be32(const uint8_t* p) { return uint32_t(p[0]) << 24 | uint32_t(p[1]) << 16 | uint32_t(p[2]) << 8 | p[3]; }
+SYMGPU_PACKET_HD inline uint32_t be32(const uint8_t* p) { return uint32_t(p[0]) << 24 | uint32_t(p[1]) << 16 | uint32_t(p[2]) << 8 | p[3]; }
 inline uint32_t be24(const uint8_t* p) { return uint32_t(p[0]) << 16 | uint32_t(p[1]) << 8 | p[2]; }
 inline uint32_t be16(const uint8_t* p) { return uint32_t(p[0]) << 8 | p[1]; }
 inline uint32_t le32(const uint8_t* p) { return uint32_t(p[3]) << 24 | uint32_t(p[2]) << 16 | uint32_t(p[1]) << 8 | p[0]; }
@@ -110,25 +118,25 @@ struct MpaHeader {
     uint32_t sample_rate;     // Hz
     uint32_t frame_size;      // bytes AFTER the 4-byte header word
 
-    int n_channels() const { return mode == MpaMode::Mono ? 1 : 2; }
-    int n_granules() const { return version == MpaVersion::Mpeg1 ? 2 : 1; }
-    uint32_t samples_per_frame() const { return layer == 1 ? 384u : layer == 2 ? 1152u : 576u * uint32_t(n_granules()); }
-    uint32_t header_size() const { return 4u + (crc ? 2u : 0u); }
-    uint32_t side_info_len() const {
+    SYMGPU_PACKET_HD int n_channels() const { return mode == MpaMode::Mono ? 1 : 2; }
+    SYMGPU_PACKET_HD int n_granules() const { return version == MpaVersion::Mpeg1 ? 2 : 1; }
+    SYMGPU_PACKET_HD uint32_t samples_per_frame() const { return layer == 1 ? 384u : layer == 2 ? 1152u : 576u * uint32_t(n_granules()); }
+    SYMGPU_PACKET_HD uint32_t header_size() const { return 4u + (crc ? 2u : 0u); }
+    SYMGPU_PACKET_HD uint32_t side_info_len() const {
         const bool mono = mode == MpaMode::Mono;
         return version == MpaVersion::Mpeg1 ? (mono ? 17u : 32u) : (mono ? 9u : 17u);
     }
 };
 
 // header.rs:71-75: eleven set bits.
-inline bool mpa_is_synced(uint32_t w) { return (w & 0xffe00000u) == 0xffe00000u; }
+SYMGPU_PACKET_HD inline bool mpa_is_synced(uint32_t w) { return (w & 0xffe00000u) == 0xffe00000u; }
 
 // header.rs:49-69: the cheap plausibility test applied while hunting for sync.
-inline bool mpa_check_header(uint32_t w) {
+SYMGPU_PACKET_HD inline bool mpa_check_header(uint32_t w) {
     return ((w >> 19) & 3) != 1 && ((w >> 17) & 3) != 0 && ((w >> 12) & 15) != 15 && ((w >> 10) & 3) != 3;
 }
 
-inline Status mpa_parse_header(uint32_t w, MpaHeader& h) {
+SYMGPU_PACKET_HD inline Status mpa_parse_header(uint32_t w, MpaHeader& h) {
     static constexpr uint16_t kbps[5][15] = {
         {0, 32, 64, 96, 128, 160, 192, 224, 256, 288, 320, 352, 384, 416, 448},  // MPEG-1 Layer I
         {0, 32, 48, 56, 64, 80, 96, 112, 128, 160, 192, 224, 256, 320, 384},     // MPEG-1 Layer II

@@ -102,6 +102,12 @@ FLAC_JOB_DTYPE = np.dtype([("offset", "<u8"), ("len", "<u4"), ("group", "<u4"), 
 FLAC_GROUP_DTYPE = np.dtype([("out_offset", "<u8"), ("max_block", "<u4"), ("bits_per_sample", "u1"), ("channels", "u1"), ("reserved", "u1", (2,))])
 assert FLAC_JOB_DTYPE.itemsize == 24 and FLAC_GROUP_DTYPE.itemsize == 16
 FLAC_JOB_DECODED, FLAC_JOB_REFUSED, FLAC_JOB_NO_ROOM, FLAC_JOB_INVALID = 0, 1, 2, 3
+# device Layer I / II decoding: `symgpu_mpa12_job`, `symgpu_mpa12_group`, `symgpu_mpa12_group_result` (24 bytes each), per-job status
+MPA12_JOB_DTYPE = np.dtype([("offset", "<u8"), ("len", "<u4"), ("trim_start", "<u4"), ("trim_end", "<u4"), ("reserved", "<u4")])
+MPA12_GROUP_DTYPE = np.dtype([("out_offset", "<u8"), ("first_job", "<u4"), ("n_jobs", "<u4"), ("slot", "<u4"), ("layer", "u1"), ("reserved", "u1", (3,))])
+MPA12_RESULT_DTYPE = np.dtype([("frames", "<u8"), ("sample_rate", "<u4"), ("packets", "<u4"), ("channels", "u1"), ("reserved", "u1", (7,))])
+assert MPA12_JOB_DTYPE.itemsize == 24 and MPA12_GROUP_DTYPE.itemsize == 24 and MPA12_RESULT_DTYPE.itemsize == 24
+MPA12_JOB_DECODED, MPA12_JOB_REFUSED, MPA12_JOB_INVALID = 0, 1, 2
 MP3_FILE_DTYPE = np.dtype([("data", "<u8"), ("n", "<u8"), ("packets", "<u8"), ("n_packets", "<u8"), ("stream", "<u4"), ("reserved", "<u4")])
 assert MP3_FILE_DTYPE.itemsize == 40
 VORBIS_SETUP_INFO_DTYPE = np.dtype([("n_codebooks", "<u4"), ("n_floors", "<u4"), ("n_residues", "<u4"), ("n_mappings", "<u4"), ("n_modes", "<u4"),
@@ -263,6 +269,10 @@ def lib():
         fn = getattr(L, name)
         fn.restype = ctypes.c_int
         fn.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, sz, vp, vp]
+    for name in ("symgpu_mpa12_decode_host", "symgpu_mpa12_decode_dev"):
+        fn = getattr(L, name)
+        fn.restype = ctypes.c_int
+        fn.argtypes = [vp, vp, sz, vp, sz, vp, sz, ctypes.c_int, vp, sz, vp, vp]
     L.symgpu_vorbis_fe_create.restype = ctypes.c_int
     L.symgpu_vorbis_fe_create.argtypes = [vp, sz, vp, sz, ctypes.POINTER(vp)]
     L.symgpu_vorbis_fe_destroy.restype = None

@@ -1,6 +1,7 @@
 // MPEG Layer I / II sample decoders (include/symgpu.h, SURVEY §8f N1): bit allocation, scale factors, (de)grouping and
 // dequantisation -- everything Layer1::decode / Layer2::decode do before they call the polyphase synthesis
-// (symphonia-bundle-mp3/src/layer1/mod.rs:73-176, layer2/mod.rs:214-369).  CPU only.
+// (symphonia-bundle-mp3/src/layer1/mod.rs:73-176, layer2/mod.rs:214-369).  The rules themselves are mpa12_entropy.h, shared
+// with the device decoder (mpa12_decode_kernel.cu); this file is the CPU loop over them and the constants' computation.
 //
 // The arithmetic is the reference's, operation for operation (f32, no contraction: the Makefile passes
 // -ffp-contract=off): Layer I  sample = scalefactor * (factor[nb] * (a + 1)),  factor = (2^nb / (2^nb - 1)) * (1 / 2^(nb-1));
@@ -10,213 +11,47 @@
 // number the standard's table prints (which for b = 15, 16 is one ulp above the power of two).
 #include <cmath>
 #include <cstring>
-#include <mutex>
 
 #include "../../include/symgpu.h"
-#include "../../include/symgpu/packetizer.hpp"
-#include "mp3_entropy.h"
+#include "mpa12_entropy.h"
 
-namespace {
+namespace symgpu {
+namespace mpa12e {
 
-using symgpu::mp3e::Bits;
-using symgpu::packet::MpaHeader;
-using symgpu::packet::MpaMode;
-using symgpu::packet::MpaVersion;
-
-struct QuantClass {
-    float c, d;
-    uint8_t read_bits;  // width of one sample, or of the codeword holding three
-    uint8_t bits;       // width of one sample after degrouping
-    uint16_t levels;
-    bool grouped;
-};
-
-struct Constants {
-    float scale[64];
-    float factor[16];       // Layer I
-    QuantClass cls[17];     // by class: 3, 5, 7, 9, 15, 31, ... 65535 levels
-    Constants() {
-        for (int i = 0; i < 63; ++i) scale[i] = float(std::pow(2.0, 1.0 - i / 3.0));
-        scale[63] = 0.0f;  // not in the standard; files use it (layer12.rs:71-74)
-        for (int nb = 0; nb < 16; ++nb) factor[nb] = 0.0f;
+const Constants& host_constants() {
+    static const Constants K = [] {
+        Constants c{};
+        for (int i = 0; i < 63; ++i) c.scale[i] = float(std::pow(2.0, 1.0 - i / 3.0));
+        c.scale[63] = 0.0f;  // not in the standard; files use it (layer12.rs:71-74)
+        for (int nb = 0; nb < 16; ++nb) c.factor[nb] = 0.0f;
         for (int nb = 2; nb < 16; ++nb) {
             const int a = 1 << nb, b = 1 << (nb - 1);
-            factor[nb] = (float(a) / float(a - 1)) * (1.0f / float(b));
+            c.factor[nb] = (float(a) / float(a - 1)) * (1.0f / float(b));
         }
         static const uint16_t levels[17] = {3, 5, 7, 9, 15, 31, 63, 127, 255, 511, 1023, 2047, 4095, 8191, 16383, 32767, 65535};
         for (int k = 0; k < 17; ++k) {
-            QuantClass& q = cls[k];
+            QuantClass& q = c.cls[k];
             q.levels = levels[k];
             int b = 0;
             while ((1u << b) < unsigned(levels[k]) + 1) ++b;
             q.bits = uint8_t(b);
+            q.inv_divisor = float(std::ldexp(1.0, -(b - 1)));
             q.grouped = levels[k] == 3 || levels[k] == 5 || levels[k] == 9;
             q.read_bits = uint8_t(q.grouped ? (levels[k] == 3 ? 5 : levels[k] == 5 ? 7 : 10) : b);
             q.c = float(double(1u << b) / double(levels[k]));
             q.d = q.grouped ? 0.5f : float(std::round(std::ldexp(1.0, -(b - 1)) * 1e11) / 1e11);
         }
-    }
-};
-const Constants& constants() {
-    static const Constants c;
-    return c;
+        return c;
+    }();
+    return K;
 }
 
-// Allocation tables (ISO 11172-3 Tables 3-B.2a-d, 13818-3 Table B.1) as the standard lays them out: a sub-band's row is
-// the list of quantiser sizes its allocation index selects (index 0: nothing allocated).
-struct Row {
-    uint8_t nbal;
-    uint16_t levels[16];
-};
-const Row kRows[8] = {
-    {2, {0, 3, 5, 65535}},
-    {2, {0, 3, 5, 9}},
-    {3, {0, 3, 5, 9, 15, 31, 63, 127}},
-    {3, {0, 3, 5, 7, 9, 15, 31, 65535}},
-    {4, {0, 3, 5, 7, 9, 15, 31, 63, 127, 255, 511, 1023, 2047, 4095, 8191, 16383}},
-    {4, {0, 3, 5, 9, 15, 31, 63, 127, 255, 511, 1023, 2047, 4095, 8191, 16383, 32767}},
-    {4, {0, 3, 5, 7, 9, 15, 31, 63, 127, 255, 511, 1023, 2047, 4095, 8191, 65535}},
-    {4, {0, 3, 7, 15, 31, 63, 127, 255, 511, 1023, 2047, 4095, 8191, 16383, 32767, 65535}},
-};
-struct Table {
-    uint8_t sblimit;
-    uint8_t runs[4][2];  // (sub-bands, row) segments
-};
-const Table kTables[5] = {
-    {27, {{3, 7}, {8, 6}, {12, 3}, {4, 0}}},   // 3-B.2a
-    {30, {{3, 7}, {8, 6}, {12, 3}, {7, 0}}},   // 3-B.2b
-    {8, {{2, 5}, {6, 2}, {0, 0}, {0, 0}}},     // 3-B.2c
-    {12, {{2, 5}, {10, 2}, {0, 0}, {0, 0}}},   // 3-B.2d
-    {30, {{4, 4}, {7, 2}, {19, 1}, {0, 0}}},   // 13818-3 B.1 (MPEG-2 / 2.5)
-};
-inline int class_of(unsigned levels) {  // 3 5 7 9 -> 0..3, 2^k - 1 -> k
-    if (levels <= 9) return int(levels - 3) / 2;
-    int k = 0;
-    while ((1u << k) <= levels) ++k;
-    return k;
-}
+}  // namespace mpa12e
+}  // namespace symgpu
 
-// layer2/mod.rs:136-166
-int table_of(const MpaHeader& h) {
-    if (h.version != MpaVersion::Mpeg1) return 4;
-    const uint32_t per_channel = h.bitrate / uint32_t(h.n_channels());
-    if (per_channel <= 48000) return h.sample_rate == 32000 ? 3 : 2;
-    if (per_channel <= 80000) return 0;
-    return h.sample_rate != 48000 ? 1 : 0;
-}
+namespace {
 
-inline int32_t centre(uint32_t raw, unsigned bits) {  // invert the top bit, sign-extend: offset binary -> two's complement
-    const uint32_t inv = raw ^ (1u << (bits - 1));
-    return int32_t(inv << (32 - bits)) >> (32 - bits);
-}
-
-bool decode_layer1(Bits& bs, const MpaHeader& h, float* out) {
-    const Constants& K = constants();
-    const int n_ch = h.n_channels(), bound = h.mode == MpaMode::JointStereo ? h.bound : 32;
-    uint8_t alloc[2][32] = {};
-    float sf[2][32] = {};
-    uint32_t v;
-    for (int sb = 0; sb < 32; ++sb) {
-        const int readers = sb < bound ? n_ch : 1;
-        for (int ch = 0; ch < readers; ++ch) {
-            if (!bs.read(4, v) || v > 14) return false;
-            alloc[ch][sb] = uint8_t(v ? v + 1 : 0);
-        }
-        if (sb >= bound) alloc[1][sb] = alloc[0][sb];
-    }
-    for (int sb = 0; sb < 32; ++sb)
-        for (int ch = 0; ch < n_ch; ++ch)
-            if (alloc[ch][sb]) {
-                if (!bs.read(6, v)) return false;
-                sf[ch][sb] = K.scale[v];
-            }
-    for (int s = 0; s < 12; ++s)
-        for (int sb = 0; sb < 32; ++sb) {
-            const int readers = sb < bound ? n_ch : 1;
-            for (int ch = 0; ch < readers; ++ch) {
-                const unsigned bits = alloc[ch][sb];
-                if (!bits) continue;
-                if (!bs.read(bits, v)) return false;
-                const float sample = K.factor[bits] * float(centre(v, bits) + 1);
-                if (sb < bound) out[(ch * 32 + sb) * 12 + s] = sf[ch][sb] * sample;
-                else
-                    for (int c = 0; c < n_ch; ++c) out[(c * 32 + sb) * 12 + s] = sf[c][sb] * sample;
-            }
-        }
-    return true;
-}
-
-bool decode_layer2(Bits& bs, const MpaHeader& h, float* out) {
-    const Constants& K = constants();
-    const Table& t = kTables[table_of(h)];
-    const int n_ch = h.n_channels(), sblimit = t.sblimit;
-    const int bound = std::min<int>(h.mode == MpaMode::JointStereo ? h.bound : 32, sblimit);
-    const Row* row[32];
-    for (int sb = 0, r = 0, left = t.runs[0][0]; sb < sblimit; ++sb, --left) {
-        while (left == 0) ++r, left = t.runs[r][0];
-        row[sb] = &kRows[t.runs[r][1]];
-    }
-    uint8_t alloc[2][32] = {}, scfsi[2][32] = {}, sf[2][3][32] = {};
-    uint32_t v;
-    for (int sb = 0; sb < sblimit; ++sb) {
-        const int readers = sb < bound ? n_ch : 1;
-        for (int ch = 0; ch < readers; ++ch) {
-            if (!bs.read(row[sb]->nbal, v)) return false;
-            alloc[ch][sb] = uint8_t(v);
-        }
-        if (sb >= bound) alloc[1][sb] = alloc[0][sb];
-    }
-    for (int sb = 0; sb < sblimit; ++sb)
-        for (int ch = 0; ch < n_ch; ++ch)
-            if (alloc[ch][sb]) {
-                if (!bs.read(2, v)) return false;
-                scfsi[ch][sb] = uint8_t(v);
-            }
-    for (int sb = 0; sb < sblimit; ++sb)
-        for (int ch = 0; ch < n_ch; ++ch)
-            if (alloc[ch][sb]) {
-                uint32_t a, b, c;
-                if (!bs.read(6, a)) return false;
-                b = c = a;
-                switch (scfsi[ch][sb]) {  // which of the three parts share a scale factor (ISO 11172-3 2.4.2.5)
-                    case 0:
-                        if (!bs.read(6, b) || !bs.read(6, c)) return false;
-                        break;
-                    case 1:
-                        if (!bs.read(6, c)) return false;
-                        break;
-                    case 2: break;
-                    default:
-                        if (!bs.read(6, b)) return false;
-                        c = b;
-                }
-                sf[ch][0][sb] = uint8_t(a), sf[ch][1][sb] = uint8_t(b), sf[ch][2][sb] = uint8_t(c);
-            }
-    for (int gr = 0; gr < 12; ++gr)
-        for (int sb = 0; sb < sblimit; ++sb) {
-            const int readers = sb < bound ? n_ch : 1;
-            for (int ch = 0; ch < readers; ++ch) {
-                if (!alloc[ch][sb]) continue;
-                const QuantClass& q = K.cls[class_of(row[sb]->levels[alloc[ch][sb]])];
-                uint32_t raw[3];
-                if (q.grouped) {
-                    if (!bs.read(q.read_bits, v)) return false;
-                    for (int k = 0; k < 3; ++k) raw[k] = v % q.levels, v /= q.levels;
-                } else {
-                    for (int k = 0; k < 3; ++k)
-                        if (!bs.read(q.read_bits, raw[k])) return false;
-                }
-                const float divisor = float(1u << (q.bits - 1));
-                float triplet[3];
-                for (int k = 0; k < 3; ++k) triplet[k] = q.c * (float(centre(raw[k], q.bits)) / divisor + q.d);
-                for (int c = (sb < bound ? ch : 0); c < (sb < bound ? ch + 1 : n_ch); ++c) {
-                    const float scale = K.scale[sf[c][gr / 4][sb]];
-                    for (int k = 0; k < 3; ++k) out[(c * 32 + sb) * 36 + 3 * gr + k] = scale * triplet[k];
-                }
-            }
-        }
-    return true;
-}
+using namespace symgpu::mpa12e;
 
 struct Spec {
     bool have = false;
@@ -224,31 +59,28 @@ struct Spec {
     int channels = 0;
 };
 
+// The packet rules of mpa12_entropy.h in the reference's order; the samples are decoded granule by granule, each codeword at
+// its closed-form position.
 symgpu_status decode_packet(Spec* spec, const uint8_t* frame, size_t n, int layer, float* subbands, symgpu_mp3_frame_info* info) {
-    using namespace symgpu::packet;
-    size_t q = 0;
-    uint32_t word = 0;
-    for (;; ++q) {  // decoder.rs:87: synchronise inside the packet
-        if (q + 4 > n) return SYMGPU_ERR_DECODE;
-        word = detail::be32(frame + q);
-        if (mpa_is_synced(word) && mpa_check_header(word)) break;
-    }
     MpaHeader h{};
-    const Status hs = mpa_parse_header(word, h);
-    if (hs != Status::Ok) return hs == Status::Unsupported ? SYMGPU_ERR_UNSUPPORTED : SYMGPU_ERR_DECODE;
-    const size_t body_len = n - q - 4;
-    if (h.frame_size != body_len) return SYMGPU_ERR_DECODE;
+    size_t q = 0;
+    const int hs = read_header(frame, n, h, q);
+    if (hs != kDecoded) return hs == kUnsupported ? SYMGPU_ERR_UNSUPPORTED : SYMGPU_ERR_DECODE;
     if (spec) {
         if (!spec->have) spec->have = true, spec->rate = h.sample_rate, spec->channels = h.n_channels();
         else if (spec->rate != h.sample_rate || spec->channels != h.n_channels()) return SYMGPU_ERR_DECODE;
     }
-    if (h.layer != layer) return SYMGPU_ERR_DECODE;
-    const size_t crc_len = h.crc ? 2 : 0;
-    if (body_len < crc_len) return SYMGPU_ERR_DECODE;
-    const int n_slots = layer == 1 ? 12 : 36;
+    Side s;
+    if (!body_of(h, layer, n, q, s.body_at, s.body_bytes)) return SYMGPU_ERR_DECODE;
+    const int n_slots = layer == 1 ? 12 : 36, per = layer == 1 ? 1 : 3;
     std::memset(subbands, 0, sizeof(float) * 2 * 32 * n_slots);
-    Bits bs(frame + q + 4 + crc_len, body_len - crc_len);
-    if (!(layer == 1 ? decode_layer1(bs, h, subbands) : decode_layer2(bs, h, subbands))) return SYMGPU_ERR_DECODE;
+    const Constants& K = host_constants();
+    const uint8_t* body = frame + s.body_at;
+    if (!read_side(K, body, h, s) || !fits(s)) return SYMGPU_ERR_DECODE;
+    for (int gr = 0; gr < 12; ++gr)
+        for (int sb = 0; sb < s.sblimit; ++sb)
+            for (int c = 0; c < s.n_ch; ++c)
+                if (!decode_codeword(K, s, body, gr, sb, c, subbands + (c * 32 + sb) * n_slots + gr * per)) return SYMGPU_ERR_DECODE;
     if (info) {
         *info = symgpu_mp3_frame_info{};
         info->sample_rate = h.sample_rate, info->channels = uint8_t(h.n_channels()), info->granules = 1;
@@ -282,7 +114,7 @@ extern "C" symgpu_status symgpu_mpa12_fe_decode_packets(const uint8_t* data, siz
 }
 
 extern "C" size_t symgpu_mpa12_constants(float* out, size_t cap) {
-    const Constants& K = constants();
+    const Constants& K = host_constants();
     float all[98];
     std::memcpy(all, K.scale, sizeof K.scale);
     for (int k = 0; k < 17; ++k) all[64 + k] = K.cls[k].c, all[81 + k] = K.cls[k].d;

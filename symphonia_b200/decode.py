@@ -498,3 +498,97 @@ def decode_flac_files(engine, files, threads=None, device=False, errors=None):
             ch = 0
         result.append((out[at:at + n * ch].reshape(n, ch), int(rates[g])))
     return result
+
+
+# ---- MPEG Layer I / II, many files decoded on the device (header, side information and samples in device code) ----------------
+
+_TORCH_DTYPES = {nat.FMT_F32: "float32", nat.FMT_S16: "int16", nat.FMT_S24: "int32", nat.FMT_S32: "int32", nat.FMT_U8: "uint8"}
+
+
+def mpa12_files_plan(files, threads=None, errors=None):
+    """Host half of decode_mpa12_files: every file indexed (symgpu_mpa_index, on `threads` host threads), their bytes concatenated
+    once, one job per packet and one group per file (group i uses state slot i).  Returns dict(data, jobs, groups, tracks, out_samples,
+    failed).  A file that cannot be indexed or is not Layer I / II (listed in `failed`) gets a group without jobs; its message goes to
+    errors[i] when `errors` is a dict."""
+    import concurrent.futures
+    import os
+    messages = {}
+
+    def index(i):
+        try:
+            track, packets = packetizer.mpa_index(files[i])
+            if int(track["layer"]) not in (1, 2):
+                raise ValueError(f"MPEG Layer {int(track['layer'])}: decode_mpa12_files takes Layer I / II files")
+            return track, packets
+        except Exception as e:  # noqa: BLE001 -- one bad file must not abort the batch; its message is kept
+            messages[i] = f"{type(e).__name__}: {e}"
+            return None
+    with concurrent.futures.ThreadPoolExecutor(max_workers=threads or os.cpu_count()) as pool:
+        ix = list(pool.map(index, range(len(files))))
+    if errors is not None:
+        errors.update(messages)
+    bufs = [np.frombuffer(f, dtype=np.uint8) if not isinstance(f, np.ndarray) else np.ascontiguousarray(f, dtype=np.uint8) for f in files]
+    good = [i for i in range(len(files)) if ix[i] is not None]
+    data = np.concatenate([bufs[i] for i in good]) if good else np.zeros(0, dtype=np.uint8)
+    groups = np.zeros(len(files), dtype=nat.MPA12_GROUP_DTYPE)
+    groups["slot"] = np.arange(len(files))
+    groups["layer"] = 1
+    jobs, byte_at, job_at, out_at = [], 0, 0, 0
+    sat = np.uint64(0xFFFFFFFF)
+    for i in good:
+        track, packets = ix[i]
+        layer, n = int(track["layer"]), len(packets)
+        g = groups[i]
+        g["out_offset"], g["first_job"], g["n_jobs"], g["layer"] = out_at, job_at, n, layer
+        j = np.zeros(n, dtype=nat.MPA12_JOB_DTYPE)
+        j["offset"], j["len"] = packets["offset"] + np.uint64(byte_at), packets["size"]
+        j["trim_start"] = packets["trim_start"]
+        j["trim_end"] = np.minimum(packets["trim_end"].astype(np.uint64), sat)
+        jobs.append(j)
+        byte_at += bufs[i].size
+        job_at += n
+        out_at += 2 * n * (384 if layer == 1 else 1152)
+    failed = [i for i in range(len(files)) if ix[i] is None]
+    groups["out_offset"][failed] = out_at
+    groups["first_job"][failed] = job_at
+    jobs = np.concatenate(jobs) if jobs else np.zeros(0, dtype=nat.MPA12_JOB_DTYPE)
+    tracks = [None if t is None else t[0] for t in ix]
+    return dict(data=data, jobs=jobs, groups=groups, tracks=tracks, out_samples=out_at, failed=failed)
+
+
+def decode_mpa12_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False, errors=None):
+    """[(samples [frames, channels] of `fmt`, sample_rate)] for a list of MPEG Layer I / II files, each equal to
+    decode_mpeg_audio(engine, file, fmt): the files are indexed on host threads, and ONE device call decodes every packet of every
+    file -- headers, bit allocation, scale factors and samples in device code, synthesis and the output stage on the GPU.
+    device=True: the bytes go to the device once and the samples are CUDA tensors, views of one output tensor.  A Layer III file or
+    one that cannot be indexed yields an empty result with sample rate 0 (its message in errors[i] when `errors` is a dict).
+    (Re)allocates the engine's MP3 state slots, one per file."""
+    plan = mpa12_files_plan(files, threads, errors)
+    groups, cap = plan["groups"], plan["out_samples"]
+    engine.mp3_streams_alloc(max(len(files), 1))
+    if device:
+        import torch
+        dev = torch.device("cuda", engine.device)
+        as_t = lambda a: torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(-1)).to(dev)  # noqa: E731
+        out = torch.empty(cap, dtype=getattr(torch, _TORCH_DTYPES[fmt]), device=dev)
+        results_t = torch.empty(len(groups) * nat.MPA12_RESULT_DTYPE.itemsize, dtype=torch.uint8, device=dev)
+        status_t = torch.empty(len(plan["jobs"]), dtype=torch.uint8, device=dev)
+        data_t, jobs_t = as_t(plan["data"]), as_t(plan["jobs"])
+        torch.cuda.current_stream(dev).synchronize()  # the copies above are on torch's stream, the decode on the engine's
+        engine.mpa12_decode_dev(data_t, jobs_t, groups, fmt, out, results_t, status_t)
+        engine.sync()
+        results = results_t.cpu().numpy().view(nat.MPA12_RESULT_DTYPE)
+    else:
+        out, results, _ = engine.mpa12_decode_host(plan["data"], plan["jobs"], groups, fmt, cap)
+    result = []
+    for g in range(len(groups)):
+        if g in plan["failed"]:
+            result.append((out[:0].reshape(0, 0), 0))
+            continue
+        r, track = results[g], plan["tracks"][g]
+        if int(r["packets"]) == 0:   # no frame survived: the track's parameters, as decode_mpeg_audio reports them
+            result.append((out[:0].reshape(0, int(track["channels"])), int(track["sample_rate"])))
+            continue
+        ch, at, n = int(r["channels"]), int(groups[g]["out_offset"]), int(r["frames"])
+        result.append((out[at:at + n * ch].reshape(n, ch), int(r["sample_rate"])))
+    return result
