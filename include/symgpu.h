@@ -740,6 +740,76 @@ typedef struct symgpu_mp3_file {        /* one stream's bytes and packet table (
 symgpu_status symgpu_mp3_decode_files_host(symgpu_ctx* ctx, const symgpu_mp3_file* files, uint32_t n_files, float* pcm, size_t pcm_frames_cap,
                                            uint32_t* good_per_file, uint32_t* frame_of, uint32_t* n_rounds);
 
+/* MPEG Layer III decoded on the device, many files per call: packets of file bytes -> interleaved samples of `format`.  The
+ * packet rules are those of symgpu_mp3_fe_decode_packets (mp3_entropy.h, the same code): one device thread per packet runs
+ * the prologue and the side read, one thread per file walks the bit reservoir over those records (byte arithmetic only), a
+ * warp per frame gathers its main data, one thread per granule-channel decodes scale factors and Huffman data, and the
+ * unchanged POW43 lookup, symgpu_mp3_synth_dev and the output stage of symgpu_pcm_pack_dev follow.
+ *   jobs    one per packet (its byte range in `bytes` and the packetiser's trims)
+ *   groups  one per file: jobs [first_job, first_job + n_jobs) in stream order, with the file's granules per frame (2 MPEG-1,
+ *           1 MPEG-2 / 2.5) and channels (the index's track).  HOST memory in both variants (the synthesis plan is made on
+ *           the host before anything is decoded).  A group whose first accepted header says otherwise refuses all its jobs
+ *           (cannot happen for jobs and groups made from symgpu_mpa_index).
+ *   out     samples of `format`: file g's output starts at groups[g].out_offset (in samples) and holds results[g].frames frames
+ *           of results[g].channels interleaved samples; its region is n_jobs x granules x 576 x channels samples.
+ *   results one per group;  status  one SYMGPU_MP3_JOB_* per job (a job that no group names is left undecoded: REFUSED).
+ *   n_rounds  the rounds the call took (may be NULL).
+ * A packet is decoded exactly when symgpu_mp3_fe_decode_packets decodes it, with one documented exception: a joint-stereo
+ * frame whose channels are on different window sequences, which the reference refuses in its stereo stage after its main
+ * data was read, is left out whole (SYMGPU_MP3_JOB_LEFT_OUT) while the reservoir moves on as for a decoded frame.  Only the
+ * first main-data over-read of a file is certain in one pass (the frames behind it were walked with a reservoir the
+ * reference empties), so the call repeats walk, gather and Huffman decoding for the files that failed, with that frame
+ * marked, until none fails: 1 + the most failed frames of any one file rounds, one 4-byte readback each.  Trims are clamped
+ * as the one-file decoder clamps them.  Each group synthesises in the Layer III state slot it names
+ * (symgpu_mp3_streams_alloc); the call resets those slots first, and their state after the call is unspecified.  The number
+ * of launches per round does not depend on the number of files. */
+typedef struct symgpu_mp3_job {             /* 24 bytes */
+    uint64_t offset;                        /* first byte of the packet in `bytes`                                              */
+    uint32_t len;                           /* its length in bytes                                                              */
+    uint32_t trim_start;                    /* the packetiser's trims (symgpu_mpa_packet), saturated to 32 bits                  */
+    uint32_t trim_end;
+    uint32_t reserved;
+} symgpu_mp3_job;
+typedef struct symgpu_mp3_group {           /* 24 bytes */
+    uint64_t out_offset;                    /* first sample of the file's output in `out`; a multiple of `channels`              */
+    uint32_t first_job;
+    uint32_t n_jobs;
+    uint32_t slot;                          /* Layer III state slot, distinct per group, below the allocated count               */
+    uint8_t granules;                       /* 1 or 2                                                                           */
+    uint8_t channels;                       /* 1 or 2                                                                           */
+    uint8_t reserved[2];
+} symgpu_mp3_group;
+typedef struct symgpu_mp3_group_result {    /* 24 bytes */
+    uint64_t frames;                        /* interleaved frames written to the file's region                                  */
+    uint32_t sample_rate;                   /* the signal specification: 0 / 0 when no packet fixed one                         */
+    uint32_t packets;                       /* packets decoded                                                                  */
+    uint8_t channels;
+    uint8_t reserved[7];
+} symgpu_mp3_group_result;
+enum {
+    SYMGPU_MP3_JOB_DECODED = 0,
+    SYMGPU_MP3_JOB_REFUSED = 1,             /* refused before its main data is read                                             */
+    SYMGPU_MP3_JOB_FAILED = 2,              /* its main data over-reads: dropped, the reservoir emptied                          */
+    SYMGPU_MP3_JOB_LEFT_OUT = 3,            /* joint-stereo window mismatch: left out whole, the reservoir moves on               */
+    SYMGPU_MP3_JOB_INVALID = 4              /* device variant only: the job's bytes lie outside `bytes`                          */
+};
+/* Host variant: every pointer is host memory.  Everything is validated before anything is launched: SYMGPU_ERR_ARG for a job
+ * outside `bytes`, a group whose jobs lie outside the table or overlap another group's, granules or channels other than 1 / 2,
+ * an out_offset that is not a multiple of channels, an unknown format, two groups naming one slot; SYMGPU_ERR_LIMIT for a slot
+ * at or above the allocated count or a region that does not fit in `out` (out_bytes).  Stages through the context's staging
+ * buffer and returns when the results are in host memory; samples of `out` outside the written frames are left as they were. */
+symgpu_status symgpu_mp3_decode_host(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_mp3_job* jobs, size_t n_jobs,
+                                     const symgpu_mp3_group* groups, size_t n_groups, int format, void* out, size_t out_bytes,
+                                     symgpu_mp3_group_result* results, uint8_t* status, uint32_t* n_rounds);
+/* Device variant: bytes, jobs, out, results and status are device memory, groups and n_rounds host memory; the groups are
+ * validated on the host as above, and the kernels check each job's byte range (SYMGPU_MP3_JOB_INVALID).  Work is queued on
+ * the context stream; the call waits for the stream once per round, for the 4-byte "did any file fail" flag, and returns
+ * with the synthesis and the output stage still queued.  Scratch of about 27 KB per job comes from the context's staging
+ * buffer. */
+symgpu_status symgpu_mp3_decode_dev(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_mp3_job* jobs, size_t n_jobs,
+                                    const symgpu_mp3_group* groups, size_t n_groups, int format, void* out, size_t out_bytes,
+                                    symgpu_mp3_group_result* results, uint8_t* status, uint32_t* n_rounds);
+
 /* ===================================================================================================
  * MPEG Layer I / II sample decoders (SURVEY 8f N1 for the Layer I / II path): a packet becomes the sub-band samples
  * symgpu_mpa12_synth_* take.  CPU only, stateless apart from the stream's signal specification.

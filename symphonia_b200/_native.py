@@ -108,6 +108,13 @@ MPA12_GROUP_DTYPE = np.dtype([("out_offset", "<u8"), ("first_job", "<u4"), ("n_j
 MPA12_RESULT_DTYPE = np.dtype([("frames", "<u8"), ("sample_rate", "<u4"), ("packets", "<u4"), ("channels", "u1"), ("reserved", "u1", (7,))])
 assert MPA12_JOB_DTYPE.itemsize == 24 and MPA12_GROUP_DTYPE.itemsize == 24 and MPA12_RESULT_DTYPE.itemsize == 24
 MPA12_JOB_DECODED, MPA12_JOB_REFUSED, MPA12_JOB_INVALID = 0, 1, 2
+# device Layer III decoding: `symgpu_mp3_job`, `symgpu_mp3_group`, `symgpu_mp3_group_result` (24 bytes each), per-job status
+MP3_JOB_DTYPE = np.dtype([("offset", "<u8"), ("len", "<u4"), ("trim_start", "<u4"), ("trim_end", "<u4"), ("reserved", "<u4")])
+MP3_GROUP_DTYPE = np.dtype([("out_offset", "<u8"), ("first_job", "<u4"), ("n_jobs", "<u4"), ("slot", "<u4"), ("granules", "u1"), ("channels", "u1"),
+                            ("reserved", "u1", (2,))])
+MP3_RESULT_DTYPE = np.dtype([("frames", "<u8"), ("sample_rate", "<u4"), ("packets", "<u4"), ("channels", "u1"), ("reserved", "u1", (7,))])
+assert MP3_JOB_DTYPE.itemsize == 24 and MP3_GROUP_DTYPE.itemsize == 24 and MP3_RESULT_DTYPE.itemsize == 24
+MP3_JOB_DECODED, MP3_JOB_REFUSED, MP3_JOB_FAILED, MP3_JOB_LEFT_OUT, MP3_JOB_INVALID = 0, 1, 2, 3, 4
 MP3_FILE_DTYPE = np.dtype([("data", "<u8"), ("n", "<u8"), ("packets", "<u8"), ("n_packets", "<u8"), ("stream", "<u4"), ("reserved", "<u4")])
 assert MP3_FILE_DTYPE.itemsize == 40
 VORBIS_SETUP_INFO_DTYPE = np.dtype([("n_codebooks", "<u4"), ("n_floors", "<u4"), ("n_residues", "<u4"), ("n_mappings", "<u4"), ("n_modes", "<u4"),
@@ -273,6 +280,10 @@ def lib():
         fn = getattr(L, name)
         fn.restype = ctypes.c_int
         fn.argtypes = [vp, vp, sz, vp, sz, vp, sz, ctypes.c_int, vp, sz, vp, vp]
+    for name in ("symgpu_mp3_decode_host", "symgpu_mp3_decode_dev"):
+        fn = getattr(L, name)
+        fn.restype = ctypes.c_int
+        fn.argtypes = [vp, vp, sz, vp, sz, vp, sz, ctypes.c_int, vp, sz, vp, vp, ctypes.POINTER(ctypes.c_uint32)]
     L.symgpu_vorbis_fe_create.restype = ctypes.c_int
     L.symgpu_vorbis_fe_create.argtypes = [vp, sz, vp, sz, ctypes.POINTER(vp)]
     L.symgpu_vorbis_fe_destroy.restype = None

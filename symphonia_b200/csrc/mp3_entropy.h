@@ -5,6 +5,10 @@
 // before it (layer3/mod.rs:272-370 advances `part2_3_begin` by exactly that).  So every CPU test of the front-end is a
 // test of the code the kernel runs.
 //
+// The per-packet rules of Layer III live here too, for the same reason: the packet prologue (shared with Layer I / II,
+// mpa12_entropy.h), the side read into a FrameSide record and one step of the bit reservoir.  symgpu_mp3_fe_decode,
+// symgpu_mp3_entropy_plan and the device decoder (mp3_decode_kernel.cu) are loops over them.
+//
 // Reference: read_scale_factors_mpeg1 / _mpeg2 (symphonia-bundle-mp3/src/layer3/bitstream.rs:240-427),
 // read_huffman_samples (layer3/requantize.rs:47-237), BitReaderLtr::read_codebook (symphonia-core/src/io/bit.rs:771-808).
 #pragma once
@@ -12,6 +16,7 @@
 #include <cstdint>
 
 #include "../../include/symgpu.h"
+#include "../../include/symgpu/packetizer.hpp"
 
 #ifdef __CUDACC__
 #define SYMGPU_HD __host__ __device__ __forceinline__
@@ -333,9 +338,252 @@ SYMGPU_HD int decode_gc_job(const GcJob& j, const uint8_t* md, const HuffSet& hs
     return status;
 }
 
+// ---- packet prologue (decoder.rs:87-128), in the reference's order; all MPEG audio layers ------------------------------
+// 1. read_header: the sync search inside the packet, the header parse, frame_size == the bytes after the header word.
+// 2. (the caller) the signal specification: the first packet that passes 1 fixes (sample rate, channels); a later packet
+//    that differs is refused.  So a packet of the wrong layer but the right size still fixes it.
+// 3. body_of: the layer check, the CRC skip.
+enum : int { kDecoded = 0, kRefused = 1, kUnsupported = 2 };
+SYMGPU_HD int read_header(const uint8_t* frame, size_t n, symgpu::packet::MpaHeader& h, size_t& q) {
+    using namespace symgpu::packet;
+    uint32_t word = 0;
+    for (q = 0;; ++q) {  // decoder.rs:87: synchronise inside the packet
+        if (q + 4 > n) return kRefused;
+        word = detail::be32(frame + q);
+        if (mpa_is_synced(word) && mpa_check_header(word)) break;
+    }
+    const Status hs = mpa_parse_header(word, h);
+    if (hs != Status::Ok) return hs == Status::Unsupported ? kUnsupported : kRefused;
+    return h.frame_size == n - q - 4 ? kDecoded : kRefused;
+}
+SYMGPU_HD bool body_of(const symgpu::packet::MpaHeader& h, int layer, size_t n, size_t q, uint32_t& at, uint32_t& bytes) {
+    if (h.layer != layer) return false;
+    const size_t body_len = n - q - 4, crc_len = h.crc ? 2 : 0;
+    if (body_len < crc_len) return false;
+    at = uint32_t(q + 4 + crc_len), bytes = uint32_t(body_len - crc_len);
+    return true;
+}
+
+// ---- Layer III side information of one packet --------------------------------------------------------------------------
+// The long-block band edges the side read needs (region boundaries), by sample-rate index: computed once on the host
+// (tables.cpp) and handed to the kernels as a parameter, never rebuilt in device code.
+struct LongEdges {
+    uint16_t e[9][23];
+};
+
+enum : uint8_t { kSideRefused = 0, kSideBad = 1, kSideOk = 2 };
+
+// What the prologue and the side read leave for the reservoir walk.  108 bytes.
+struct FrameSide {
+    uint32_t body_at;          // byte offset, in the packet, of the side information (after the header word and the CRC)
+    uint32_t body_bytes;       // bytes from there to the end of the packet
+    uint16_t main_data_begin;
+    uint8_t state;             // kSideRefused (the prologue refused the packet), kSideBad (the side read failed), kSideOk
+    uint8_t n_ch, n_gr, mpeg1, intensity, side_len;
+    uint8_t unit_flags;        // frame-level SYMGPU_MP3_F_* bits
+    uint8_t sample_rate_idx;
+    uint8_t mismatch;          // joint stereo with channels on different window sequences (stereo.rs:503-505)
+    uint8_t scfsi[2];          // bit g: group g of granule 1 repeats granule 0's scale factors
+    uint8_t reserved;
+    GcSide gc[2][2];
+};
+
+// bitstream.rs:57-236
+SYMGPU_HD bool read_side_info(Bits& bs, const symgpu::packet::MpaHeader& h, const uint16_t* long_edges, FrameSide& f) {
+    using symgpu::packet::MpaVersion;
+    const bool mpeg1 = h.version == MpaVersion::Mpeg1;
+    const int n_ch = h.n_channels(), n_gr = h.n_granules();
+    uint32_t v;
+    if (mpeg1) {
+        if (!bs.read(9, v)) return false;
+        f.main_data_begin = uint16_t(v);
+        if (!bs.skip(n_ch == 1 ? 5 : 3)) return false;
+        for (int ch = 0; ch < n_ch; ++ch) {
+            if (!bs.read(4, v)) return false;
+            f.scfsi[ch] = uint8_t((v >> 3 & 1) | (v >> 1 & 2) | (v << 1 & 4) | (v << 3 & 8));  // first bit read = group 0
+        }
+    } else {
+        if (!bs.read(8, v)) return false;
+        f.main_data_begin = uint16_t(v);
+        if (!bs.skip(n_ch == 1 ? 1 : 2)) return false;
+    }
+    for (int gr = 0; gr < n_gr; ++gr)
+        for (int ch = 0; ch < n_ch; ++ch) {
+            GcSide& c = f.gc[gr][ch];
+            if (!bs.read(12, v)) return false;
+            c.part2_3_length = uint16_t(v);
+            if (!bs.read(9, v)) return false;
+            c.big_values = uint16_t(v);
+            if (c.big_values > 288) return false;
+            if (!bs.read(8, v)) return false;
+            c.global_gain = uint8_t(v);
+            if (!bs.read(mpeg1 ? 4 : 9, v)) return false;
+            c.scalefac_compress = uint16_t(v);
+            if (!bs.read(1, v)) return false;
+            if (v) {  // window switching
+                uint32_t type, mixed;
+                if (!bs.read(2, type) || !bs.read(1, mixed)) return false;
+                if (type == 0) return false;
+                c.block_type = uint8_t(type == 1 ? SYMGPU_MP3_START : type == 2 ? SYMGPU_MP3_SHORT : SYMGPU_MP3_END);
+                c.mixed = type == 2 && mixed;
+                for (int i = 0; i < 2; ++i) {
+                    if (!bs.read(5, v)) return false;
+                    c.table_select[i] = uint8_t(v);
+                }
+                for (int i = 0; i < 3; ++i) {
+                    if (!bs.read(3, v)) return false;
+                    c.subblock_gain[i] = uint8_t(v);
+                }
+                // region0 ends after 36 lines (MPEG-1, and short blocks of MPEG-2), 54 (MPEG-2 long transitions), or,
+                // for MPEG-2.5, after 6 (pure short) / 8 long bands of the rate's table (bitstream.rs:108-150)
+                if (h.version == MpaVersion::Mpeg2p5) c.region1_start = long_edges[type == 2 && !mixed ? 6 : 8];
+                else c.region1_start = (mpeg1 || type == 2) ? 36 : 54;
+                c.region2_start = 576;
+            } else {
+                c.block_type = SYMGPU_MP3_LONG;
+                for (int i = 0; i < 3; ++i) {
+                    if (!bs.read(5, v)) return false;
+                    c.table_select[i] = uint8_t(v);
+                }
+                uint32_t r0, r1;
+                if (!bs.read(4, r0) || !bs.read(3, r1)) return false;
+                const unsigned a = r0 + 1, b = r1 + a + 1;
+                c.region1_start = long_edges[a];
+                c.region2_start = b <= 22 ? long_edges[b] : 576;
+            }
+            if (mpeg1) {
+                if (!bs.read(1, v)) return false;
+                c.preflag = uint8_t(v);
+            }
+            if (!bs.read(1, v)) return false;
+            c.scalefac_scale = uint8_t(v);
+            if (!bs.read(1, v)) return false;
+            c.count1table = uint8_t(v);
+        }
+    return true;
+}
+
+// The side read of a packet that passed the prologue and the layer check: `side` = the packet + at, `bytes` long.  Fills
+// the whole record; state kSideBad where the read fails (the reference then empties the reservoir).
+SYMGPU_HD void read_frame_side(const uint8_t* side, uint32_t at, uint32_t bytes, const symgpu::packet::MpaHeader& h, const LongEdges& E,
+                               FrameSide& f) {
+    using symgpu::packet::MpaMode;
+    f = FrameSide{};
+    f.body_at = at, f.body_bytes = bytes;
+    f.n_ch = uint8_t(h.n_channels()), f.n_gr = uint8_t(h.n_granules()), f.mpeg1 = h.version == symgpu::packet::MpaVersion::Mpeg1;
+    f.intensity = h.mode == MpaMode::JointStereo && h.intensity;
+    f.side_len = uint8_t(h.side_info_len());
+    f.sample_rate_idx = h.sample_rate_idx;
+    const bool mid_side = h.mode == MpaMode::JointStereo && h.mid_side;
+    f.unit_flags = uint8_t((f.mpeg1 ? SYMGPU_MP3_F_MPEG1 : 0) | (mid_side ? SYMGPU_MP3_F_MID_SIDE : 0) | (f.intensity ? SYMGPU_MP3_F_INTENSITY : 0));
+    Bits bs(side, bytes);
+    // (side_len > bytes cannot happen for a frame of the right size; the reference would panic slicing)
+    if (!read_side_info(bs, h, E.e[h.sample_rate_idx], f) || f.side_len > bytes) {
+        f.state = kSideBad;
+        return;
+    }
+    f.state = kSideOk;
+    // a joint-stereo pair must share its window sequence: the reference refuses the frame in its stereo stage, after the
+    // main data was read (stereo.rs:503-505)
+    if (f.n_ch == 2 && (mid_side || f.intensity))
+        for (int gr = 0; gr < f.n_gr; ++gr) {
+            const GcSide &a = f.gc[gr][0], &b = f.gc[gr][1];
+            if (a.block_type != b.block_type || (a.block_type == SYMGPU_MP3_SHORT && a.mixed != b.mixed)) f.mismatch = 1;
+        }
+}
+
+// ---- one step of the bit reservoir (BitResevoir::fill / consume, layer3/mod.rs:42-108, :272-370) ------------------------
+// The reservoir as byte counts: `len` bytes held, `consumed` of them read; md_at = where the next frame's main data goes in
+// the compacted stream md.  A frame's reservoir window is the `reuse` bytes main_data_begin reaches back to (at most what
+// is unread) plus its own slot: one contiguous range of md.
+struct Reservoir {
+    uint32_t len, consumed;
+    uint64_t md_at;
+};
+enum : int { kStepDecoded = 0, kStepRefused = 1, kStepFailed = 2, kStepLeftOut = 3 };
+struct StepOut {
+    uint64_t copy_at;      // where the frame's slot goes in md (kStepDecoded, kStepLeftOut)
+    uint32_t slot;         // its main-data bytes in this packet
+    uint32_t reuse;        // bytes of the window that come from earlier frames
+    uint32_t underflow;    // main_data_begin pointed this many bytes before what the reservoir holds
+    uint32_t used;         // bytes of the window the frame's granules take
+};
+
+// One packet's effect on the reservoir.  bad: 0, 1 = its main data is known to over-read (the reference drops the frame
+// and empties the reservoir), 2 = left out although its main data is consumed (the device path passes 2 for s.mismatch).
+//   kStepRefused  the prologue refused the packet (nothing changes); the side read failed (the reservoir is emptied);
+//                 main_data_begin + slot > 2048 (refused before the reservoir is touched, mod.rs:49-51)
+//   kStepFailed   bad == 1: the reservoir is emptied (mod.rs:409-414)
+//   kStepLeftOut  the reservoir moves on as for a decoded frame; the frame yields no audio
+//   kStepDecoded  a frame
+// For kStepDecoded and kStepLeftOut, jobs[0..3] (when not null) are the frame's four granule-channels, unit slots
+// out_frame * 4 + granule * 2 + channel, seg_begin in md.
+SYMGPU_HD int reservoir_step(Reservoir& r, const FrameSide& s, uint8_t bad, uint32_t out_frame, GcJob* jobs, StepOut& o) {
+    if (s.state == kSideRefused) return kStepRefused;
+    if (s.state == kSideBad) {
+        r.len = r.consumed = 0;
+        return kStepRefused;
+    }
+    const uint32_t slot = s.body_bytes - s.side_len, begin = s.main_data_begin;
+    if (begin + slot > 2048) return kStepRefused;
+    if (bad == 1) {
+        r.len = r.consumed = 0;
+        return kStepFailed;
+    }
+    const uint32_t unread = r.len - r.consumed;
+    const uint32_t reuse = begin <= unread ? begin : unread;
+    o.copy_at = r.md_at, o.slot = slot, o.reuse = reuse, o.underflow = begin - reuse;
+    const uint64_t seg_begin = r.md_at - reuse;
+    const uint32_t seg_len = reuse + slot;
+    r.md_at += slot;
+    r.len = seg_len, r.consumed = 0;
+    const uint32_t underflow_bits = 8 * o.underflow;
+    uint32_t skipped = 0, gr0_begin[2] = {~0u, ~0u};
+    uint32_t part_begin = 0;
+    for (int gr = 0; gr < 2; ++gr) {
+        const bool silent = gr < s.n_gr && skipped < underflow_bits;
+        for (int ch = 0; ch < 2; ++ch) {
+            GcJob j{};
+            j.seg_begin = seg_begin, j.seg_len = seg_len, j.out_index = out_frame * 4 + uint32_t(gr * 2 + ch);
+            j.unit_flags = s.unit_flags, j.sample_rate_idx = s.sample_rate_idx, j.mpeg1 = s.mpeg1, j.gr0_bit_begin = ~0u;
+            if (gr >= s.n_gr || ch >= s.n_ch) {
+                j.kind = kJobMute;
+            } else {
+                const GcSide& c = s.gc[gr][ch];
+                j.side = c;
+                j.intensity_channel = ch > 0 && s.intensity, j.scfsi = s.scfsi[ch];
+                if (silent) {
+                    j.kind = kJobSilent;
+                    skipped += c.part2_3_length;
+                } else {
+                    j.kind = kJobDecode;
+                    j.bit_begin = part_begin;
+                    if (gr == 0) gr0_begin[ch] = j.bit_begin;
+                    else {
+                        j.gr0_bit_begin = gr0_begin[ch];
+                        j.gr0_scalefac_compress = s.gc[0][ch].scalefac_compress, j.gr0_block_type = s.gc[0][ch].block_type, j.gr0_mixed = s.gc[0][ch].mixed;
+                    }
+                    part_begin += c.part2_3_length;
+                }
+            }
+            if (jobs) jobs[gr * 2 + ch] = j;
+        }
+        if (silent && skipped > underflow_bits) part_begin = skipped - underflow_bits;
+    }
+    o.used = (part_begin + 7) >> 3;
+    r.consumed = r.len < o.used ? r.len : o.used;
+    return bad == 2 ? kStepLeftOut : kStepDecoded;
+}
+
 }  // namespace mp3e
 
 // The flat tables (host memory, built once; thread-safe).  `words` = length of lut.
 const mp3e::HuffSet& mp3_huffset_host(size_t* words);
+// The long-block band edges of every sample rate (host memory, built once from tables.cpp; thread-safe).
+const mp3e::LongEdges& mp3_long_edges_host();
+#ifdef __CUDACC__
+// The same Huffman tables with `lut` in global memory of `device`, uploaded once per device (mp3_entropy_kernel.cu).
+cudaError_t device_huffset(int device, mp3e::HuffSet& out);
+#endif
 
 }  // namespace symgpu

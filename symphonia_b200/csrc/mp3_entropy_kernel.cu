@@ -36,7 +36,9 @@ struct DeviceLut {
 };
 DeviceLut g_lut;
 
-cudaError_t device_huffset(int device, HuffSet& out) {
+}  // namespace
+
+cudaError_t symgpu::device_huffset(int device, HuffSet& out) {
     if (device < 0 || device >= 64) return cudaErrorInvalidDevice;
     size_t words = 0;
     const HuffSet& host = symgpu::mp3_huffset_host(&words);
@@ -54,15 +56,13 @@ cudaError_t device_huffset(int device, HuffSet& out) {
     return cudaSuccess;
 }
 
-}  // namespace
-
 extern "C" symgpu_status symgpu_mp3_entropy_dev(symgpu_ctx* ctx, const uint8_t* d_md, size_t md_len, const symgpu_mp3_gc_job* d_jobs, size_t n_jobs,
                                                 symgpu_mp3_gc* d_units, int16_t* d_quant, uint32_t* d_failed) {
     if (!ctx || (n_jobs && (!d_jobs || !d_units || !d_quant || !d_failed)) || (!d_md && md_len) || n_jobs > 0xffffffffull) return SYMGPU_ERR_ARG;
     if (n_jobs == 0) return SYMGPU_OK;
     DeviceGuard guard(ctx->device);
     HuffSet hs;
-    CU(ctx, device_huffset(ctx->device, hs));
+    CU(ctx, symgpu::device_huffset(ctx->device, hs));
     const unsigned block = 128, grid = unsigned((n_jobs + block - 1) / block);
     mp3_entropy_kernel<<<grid, block, 0, ctx->stream>>>(d_md, reinterpret_cast<const GcJob*>(d_jobs), uint32_t(n_jobs), hs, d_units, d_quant, d_failed);
     ctx->launches += 1;

@@ -23,7 +23,6 @@ namespace {
 #include "mp3_huffman_data.inc"
 
 using symgpu::packet::MpaHeader;
-using symgpu::packet::MpaVersion;
 
 // ---------------------------------------------------------------------------------------------- Huffman tables
 // Two-level direct lookup: the first kFirstBits bits of the window select either a finished entry or a second-level
@@ -83,120 +82,39 @@ const HostTables& host_tables() {
     return t;
 }
 
-// ---------------------------------------------------------------------------------------------- frame data
-using symgpu::mp3e::Bits;
-using symgpu::mp3e::GcSide;
-
-struct Frame {
-    unsigned main_data_begin;
-    unsigned scfsi[2];  // bit g: group g of granule 1 repeats granule 0's scale factors
-    GcSide gc[2][2];
-    uint8_t scalefacs[2][2][39];
-    uint16_t rzero[2][2];
-};
-
-// bitstream.rs:57-236
-bool read_side_info(Bits& bs, const MpaHeader& h, Frame& f) {
-    const bool mpeg1 = h.version == MpaVersion::Mpeg1;
-    const int n_ch = h.n_channels(), n_gr = h.n_granules();
-    const uint16_t* long_edges = symgpu::mp3_tables_host().edges[h.sample_rate_idx][symgpu::kKindLong];
-    uint32_t v;
-    if (mpeg1) {
-        if (!bs.read(9, v)) return false;
-        f.main_data_begin = v;
-        if (!bs.skip(n_ch == 1 ? 5 : 3)) return false;
-        for (int ch = 0; ch < n_ch; ++ch) {
-            if (!bs.read(4, v)) return false;
-            f.scfsi[ch] = (v >> 3 & 1) | (v >> 1 & 2) | (v << 1 & 4) | (v << 3 & 8);  // first bit read = group 0
-        }
-    } else {
-        if (!bs.read(8, v)) return false;
-        f.main_data_begin = v;
-        if (!bs.skip(n_ch == 1 ? 1 : 2)) return false;
-    }
-    for (int gr = 0; gr < n_gr; ++gr)
-        for (int ch = 0; ch < n_ch; ++ch) {
-            GcSide& c = f.gc[gr][ch];
-            if (!bs.read(12, v)) return false;
-            c.part2_3_length = uint16_t(v);
-            if (!bs.read(9, v)) return false;
-            c.big_values = uint16_t(v);
-            if (c.big_values > 288) return false;
-            if (!bs.read(8, v)) return false;
-            c.global_gain = uint8_t(v);
-            if (!bs.read(mpeg1 ? 4 : 9, v)) return false;
-            c.scalefac_compress = uint16_t(v);
-            if (!bs.read(1, v)) return false;
-            if (v) {  // window switching
-                uint32_t type, mixed;
-                if (!bs.read(2, type) || !bs.read(1, mixed)) return false;
-                if (type == 0) return false;
-                c.block_type = uint8_t(type == 1 ? SYMGPU_MP3_START : type == 2 ? SYMGPU_MP3_SHORT : SYMGPU_MP3_END);
-                c.mixed = type == 2 && mixed;
-                for (int i = 0; i < 2; ++i) {
-                    if (!bs.read(5, v)) return false;
-                    c.table_select[i] = uint8_t(v);
-                }
-                for (int i = 0; i < 3; ++i) {
-                    if (!bs.read(3, v)) return false;
-                    c.subblock_gain[i] = uint8_t(v);
-                }
-                // region0 ends after 36 lines (MPEG-1, and short blocks of MPEG-2), 54 (MPEG-2 long transitions), or,
-                // for MPEG-2.5, after 6 (pure short) / 8 long bands of the rate's table (bitstream.rs:108-150)
-                if (h.version == MpaVersion::Mpeg2p5) c.region1_start = long_edges[type == 2 && !mixed ? 6 : 8];
-                else c.region1_start = (mpeg1 || type == 2) ? 36 : 54;
-                c.region2_start = 576;
-            } else {
-                c.block_type = SYMGPU_MP3_LONG;
-                for (int i = 0; i < 3; ++i) {
-                    if (!bs.read(5, v)) return false;
-                    c.table_select[i] = uint8_t(v);
-                }
-                uint32_t r0, r1;
-                if (!bs.read(4, r0) || !bs.read(3, r1)) return false;
-                const unsigned a = r0 + 1, b = r1 + a + 1;
-                c.region1_start = long_edges[a];
-                c.region2_start = b <= 22 ? long_edges[b] : 576;
-            }
-            if (mpeg1) {
-                if (!bs.read(1, v)) return false;
-                c.preflag = uint8_t(v);
-            }
-            if (!bs.read(1, v)) return false;
-            c.scalefac_scale = uint8_t(v);
-            if (!bs.read(1, v)) return false;
-            c.count1table = uint8_t(v);
-        }
-    return true;
-}
+// ---------------------------------------------------------------------------------------------- packet prologue
+using symgpu::mp3e::FrameSide;
+using symgpu::mp3e::GcJob;
 
 // decoder.rs:84-131: synchronise inside the packet, parse, insist that the packet is exactly one frame of the stream's
-// signal specification (fixed by the first packet ever shown, good or bad) and of Layer III; skip the CRC.
+// signal specification (fixed by the first packet whose header passes) and of Layer III, skip the CRC; then the side
+// information (mp3_entropy.h, the code the device runs).  s.state says how far the packet got.
 struct Spec {
     bool have = false;
     uint32_t rate = 0;
     int channels = 0;
 };
-symgpu_status open_packet(Spec& spec, const uint8_t* frame, size_t n, MpaHeader& h, const uint8_t*& buf, size_t& buf_len) {
-    using namespace symgpu::packet;
+symgpu_status open_frame(Spec& spec, const uint8_t* frame, size_t n, FrameSide& s) {
+    using namespace symgpu::mp3e;
+    s = FrameSide{};
+    MpaHeader h{};
     size_t q = 0;
-    uint32_t word = 0;
-    for (;; ++q) {
-        if (q + 4 > n) return SYMGPU_ERR_DECODE;
-        word = detail::be32(frame + q);
-        if (mpa_is_synced(word) && mpa_check_header(word)) break;
-    }
-    const Status hs = mpa_parse_header(word, h);
-    if (hs != Status::Ok) return hs == Status::Unsupported ? SYMGPU_ERR_UNSUPPORTED : SYMGPU_ERR_DECODE;
-    const size_t body_len = n - q - 4;
-    if (h.frame_size != body_len) return SYMGPU_ERR_DECODE;
+    const int hs = read_header(frame, n, h, q);
+    if (hs != kDecoded) return hs == kUnsupported ? SYMGPU_ERR_UNSUPPORTED : SYMGPU_ERR_DECODE;
     if (!spec.have) spec.have = true, spec.rate = h.sample_rate, spec.channels = h.n_channels();
     else if (spec.rate != h.sample_rate || spec.channels != h.n_channels()) return SYMGPU_ERR_DECODE;
-    if (h.layer != 3) return SYMGPU_ERR_DECODE;
-    const size_t crc_len = h.crc ? 2 : 0;
-    if (body_len < crc_len) return SYMGPU_ERR_DECODE;
-    buf = frame + q + 4 + crc_len, buf_len = body_len - crc_len;
+    uint32_t at = 0, bytes = 0;
+    if (!body_of(h, 3, n, q, at, bytes)) return SYMGPU_ERR_DECODE;
+    read_frame_side(frame + at, at, bytes, h, symgpu::mp3_long_edges_host(), s);
     return SYMGPU_OK;
+}
+
+void frame_info(const FrameSide& s, const symgpu::mp3e::StepOut& o, symgpu_mp3_frame_info* info) {
+    static const uint32_t rates[9] = {44100, 48000, 32000, 22050, 24000, 16000, 11025, 12000, 8000};
+    *info = symgpu_mp3_frame_info{};
+    info->sample_rate = rates[s.sample_rate_idx], info->channels = s.n_ch, info->granules = s.n_gr;
+    info->sample_rate_idx = s.sample_rate_idx, info->version = uint8_t(s.mpeg1 ? 0 : s.sample_rate_idx < 6 ? 1 : 2);
+    info->underflow_bytes = o.underflow, info->main_data_bytes = o.used;
 }
 
 }  // namespace
@@ -207,6 +125,16 @@ struct symgpu_mp3_fe {
     Spec spec;
     void clear() { len = consumed = 0; }
 };
+
+const symgpu::mp3e::LongEdges& symgpu::mp3_long_edges_host() {
+    static const mp3e::LongEdges E = [] {
+        mp3e::LongEdges e{};
+        for (int r = 0; r < 9; ++r)
+            for (int k = 0; k < 23; ++k) e.e[r][k] = mp3_tables_host().edges[r][kKindLong][k];
+        return e;
+    }();
+    return E;
+}
 
 const symgpu::mp3e::HuffSet& symgpu::mp3_huffset_host(size_t* words) {
     if (words) *words = host_tables().lut.size();
@@ -226,94 +154,29 @@ extern "C" void symgpu_mp3_fe_reset(symgpu_mp3_fe* fe) {
 
 extern "C" symgpu_status symgpu_mp3_fe_decode(symgpu_mp3_fe* fe, const uint8_t* frame, size_t n, symgpu_mp3_gc* units, int16_t* quant,
                                               symgpu_mp3_frame_info* info) {
-    using namespace symgpu::packet;
+    using namespace symgpu::mp3e;
     if (!fe || (!frame && n) || !units || !quant) return SYMGPU_ERR_ARG;
-    MpaHeader h{};
-    const uint8_t* buf = nullptr;
-    size_t buf_len = 0;
+    FrameSide s;
     {
-        const symgpu_status hs = open_packet(fe->spec, frame, n, h, buf, buf_len);
+        const symgpu_status hs = open_frame(fe->spec, frame, n, s);
         if (hs != SYMGPU_OK) return hs;
     }
-    Frame f{};
-    Bits side(buf, buf_len);
-    if (!read_side_info(side, h, f)) return fe->clear(), SYMGPU_ERR_DECODE;
-    const size_t side_len = h.side_info_len();
-    if (side_len > buf_len) return fe->clear(), SYMGPU_ERR_DECODE;  // (the reference would panic slicing; cannot happen for a sized frame)
-
-    // BitResevoir::fill (mod.rs:42-95)
-    const uint8_t* md = buf + side_len;
-    const size_t md_len = buf_len - side_len, begin = f.main_data_begin;
-    if (begin + md_len > sizeof fe->reservoir) return SYMGPU_ERR_DECODE;  // returned before anything changes, reservoir kept
-    const size_t unread = fe->len - fe->consumed;
-    uint32_t underflow = 0;
-    if (begin <= unread) {
-        std::memmove(fe->reservoir, fe->reservoir + fe->len - begin, begin);
-        std::memcpy(fe->reservoir + begin, md, md_len);
-        fe->len = begin + md_len;
-    } else {
-        std::memmove(fe->reservoir, fe->reservoir + fe->len - unread, unread);
-        std::memcpy(fe->reservoir + unread, md, md_len);
-        fe->len = unread + md_len;
-        underflow = uint32_t(begin - unread);
+    // the reservoir step of the plan (mp3_entropy.h), then its jobs run in order against the reservoir's bytes
+    Reservoir r{uint32_t(fe->len), uint32_t(fe->consumed), fe->len};
+    GcJob jobs[4];
+    StepOut o{};
+    if (reservoir_step(r, s, 0, 0, jobs, o) != kStepDecoded) return fe->len = r.len, fe->consumed = r.consumed, SYMGPU_ERR_DECODE;
+    std::memmove(fe->reservoir, fe->reservoir + fe->len - o.reuse, o.reuse);  // BitResevoir::fill (mod.rs:42-95)
+    std::memcpy(fe->reservoir + o.reuse, frame + s.body_at + s.side_len, o.slot);
+    fe->len = r.len, fe->consumed = r.consumed;
+    const HuffSet& hs = host_tables().set;
+    int failed = 0;
+    for (int k = 0; k < 4; ++k) {
+        jobs[k].seg_begin = 0;
+        failed |= decode_gc_job(jobs[k], fe->reservoir, hs, units + k, quant + k * 576);
     }
-    fe->consumed = 0;
-
-    // read_main_data (mod.rs:272-370)
-    const int n_ch = h.n_channels(), n_gr = h.n_granules();
-    const bool mpeg1 = h.version == MpaVersion::Mpeg1;
-    const bool intensity = h.mode == MpaMode::JointStereo && h.intensity;
-    const uint32_t underflow_bits = 8 * underflow;
-    size_t part_begin = 0;
-    uint32_t skipped = 0;
-    std::memset(quant, 0, 4 * 576 * sizeof(int16_t));
-    for (int gr = 0; gr < n_gr; ++gr) {
-        if (skipped < underflow_bits) {  // the granule's bits are (partly) in frames never seen: silence it
-            for (int ch = 0; ch < n_ch; ++ch) skipped += f.gc[gr][ch].part2_3_length;
-            if (skipped > underflow_bits) part_begin = skipped - underflow_bits;
-            continue;
-        }
-        for (int ch = 0; ch < n_ch; ++ch) {
-            if ((part_begin >> 3) > fe->len) return fe->clear(), SYMGPU_ERR_DECODE;
-            Bits bs(fe->reservoir, fe->len, part_begin);
-            if (bs.at > bs.n_bits) return fe->clear(), SYMGPU_ERR_DECODE;
-            GcSide& c = f.gc[gr][ch];
-            const int part2 = mpeg1 ? symgpu::mp3e::read_scale_factors_mpeg1(bs, c, gr ? f.scalefacs[0][ch] : nullptr, f.scfsi[ch], f.scalefacs[gr][ch])
-                                    : symgpu::mp3e::read_scale_factors_mpeg2(bs, ch > 0 && intensity, c, &c.preflag, f.scalefacs[gr][ch]);
-            if (part2 < 0 || uint32_t(part2) > c.part2_3_length) return fe->clear(), SYMGPU_ERR_DECODE;
-            const int rz = symgpu::mp3e::read_huffman(bs, host_tables().set, c, uint32_t(c.part2_3_length) - uint32_t(part2), quant + (gr * 2 + ch) * 576);
-            if (rz < 0) return fe->clear(), SYMGPU_ERR_DECODE;
-            f.rzero[gr][ch] = uint16_t(rz);
-            part_begin += c.part2_3_length;
-        }
-    }
-    const size_t used = (part_begin + 7) >> 3;
-    fe->consumed = std::min(fe->len, fe->consumed + used);
-
-    // GranuleChannel -> symgpu_mp3_gc
-    const uint8_t frame_flags = uint8_t((mpeg1 ? SYMGPU_MP3_F_MPEG1 : 0) | (h.mode == MpaMode::JointStereo && h.mid_side ? SYMGPU_MP3_F_MID_SIDE : 0) |
-                                        (intensity ? SYMGPU_MP3_F_INTENSITY : 0));
-    for (int gr = 0; gr < 2; ++gr)
-        for (int ch = 0; ch < 2; ++ch) {
-            symgpu_mp3_gc& u = units[gr * 2 + ch];
-            std::memset(&u, 0, sizeof u);
-            u.sample_rate_idx = h.sample_rate_idx;
-            if (gr >= n_gr || ch >= n_ch) {
-                u.flags = uint8_t(frame_flags | SYMGPU_MP3_F_MUTE);
-                continue;
-            }
-            const GcSide& c = f.gc[gr][ch];
-            u.rzero = f.rzero[gr][ch], u.global_gain = c.global_gain, u.block_type = c.block_type;
-            u.flags = uint8_t(frame_flags | (c.mixed ? SYMGPU_MP3_F_MIXED : 0) | (c.scalefac_scale ? SYMGPU_MP3_F_SCALEFAC_SCALE : 0) |
-                              (c.preflag ? SYMGPU_MP3_F_PREFLAG : 0) | ((c.scalefac_compress & 1) ? SYMGPU_MP3_F_SFC_LSB : 0));
-            std::memcpy(u.subblock_gain, c.subblock_gain, 3);
-            std::memcpy(u.scalefacs, f.scalefacs[gr][ch], 39);
-        }
-    if (info) {
-        info->sample_rate = h.sample_rate, info->channels = uint8_t(n_ch), info->granules = uint8_t(n_gr);
-        info->sample_rate_idx = h.sample_rate_idx, info->version = uint8_t(h.version);
-        info->underflow_bytes = underflow, info->main_data_bytes = uint32_t(used);
-    }
+    if (failed) return fe->clear(), SYMGPU_ERR_DECODE;
+    if (info) frame_info(s, o, info);
     return SYMGPU_OK;
 }
 
@@ -343,86 +206,26 @@ extern "C" symgpu_status symgpu_mp3_entropy_plan(const uint8_t* data, size_t n, 
     if ((!data && n) || (n_packets && !packets) || !md_len || !n_good || (!md && md_cap)) return SYMGPU_ERR_ARG;
     GcJob* jobs = reinterpret_cast<GcJob*>(jobs_out);
     Spec spec;
-    size_t len = 0, consumed = 0;  // the reservoir, as byte counts only
-    size_t md_at = 0, good = 0;
+    Reservoir r{0, 0, 0};  // the reservoir, as byte counts only
+    size_t good = 0;
     for (size_t i = 0; i < n_packets; ++i) {
         if (packets[i].offset > n || packets[i].size > n - packets[i].offset) return SYMGPU_ERR_ARG;
-        MpaHeader h{};
-        const uint8_t* buf = nullptr;
-        size_t buf_len = 0;
-        if (open_packet(spec, data + packets[i].offset, packets[i].size, h, buf, buf_len) != SYMGPU_OK) continue;
-        Frame f{};
-        Bits side(buf, buf_len);
-        const size_t side_len = h.side_info_len();
-        if (!read_side_info(side, h, f) || side_len > buf_len) {
-            len = consumed = 0;
-            continue;
-        }
-        const size_t slot = buf_len - side_len, begin = f.main_data_begin;
-        if (begin + slot > 2048) continue;  // refused before the reservoir is touched (mod.rs:49-51)
-        const size_t unread = len - consumed;
-        const size_t reuse = begin <= unread ? begin : unread;
-        const uint32_t underflow = uint32_t(begin - reuse);
-        if (bad && bad[i] == 1) {  // known to fail while its main data is read: the reference then empties the reservoir (mod.rs:409-414)
-            len = consumed = 0;
-            continue;
-        }
-        const bool leave_out = bad && bad[i] == 2;  // refused AFTER its main data was read (stereo.rs:503-505): the reservoir moves on, no audio
-        if (md_at + slot > md_cap) return SYMGPU_ERR_LIMIT;
-        if (md) std::memcpy(md + md_at, buf + side_len, slot);
-        const uint64_t seg_begin = md_at - reuse;
-        const uint32_t seg_len = uint32_t(reuse + slot);
-        md_at += slot;
-        len = seg_len, consumed = 0;
-
-        const int n_ch = h.n_channels(), n_gr = h.n_granules();
-        const bool mpeg1 = h.version == MpaVersion::Mpeg1;
-        const bool intensity = h.mode == symgpu::packet::MpaMode::JointStereo && h.intensity;
-        const uint8_t frame_flags = uint8_t((mpeg1 ? SYMGPU_MP3_F_MPEG1 : 0) | (h.mode == symgpu::packet::MpaMode::JointStereo && h.mid_side ? SYMGPU_MP3_F_MID_SIDE : 0) |
-                                            (intensity ? SYMGPU_MP3_F_INTENSITY : 0));
-        const uint32_t underflow_bits = 8 * underflow;
-        uint32_t skipped = 0, gr0_begin[2] = {~0u, ~0u};
-        size_t part_begin = 0;
-        for (int gr = 0; gr < 2; ++gr) {
-            const bool silent = gr < n_gr && skipped < underflow_bits;
-            for (int ch = 0; ch < 2; ++ch) {
-                GcJob j{};
-                j.seg_begin = seg_begin, j.seg_len = seg_len, j.out_index = uint32_t(good * 4 + gr * 2 + ch);
-                j.unit_flags = frame_flags, j.sample_rate_idx = h.sample_rate_idx, j.mpeg1 = mpeg1, j.gr0_bit_begin = ~0u;
-                if (gr >= n_gr || ch >= n_ch) {
-                    j.kind = kJobMute;
-                } else {
-                    j.side = f.gc[gr][ch];
-                    j.intensity_channel = ch > 0 && intensity, j.scfsi = uint8_t(f.scfsi[ch]);
-                    if (silent) {
-                        j.kind = kJobSilent;
-                        skipped += f.gc[gr][ch].part2_3_length;
-                    } else {
-                        j.kind = kJobDecode;
-                        j.bit_begin = uint32_t(part_begin);
-                        if (gr == 0) gr0_begin[ch] = j.bit_begin;
-                        else {
-                            j.gr0_bit_begin = gr0_begin[ch];
-                            j.gr0_scalefac_compress = f.gc[0][ch].scalefac_compress, j.gr0_block_type = f.gc[0][ch].block_type, j.gr0_mixed = f.gc[0][ch].mixed;
-                        }
-                        part_begin += f.gc[gr][ch].part2_3_length;
-                    }
-                }
-                if (jobs && !leave_out) jobs[good * 4 + gr * 2 + ch] = j;
-            }
-            if (silent && skipped > underflow_bits) part_begin = skipped - underflow_bits;
-        }
-        consumed = std::min(len, (part_begin + 7) >> 3);
-        if (leave_out) continue;
-        if (good == 0 && info) {
-            info->sample_rate = h.sample_rate, info->channels = uint8_t(n_ch), info->granules = uint8_t(n_gr);
-            info->sample_rate_idx = h.sample_rate_idx, info->version = uint8_t(h.version), info->underflow_bytes = underflow;
-            info->main_data_bytes = uint32_t((part_begin + 7) >> 3);
-        }
+        const uint8_t* frame = data + packets[i].offset;
+        FrameSide s;
+        if (open_frame(spec, frame, packets[i].size, s) != SYMGPU_OK) continue;
+        GcJob four[4];
+        StepOut o{};
+        const int step = reservoir_step(r, s, bad ? bad[i] : 0, uint32_t(good), four, o);
+        if (step != kStepDecoded && step != kStepLeftOut) continue;
+        if (o.copy_at + o.slot > md_cap) return SYMGPU_ERR_LIMIT;
+        if (md) std::memcpy(md + o.copy_at, frame + s.body_at + s.side_len, o.slot);
+        if (step == kStepLeftOut) continue;  // refused AFTER its main data was read (stereo.rs:503-505): the reservoir moves on, no audio
+        if (jobs) std::memcpy(jobs + good * 4, four, sizeof four);
+        if (good == 0 && info) frame_info(s, o, info);
         if (frame_of) frame_of[good] = uint32_t(i);
         ++good;
     }
-    *md_len = md_at, *n_good = good;
+    *md_len = r.md_at, *n_good = good;
     return SYMGPU_OK;
 }
 

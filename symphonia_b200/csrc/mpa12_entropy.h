@@ -44,7 +44,12 @@ struct Constants {
 };
 const Constants& host_constants();  // host only
 
-enum : int { kDecoded = 0, kRefused = 1, kUnsupported = 2 };
+// The packet prologue is shared with Layer III (mp3_entropy.h).
+using symgpu::mp3e::body_of;
+using symgpu::mp3e::kDecoded;
+using symgpu::mp3e::kRefused;
+using symgpu::mp3e::kUnsupported;
+using symgpu::mp3e::read_header;
 
 // What the side read leaves for the sample codewords of one frame.  404 bytes.
 struct Side {
@@ -111,31 +116,6 @@ SYMGPU_HD int table_of(const MpaHeader& h) {
 SYMGPU_HD int32_t centre(uint32_t raw, unsigned bits) {  // invert the top bit, sign-extend: offset binary -> two's complement
     const uint32_t inv = raw ^ (1u << (bits - 1));
     return int32_t(inv << (32 - bits)) >> (32 - bits);
-}
-
-// ---- packet prologue (decoder.rs:87-128), in the reference's order --------------------------------------------------------
-// 1. read_header: the sync search inside the packet, the header parse, frame_size == the bytes after the header word.
-// 2. (the caller) the signal specification: the first packet that passes 1 fixes (sample rate, channels); a later packet
-//    that differs is refused.  So a packet of the wrong layer but the right size still fixes it.
-// 3. body_of: the layer check, the CRC skip.
-SYMGPU_HD int read_header(const uint8_t* frame, size_t n, MpaHeader& h, size_t& q) {
-    using namespace symgpu::packet;
-    uint32_t word = 0;
-    for (q = 0;; ++q) {  // decoder.rs:87: synchronise inside the packet
-        if (q + 4 > n) return kRefused;
-        word = detail::be32(frame + q);
-        if (mpa_is_synced(word) && mpa_check_header(word)) break;
-    }
-    const Status hs = mpa_parse_header(word, h);
-    if (hs != Status::Ok) return hs == Status::Unsupported ? kUnsupported : kRefused;
-    return h.frame_size == n - q - 4 ? kDecoded : kRefused;
-}
-SYMGPU_HD bool body_of(const MpaHeader& h, int layer, size_t n, size_t q, uint32_t& at, uint32_t& bytes) {
-    if (h.layer != layer) return false;
-    const size_t body_len = n - q - 4, crc_len = h.crc ? 2 : 0;
-    if (body_len < crc_len) return false;
-    at = uint32_t(q + 4 + crc_len), bytes = uint32_t(body_len - crc_len);
-    return true;
 }
 
 // ---- side read ---------------------------------------------------------------------------------------------------------

@@ -505,26 +505,41 @@ def decode_flac_files(engine, files, threads=None, device=False, errors=None):
 _TORCH_DTYPES = {nat.FMT_F32: "float32", nat.FMT_S16: "int16", nat.FMT_S24: "int32", nat.FMT_S32: "int32", nat.FMT_U8: "uint8"}
 
 
-def mpa12_files_plan(files, threads=None, errors=None):
-    """Host half of decode_mpa12_files: every file indexed (symgpu_mpa_index, on `threads` host threads), their bytes concatenated
-    once, one job per packet and one group per file (group i uses state slot i).  Returns dict(data, jobs, groups, tracks, out_samples,
-    failed).  A file that cannot be indexed or is not Layer I / II (listed in `failed`) gets a group without jobs; its message goes to
-    errors[i] when `errors` is a dict."""
+def mpa_index_files(files, threads=None):
+    """symgpu_mpa_index of every file on `threads` host threads: [(track, packets) | None], {i: message} for the files that cannot be
+    indexed."""
     import concurrent.futures
     import os
     messages = {}
 
     def index(i):
         try:
-            track, packets = packetizer.mpa_index(files[i])
-            if int(track["layer"]) not in (1, 2):
-                raise ValueError(f"MPEG Layer {int(track['layer'])}: decode_mpa12_files takes Layer I / II files")
-            return track, packets
+            return packetizer.mpa_index(files[i])
         except Exception as e:  # noqa: BLE001 -- one bad file must not abort the batch; its message is kept
             messages[i] = f"{type(e).__name__}: {e}"
             return None
     with concurrent.futures.ThreadPoolExecutor(max_workers=threads or os.cpu_count()) as pool:
         ix = list(pool.map(index, range(len(files))))
+    return ix, messages
+
+
+def _keep_layers(ix, messages, layers, what):
+    """The index with the files of other layers dropped (and their message added)."""
+    ix = list(ix)
+    for i, t in enumerate(ix):
+        if t is not None and int(t[0]["layer"]) not in layers:
+            messages[i] = f"ValueError: MPEG Layer {int(t[0]['layer'])}: {what}"
+            ix[i] = None
+    return ix
+
+
+def mpa12_files_plan(files, threads=None, errors=None, index=None):
+    """Host half of decode_mpa12_files: every file indexed (symgpu_mpa_index, on `threads` host threads), their bytes concatenated
+    once, one job per packet and one group per file (group i uses state slot i).  Returns dict(data, jobs, groups, tracks, out_samples,
+    failed).  A file that cannot be indexed or is not Layer I / II (listed in `failed`) gets a group without jobs; its message goes to
+    errors[i] when `errors` is a dict.  index: the result of mpa_index_files (else computed here)."""
+    ix, messages = mpa_index_files(files, threads) if index is None else (index[0], dict(index[1]))
+    ix = _keep_layers(ix, messages, (1, 2), "decode_mpa12_files takes Layer I / II files")
     if errors is not None:
         errors.update(messages)
     bufs = [np.frombuffer(f, dtype=np.uint8) if not isinstance(f, np.ndarray) else np.ascontiguousarray(f, dtype=np.uint8) for f in files]
@@ -556,14 +571,14 @@ def mpa12_files_plan(files, threads=None, errors=None):
     return dict(data=data, jobs=jobs, groups=groups, tracks=tracks, out_samples=out_at, failed=failed)
 
 
-def decode_mpa12_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False, errors=None):
+def decode_mpa12_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False, errors=None, index=None):
     """[(samples [frames, channels] of `fmt`, sample_rate)] for a list of MPEG Layer I / II files, each equal to
     decode_mpeg_audio(engine, file, fmt): the files are indexed on host threads, and ONE device call decodes every packet of every
     file -- headers, bit allocation, scale factors and samples in device code, synthesis and the output stage on the GPU.
     device=True: the bytes go to the device once and the samples are CUDA tensors, views of one output tensor.  A Layer III file or
     one that cannot be indexed yields an empty result with sample rate 0 (its message in errors[i] when `errors` is a dict).
-    (Re)allocates the engine's MP3 state slots, one per file."""
-    plan = mpa12_files_plan(files, threads, errors)
+    (Re)allocates the engine's MP3 state slots, one per file.  index: the result of mpa_index_files (else computed here)."""
+    plan = mpa12_files_plan(files, threads, errors, index)
     groups, cap = plan["groups"], plan["out_samples"]
     engine.mp3_streams_alloc(max(len(files), 1))
     if device:
@@ -591,4 +606,111 @@ def decode_mpa12_files(engine, files, fmt=nat.FMT_S16, threads=None, device=Fals
             continue
         ch, at, n = int(r["channels"]), int(groups[g]["out_offset"]), int(r["frames"])
         result.append((out[at:at + n * ch].reshape(n, ch), int(r["sample_rate"])))
+    return result
+
+
+# ---- MPEG Layer III, many files decoded on the device (side information, bit reservoir and Huffman data in device code) ---------
+
+def mp3_files_plan(files, threads=None, errors=None, index=None):
+    """Host half of decode_mp3_files: every file indexed (symgpu_mpa_index, on `threads` host threads), their bytes concatenated once,
+    one job per packet and one group per file (group i uses state slot i; granules and channels from the file's track).  Returns
+    dict(data, jobs, groups, tracks, out_samples, failed).  A file that cannot be indexed or is not Layer III (listed in `failed`) gets
+    a group without jobs; its message goes to errors[i] when `errors` is a dict.  index: the result of mpa_index_files."""
+    ix, messages = mpa_index_files(files, threads) if index is None else (index[0], dict(index[1]))
+    ix = _keep_layers(ix, messages, (3,), "decode_mp3_files takes Layer III files")
+    if errors is not None:
+        errors.update(messages)
+    bufs = [np.frombuffer(f, dtype=np.uint8) if not isinstance(f, np.ndarray) else np.ascontiguousarray(f, dtype=np.uint8) for f in files]
+    good = [i for i in range(len(files)) if ix[i] is not None]
+    data = np.concatenate([bufs[i] for i in good]) if good else np.zeros(0, dtype=np.uint8)
+    groups = np.zeros(len(files), dtype=nat.MP3_GROUP_DTYPE)
+    groups["slot"] = np.arange(len(files))
+    groups["granules"], groups["channels"] = 2, 2
+    jobs, byte_at, job_at, out_at = [], 0, 0, 0
+    sat = np.uint64(0xFFFFFFFF)
+    for i in good:
+        track, packets = ix[i]
+        n, granules, channels = len(packets), 2 if int(track["version"]) == 0 else 1, int(track["channels"])
+        g = groups[i]
+        g["out_offset"], g["first_job"], g["n_jobs"], g["granules"], g["channels"] = out_at, job_at, n, granules, channels
+        j = np.zeros(n, dtype=nat.MP3_JOB_DTYPE)
+        j["offset"], j["len"] = packets["offset"] + np.uint64(byte_at), packets["size"]
+        j["trim_start"] = packets["trim_start"]
+        j["trim_end"] = np.minimum(packets["trim_end"].astype(np.uint64), sat)
+        jobs.append(j)
+        byte_at += bufs[i].size
+        job_at += n
+        out_at += n * granules * 576 * channels
+    failed = [i for i in range(len(files)) if ix[i] is None]
+    groups["out_offset"][failed] = out_at
+    groups["first_job"][failed] = job_at
+    jobs = np.concatenate(jobs) if jobs else np.zeros(0, dtype=nat.MP3_JOB_DTYPE)
+    tracks = [None if t is None else t[0] for t in ix]
+    return dict(data=data, jobs=jobs, groups=groups, tracks=tracks, out_samples=out_at, failed=failed)
+
+
+def decode_mp3_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False, errors=None, index=None, stats=None):
+    """[(samples [frames, channels] of `fmt`, sample_rate)] for a list of MP3 (MPEG Layer III) files, each equal to
+    decode_mpeg_audio(engine, file, fmt): the files are indexed on host threads, and ONE device call decodes every packet of every
+    file -- headers, side information, the bit reservoir, scale factors and Huffman data in device code, synthesis and the output
+    stage on the GPU.  device=True: the bytes go to the device once and the samples are CUDA tensors, views of one output tensor.
+    A Layer I / II file or one that cannot be indexed yields an empty result with sample rate 0 (its message in errors[i] when
+    `errors` is a dict).  One deviation from decode_mpeg_audio: a joint-stereo frame whose channels are on different window
+    sequences (which the reference refuses after reading it) is left out whole.  stats: a dict that receives `rounds` and the
+    per-packet `status`.  (Re)allocates the engine's MP3 state slots, one per file.  index: the result of mpa_index_files."""
+    plan = mp3_files_plan(files, threads, errors, index)
+    groups, cap = plan["groups"], plan["out_samples"]
+    engine.mp3_streams_alloc(max(len(files), 1))
+    if device:
+        import torch
+        dev = torch.device("cuda", engine.device)
+        as_t = lambda a: torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(-1)).to(dev)  # noqa: E731
+        out = torch.empty(cap, dtype=getattr(torch, _TORCH_DTYPES[fmt]), device=dev)
+        results_t = torch.empty(len(groups) * nat.MP3_RESULT_DTYPE.itemsize, dtype=torch.uint8, device=dev)
+        status_t = torch.empty(len(plan["jobs"]), dtype=torch.uint8, device=dev)
+        data_t, jobs_t = as_t(plan["data"]), as_t(plan["jobs"])
+        torch.cuda.current_stream(dev).synchronize()  # the copies above are on torch's stream, the decode on the engine's
+        rounds = engine.mp3_decode_dev(data_t, jobs_t, groups, fmt, out, results_t, status_t)
+        engine.sync()
+        results = results_t.cpu().numpy().view(nat.MP3_RESULT_DTYPE)
+        status = status_t.cpu().numpy()
+    else:
+        out, results, status, rounds = engine.mp3_decode_host(plan["data"], plan["jobs"], groups, fmt, cap)
+    if stats is not None:
+        stats.update(rounds=rounds, status=status)
+    result = []
+    for g in range(len(groups)):
+        if g in plan["failed"]:
+            result.append((out[:0].reshape(0, 0), 0))
+            continue
+        r, track = results[g], plan["tracks"][g]
+        if int(r["packets"]) == 0:   # no frame survived: the track's parameters, as decode_mpeg_audio reports them
+            result.append((out[:0].reshape(0, int(track["channels"])), int(track["sample_rate"])))
+            continue
+        ch, at, n = int(r["channels"]), int(groups[g]["out_offset"]), int(r["frames"])
+        result.append((out[at:at + n * ch].reshape(n, ch), int(r["sample_rate"])))
+    return result
+
+
+def decode_mpeg_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False, errors=None):
+    """[(samples [frames, channels] of `fmt`, sample_rate)] for a list of MPEG audio files of any layer, each what
+    decode_mpeg_audio(engine, file, fmt) returns: every file is indexed once, Layer III files go to decode_mp3_files and Layer I / II
+    files to decode_mpa12_files (one device call each).  A file that cannot be indexed yields an empty result with sample rate 0 (its
+    message in errors[i] when `errors` is a dict)."""
+    ix, messages = mpa_index_files(files, threads)
+    if errors is not None:
+        errors.update(messages)
+    result = [None] * len(files)
+    for layers, decode in (((3,), decode_mp3_files), ((1, 2), decode_mpa12_files)):
+        mine = [i for i, t in enumerate(ix) if t is not None and int(t[0]["layer"]) in layers]
+        if mine:
+            got = decode(engine, [files[i] for i in mine], fmt, threads, device, None, ([ix[i] for i in mine], {}))
+            for i, r in zip(mine, got):
+                result[i] = r
+    for i in messages:
+        empty = np.zeros((0, 0), dtype=nat.FMT_NUMPY[fmt])
+        if device:
+            import torch
+            empty = torch.empty((0, 0), dtype=getattr(torch, _TORCH_DTYPES[fmt]), device=torch.device("cuda", engine.device))
+        result[i] = (empty, 0)
     return result
