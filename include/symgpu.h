@@ -810,6 +810,67 @@ symgpu_status symgpu_mp3_decode_dev(symgpu_ctx* ctx, const uint8_t* bytes, size_
                                     const symgpu_mp3_group* groups, size_t n_groups, int format, void* out, size_t out_bytes,
                                     symgpu_mp3_group_result* results, uint8_t* status, uint32_t* n_rounds);
 
+/* AAC-LC decoded on the device, many files per call: raw_data_blocks of file bytes -> interleaved samples of `format`.  The
+ * packet rules are those of symgpu_aac_fe_decode (aac_entropy.h, the same code): one device thread per packet decodes it from
+ * a fresh state, one thread per file walks the packets' records in stream order (element layout, noise generators, window
+ * shapes), the packets that drew noise are decoded again from their real generator states, the pulses' new line values are
+ * computed on the host with the C library's powf (Pulse::synth), and the unchanged symgpu_aac_synth_dev and output stage of
+ * symgpu_pcm_pack_dev follow.
+ *   jobs    one per packet: the raw_data_block's byte range in `bytes` (symgpu_adts_index: offset, size)
+ *   groups  one per file: jobs [first_job, first_job + n_jobs) in stream order, the stream's sample rate and channels (the ADTS
+ *           index's first frame: AdtsReader::try_new).  HOST memory in both variants.
+ *   out     samples of `format`: file g's output starts at groups[g].out_offset (in samples) and holds results[g].frames frames
+ *           of results[g].channels interleaved samples; its region is n_jobs x 1024 x channels samples.
+ *   results one per group;  status  one SYMGPU_AAC_JOB_* per job (a job that no group names is left undecoded: REFUSED).
+ *   n_redecoded  the packets decoded a second time because they drew noise (may be NULL).
+ * A packet is decoded exactly when symgpu_aac_fe_decode_packets decodes it, with the same units, TNS filters and coefficients,
+ * whatever the file's mix of refused packets, layout changes and pulses reading scale factors earlier packets left behind.
+ * Every packet gives 1024 frames; nothing is trimmed.  Each group synthesises in the AAC state slot it names
+ * (symgpu_aac_streams_alloc); the call resets those slots first, and their state after the call is unspecified.  The number of
+ * launches does not depend on the number of files. */
+typedef struct symgpu_aac_group {           /* 24 bytes */
+    uint64_t out_offset;                    /* first sample of the file's output in `out`; a multiple of `channels`              */
+    uint32_t first_job;
+    uint32_t n_jobs;
+    uint32_t sample_rate;                   /* picks the band tables (AacDecoder::try_new); not 0                                */
+    uint16_t slot;                          /* AAC state slot, distinct per group, below the allocated count                     */
+    uint8_t channels;                       /* 1 or 2                                                                           */
+    uint8_t reserved;
+} symgpu_aac_group;
+typedef struct symgpu_aac_group_result {    /* 24 bytes */
+    uint64_t frames;                        /* interleaved frames written to the file's region                                  */
+    uint32_t sample_rate;                   /* the group's                                                                      */
+    uint32_t packets;                       /* packets decoded                                                                  */
+    uint8_t channels;
+    uint8_t reserved[7];
+} symgpu_aac_group_result;
+enum {
+    SYMGPU_AAC_JOB_DECODED = 0,
+    SYMGPU_AAC_JOB_REFUSED = 1,             /* SYMGPU_ERR_DECODE in symgpu_aac_fe_decode, or no group names the job            */
+    SYMGPU_AAC_JOB_UNSUPPORTED = 2,         /* SYMGPU_ERR_UNSUPPORTED: CCE / PCE / predictor data / elements not covering the channels */
+    SYMGPU_AAC_JOB_INVALID = 3              /* device variant only: the job's bytes lie outside `bytes`                          */
+};
+/* Host variant: every pointer is host memory.  Everything is validated before anything is launched: SYMGPU_ERR_ARG for a job
+ * outside `bytes`, a group whose jobs lie outside the table or overlap another group's, channels other than 1 / 2, a sample rate
+ * of 0, an out_offset that is not a multiple of channels, an unknown format, two groups naming one slot; SYMGPU_ERR_LIMIT for a
+ * slot at or above the allocated count or a region that does not fit in `out` (out_bytes).  Stages through the context's
+ * staging buffer and returns when the results are in host memory; samples of `out` outside the written frames are left as they
+ * were. */
+symgpu_status symgpu_aac_decode_host(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_piece* jobs, size_t n_jobs,
+                                     const symgpu_aac_group* groups, size_t n_groups, int format, void* out, size_t out_bytes,
+                                     symgpu_aac_group_result* results, uint8_t* status, uint32_t* n_redecoded);
+/* Device variant: bytes, jobs, out, results and status are device memory, groups and n_redecoded host memory; the groups are
+ * validated on the host as above, and the kernels check each job's byte range (SYMGPU_AAC_JOB_INVALID).  Work is queued on the
+ * context stream; the call waits for the stream once, for an 8-byte readback (the number of pulse records and of packets
+ * decoded twice), and once more when pulse records exist: they come back to the host (at most two per packet, 64 bytes each)
+ * and are copied back to the device without a further wait.  It returns with the synthesis and the output stage still
+ * queued.  Scratch of about 37 KB per job comes from the context's staging buffer; the packet rules' tables (about 90 KB) are
+ * uploaded to the context on its first call.  A call without jobs reports each group's sample rate and channels with 0 frames,
+ * as a call with jobs does for a group without any. */
+symgpu_status symgpu_aac_decode_dev(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_piece* jobs, size_t n_jobs,
+                                    const symgpu_aac_group* groups, size_t n_groups, int format, void* out, size_t out_bytes,
+                                    symgpu_aac_group_result* results, uint8_t* status, uint32_t* n_redecoded);
+
 /* ===================================================================================================
  * MPEG Layer I / II sample decoders (SURVEY 8f N1 for the Layer I / II path): a packet becomes the sub-band samples
  * symgpu_mpa12_synth_* take.  CPU only, stateless apart from the stream's signal specification.

@@ -115,6 +115,12 @@ MP3_GROUP_DTYPE = np.dtype([("out_offset", "<u8"), ("first_job", "<u4"), ("n_job
 MP3_RESULT_DTYPE = np.dtype([("frames", "<u8"), ("sample_rate", "<u4"), ("packets", "<u4"), ("channels", "u1"), ("reserved", "u1", (7,))])
 assert MP3_JOB_DTYPE.itemsize == 24 and MP3_GROUP_DTYPE.itemsize == 24 and MP3_RESULT_DTYPE.itemsize == 24
 MP3_JOB_DECODED, MP3_JOB_REFUSED, MP3_JOB_FAILED, MP3_JOB_LEFT_OUT, MP3_JOB_INVALID = 0, 1, 2, 3, 4
+# device AAC-LC decoding: jobs are PIECE_DTYPE; `symgpu_aac_group`, `symgpu_aac_group_result` (24 bytes each), per-job status
+AAC_GROUP_DTYPE = np.dtype([("out_offset", "<u8"), ("first_job", "<u4"), ("n_jobs", "<u4"), ("sample_rate", "<u4"), ("slot", "<u2"), ("channels", "u1"),
+                            ("reserved", "u1")])
+AAC_RESULT_DTYPE = np.dtype([("frames", "<u8"), ("sample_rate", "<u4"), ("packets", "<u4"), ("channels", "u1"), ("reserved", "u1", (7,))])
+assert AAC_GROUP_DTYPE.itemsize == 24 and AAC_RESULT_DTYPE.itemsize == 24
+AAC_JOB_DECODED, AAC_JOB_REFUSED, AAC_JOB_UNSUPPORTED, AAC_JOB_INVALID = 0, 1, 2, 3
 MP3_FILE_DTYPE = np.dtype([("data", "<u8"), ("n", "<u8"), ("packets", "<u8"), ("n_packets", "<u8"), ("stream", "<u4"), ("reserved", "<u4")])
 assert MP3_FILE_DTYPE.itemsize == 40
 VORBIS_SETUP_INFO_DTYPE = np.dtype([("n_codebooks", "<u4"), ("n_floors", "<u4"), ("n_residues", "<u4"), ("n_mappings", "<u4"), ("n_modes", "<u4"),
@@ -280,7 +286,7 @@ def lib():
         fn = getattr(L, name)
         fn.restype = ctypes.c_int
         fn.argtypes = [vp, vp, sz, vp, sz, vp, sz, ctypes.c_int, vp, sz, vp, vp]
-    for name in ("symgpu_mp3_decode_host", "symgpu_mp3_decode_dev"):
+    for name in ("symgpu_mp3_decode_host", "symgpu_mp3_decode_dev", "symgpu_aac_decode_host", "symgpu_aac_decode_dev"):
         fn = getattr(L, name)
         fn.restype = ctypes.c_int
         fn.argtypes = [vp, vp, sz, vp, sz, vp, sz, ctypes.c_int, vp, sz, vp, vp, ctypes.POINTER(ctypes.c_uint32)]

@@ -5,8 +5,9 @@
 //   ChannelPair::decode_ga_sce / decode_ga_cpe  aac/cpe.rs:51-161      (common window, ms mask, intensity, mid/side)
 //   IcsInfo::decode, Ics::decode*               aac/ics/mod.rs:120-447 (sections, scale factors, spectrum, noise)
 //   Pulse::read / synth, Tns::read (+ ranges)   aac/ics/pulse.rs:35-105, aac/ics/tns.rs:35-199
-// CPU only.  State is changed in place as the reference changes it: a packet that fails half way leaves the window
-// history and the noise generator where the failure found them.
+// The per-packet rules are the host/device functions of aac_entropy.h; this file keeps the stream state between packets and
+// is a loop over them.  CPU only.  State is changed in place as the reference changes it: a packet that fails half way leaves
+// the window history and the noise generator where the failure found them.
 //
 // Floating point: single IEEE operations in the reference's order (host code is compiled with -ffp-contract=off); the
 // tables use the C library's powf, which is what f32::powf calls (tests/test_aac_frontend.py: the scale-factor tables are the
@@ -20,59 +21,13 @@
 #include <vector>
 
 #include "../../include/symgpu.h"
+#include "aac_entropy.h"
 
 namespace {
 
+namespace ae = symgpu::aace;
+
 #include "aac_huffman_data.inc"
-
-// ---- Huffman books as binary trees over the (length, code) lists ----------------------------------------------------------
-struct Book {
-    std::vector<int32_t> node;  // pairs: child for bit 0, child for bit 1; >= 0 inner node index, < 0: ~value
-    uint32_t max_len = 0;
-    uint16_t lut[1024];         // the next 10 bits -> value << 5 | length for codes of <= 10 bits, 0 for longer ones
-    void build(const uint32_t* words, size_t n) {
-        node.assign(2, 0);
-        std::memset(lut, 0, sizeof lut);
-        for (size_t v = 0; v < n; ++v) {
-            const uint32_t len = words[v] >> 24, code = words[v] & 0xffffff;
-            if (len > max_len) max_len = len;
-            if (len <= 10)
-                for (uint32_t k = 0; k < (1u << (10 - len)); ++k) lut[(code << (10 - len)) | k] = uint16_t(v << 5 | len);
-            size_t at = 0;
-            for (uint32_t b = len; b-- > 0;) {
-                const uint32_t bit = (code >> b) & 1;
-                if (b == 0) {
-                    node[2 * at + bit] = ~int32_t(v);
-                } else {
-                    if (node[2 * at + bit] == 0) {
-                        node[2 * at + bit] = int32_t(node.size() / 2);
-                        node.push_back(0), node.push_back(0);
-                    }
-                    at = size_t(node[2 * at + bit]);
-                }
-            }
-        }
-    }
-};
-
-struct Tables {
-    Book spec[11], scf;
-    float pow43[8192], normal_scf[256], intensity_scf[256];
-    Tables() {
-        const uint32_t* w[11] = {kAacHuff_1, kAacHuff_2, kAacHuff_3, kAacHuff_4, kAacHuff_5, kAacHuff_6, kAacHuff_7, kAacHuff_8, kAacHuff_9, kAacHuff_10, kAacHuff_11};
-        const size_t n[11] = {81, 81, 81, 81, 81, 81, 64, 64, 169, 169, 289};
-        for (int k = 0; k < 11; ++k) spec[k].build(w[k], n[k]);
-        scf.build(kAacHuff_scf, 121);
-        const float p43 = 4.0f / 3.0f;
-        for (int i = 0; i < 8192; ++i) pow43[i] = powf(float(i), p43);                              // ics/mod.rs:44-50
-        for (int i = 0; i < 256; ++i) normal_scf[i] = powf(2.0f, 0.25f * float(i - 56 - 100));      // :58-66
-        for (int i = 0; i < 256; ++i) intensity_scf[i] = powf(0.5f, 0.25f * float(i - 155));        // :74-82
-    }
-};
-const Tables& tables() {
-    static const Tables t;
-    return t;
-}
 
 // ---- aac/common.rs:22-92, :121-172; tns.rs:22-24 --------------------------------------------------------------------------
 const uint16_t L48[] = {0, 4, 8, 12, 16, 20, 24, 28, 32, 36, 40, 48, 56, 64, 72, 80, 88, 96, 108, 120, 132, 144, 160, 176, 196, 216, 240, 264, 292, 320,
@@ -94,14 +49,14 @@ const uint16_t L64[] = {0, 4, 8, 12, 16, 20, 24, 28, 32, 36, 40, 44, 48, 52, 56,
 const uint16_t S64[] = {0, 4, 8, 12, 16, 20, 24, 32, 40, 48, 64, 92, 128};
 const uint16_t L96[] = {0, 4, 8, 12, 16, 20, 24, 28, 32, 36, 40, 44, 48, 52, 56, 64, 72, 80, 88, 96, 108, 120, 132, 144, 156, 172, 188, 212, 240, 276,
                         320, 384, 448, 512, 576, 640, 704, 768, 832, 896, 960, 1024};
-struct Bands {
+struct BandList {
     const uint16_t* v;
     size_t len;  // entries (bands + 1)
 };
-#define BANDS(a) Bands{a, sizeof(a) / sizeof(a[0])}
+#define BANDS(a) BandList{a, sizeof(a) / sizeof(a[0])}
 struct SubbandInfo {
     uint32_t min_rate;
-    Bands lng, shrt;
+    BandList lng, shrt;
 };
 const SubbandInfo kInfo[12] = {{92017, BANDS(L96), BANDS(S64)}, {75132, BANDS(L96), BANDS(S64)}, {55426, BANDS(L64), BANDS(S64)}, {46009, BANDS(L48), BANDS(S48)},
                                {37566, BANDS(L48), BANDS(S48)}, {27713, BANDS(L32), BANDS(S48)}, {23004, BANDS(L24), BANDS(S24)}, {18783, BANDS(L24), BANDS(S24)},
@@ -109,7 +64,59 @@ const SubbandInfo kInfo[12] = {{92017, BANDS(L96), BANDS(S64)}, {75132, BANDS(L9
 const uint8_t kTnsMaxLong[12] = {31, 31, 34, 40, 42, 51, 46, 46, 42, 42, 42, 39};
 const uint8_t kTnsMaxShort[12] = {9, 9, 10, 14, 14, 14, 14, 14, 14, 14, 14, 14};
 
-// ---- BitReaderLtr + FiniteBitStream: a failed read fails the packet, so only positions matter ----------------------------
+// ---- the tables of aac_entropy.h ---------------------------------------------------------------------------------------------
+void build_book(ae::Book& b, const uint32_t* words, size_t n) {  // the (length, code) list -> first-level LUT + binary tree
+    std::memset(&b, 0, sizeof b);
+    size_t n_nodes = 1;
+    for (size_t v = 0; v < n; ++v) {
+        const uint32_t len = words[v] >> 24, code = words[v] & 0xffffff;
+        if (len > b.max_len) b.max_len = len;
+        if (len <= 10)
+            for (uint32_t k = 0; k < (1u << (10 - len)); ++k) b.lut[(code << (10 - len)) | k] = uint16_t(v << 5 | len);
+        size_t at = 0;
+        for (uint32_t bit_no = len; bit_no-- > 0;) {
+            const uint32_t bit = (code >> bit_no) & 1;
+            if (bit_no == 0) {
+                b.node[2 * at + bit] = ~int32_t(v);
+            } else {
+                if (b.node[2 * at + bit] == 0) b.node[2 * at + bit] = int32_t(n_nodes++);
+                at = size_t(b.node[2 * at + bit]);
+            }
+        }
+    }
+}
+
+struct HostTables {
+    ae::Tables t;
+    HostTables() {
+        std::memset(&t, 0, sizeof t);
+        const uint32_t* w[11] = {kAacHuff_1, kAacHuff_2, kAacHuff_3, kAacHuff_4, kAacHuff_5, kAacHuff_6, kAacHuff_7, kAacHuff_8, kAacHuff_9, kAacHuff_10, kAacHuff_11};
+        const size_t n[11] = {81, 81, 81, 81, 81, 81, 64, 64, 169, 169, 289};
+        for (int k = 0; k < 11; ++k) build_book(t.book[k], w[k], n[k]);
+        build_book(t.book[11], kAacHuff_scf, 121);
+        const float p43 = 4.0f / 3.0f;
+        for (int i = 0; i < 8192; ++i) t.pow43[i] = powf(float(i), p43);                              // ics/mod.rs:44-50
+        for (int i = 0; i < 256; ++i) t.normal_scf[i] = powf(2.0f, 0.25f * float(i - 56 - 100));      // :58-66
+        for (int i = 0; i < 256; ++i) t.intensity_scf[i] = powf(0.5f, 0.25f * float(i - 155));        // :74-82
+        for (int res = 0; res < 2; ++res) {                                                            // tns.rs:84-110
+            const float fac = res ? 8.0f : 4.0f;
+            const float half_pi = 1.57079632679489661923132169163975144f;
+            const float iqfac = (fac - 0.5f) / half_pi, iqfac_m = (fac + 0.5f) / half_pi;
+            for (int i = 0; i < 16; ++i) {
+                const float c = float(i - 8);
+                t.tns_sin[res][i] = sinf(c >= 0.0f ? c / iqfac : c / iqfac_m);
+            }
+        }
+        for (int r = 0; r < 12; ++r) {
+            std::memcpy(t.lng[r], kInfo[r].lng.v, kInfo[r].lng.len * sizeof(uint16_t));
+            std::memcpy(t.shrt[r], kInfo[r].shrt.v, kInfo[r].shrt.len * sizeof(uint16_t));
+            t.n_lng[r] = uint8_t(kInfo[r].lng.len), t.n_shrt[r] = uint8_t(kInfo[r].shrt.len);
+            t.tns_max_long[r] = kTnsMaxLong[r], t.tns_max_short[r] = kTnsMaxShort[r];
+        }
+    }
+};
+
+// ---- BitReaderLtr for the AudioSpecificConfig parser: a failed read sticks, READ_OK() checks it --------------------------
 struct Bits {
     const uint8_t* p;
     size_t n_bytes, n_bits, at = 0;
@@ -136,71 +143,19 @@ struct Bits {
         return v;
     }
     bool read_bool() { return read(1) == 1; }
-    void ignore(uint64_t w) {
-        if (!ok || w > left()) ok = false;
-        else at += size_t(w);
-    }
-    void realign() { at = (at + 7) & ~size_t(7); }
-    uint32_t unary_ones() {
-        uint32_t n = 0;
-        for (;;) {
-            if (!ok || at >= n_bits) return ok = false, 0;
-            const uint64_t v = peek() | ((uint64_t(1) << 7) - 1);  // only the top 57 bits are the stream
-            const uint32_t ones = ~v ? uint32_t(__builtin_clzll(~v)) : 64u;  // the run of ones at the front
-            if (ones >= 57) {
-                n += 57, at += 57;
-                continue;
-            }
-            if (at + ones >= n_bits) return ok = false, 0;  // the ones run into the end: no terminating zero
-            n += ones, at += ones + 1;
-            return n;
-        }
-    }
-    uint32_t codebook(const Book& b) {  // bit.rs:771-808: matched against the data padded with zeros, then must fit
-        if (!ok) return 0;
-        const uint64_t v = peek();
-        const uint32_t e = b.lut[v >> 54];
-        if (e) {
-            const uint32_t len = e & 31;
-            if (len > left()) return ok = false, 0;
-            at += len;
-            return e >> 5;
-        }
-        size_t node = 0;
-        for (uint32_t len = 1; len <= b.max_len; ++len) {
-            const int32_t next = b.node[2 * node + ((v >> (64 - len)) & 1)];
-            if (next < 0) {
-                if (len > left()) return ok = false, 0;
-                at += len;
-                return uint32_t(~next);
-            }
-            node = size_t(next);
-        }
-        return ok = false, 0;  // unreachable: the books are complete prefix codes
-    }
 };
 
-struct Lcg {  // common.rs:96-111
-    uint32_t state = 0x1f2e3d4c;
-    uint64_t draws = 0;
-    int32_t next() { return ++draws, int32_t(state = state * 1664525u + 1013904223u); }
-    // The state after `n` more draws: the n-th power of the affine map x -> a x + c, by squaring (mod 2^32).
-    static uint32_t jump(uint32_t s, uint64_t n) {
-        uint32_t a = 1664525u, c = 1013904223u, ra = 1, rc = 0;
-        for (; n; n >>= 1) {
-            if (n & 1) ra *= a, rc = rc * a + c;
-            c = c * a + c, a *= a;
-        }
-        return ra * s + rc;
+
+struct Pair {  // cpe.rs:25-49
+    bool is_pair;
+    uint32_t channel;
+    bool ms_used[8][64] = {};
+    ae::Ics ics[2];
+    ae::Lcg lcg;
+    float coeffs[2][1024];
+    Pair(bool pair, uint32_t ch, uint32_t rate_idx) : is_pair(pair), channel(ch) {
+        for (int c = 0; c < 2; ++c) ae::init_ics(ics[c], rate_idx, coeffs[c]);
     }
-};
-
-enum : uint8_t { ZERO_HCB = 0, RESERVED_HCB = 12, NOISE_HCB = 13, INTENSITY_HCB2 = 14, INTENSITY_HCB = 15 };
-
-struct TnsFilter {
-    uint32_t length = 0, order = 0;
-    bool direction = false;
-    float coef[21] = {};
 };
 
 #define CHECK(cond) \
@@ -209,420 +164,29 @@ struct TnsFilter {
     } while (0)
 #define READ_OK() CHECK(bs.ok)
 
-struct Ics {
-    // IcsInfo
-    uint8_t window_sequence = 0, prev_window_sequence = 0;
-    bool window_shape = false, prev_window_shape = false;
-    bool grouping[8] = {};
-    uint32_t group_start[8] = {};
-    uint32_t window_groups = 0, num_windows = 0, max_sfb = 0;
-    bool long_win = true;
-    // Ics
-    uint32_t global_gain = 0;
-    bool has_pulse = false, has_tns = false, stale_scale_read = false;
-    uint32_t n_pulse = 0, pulse_start = 0;
-    uint8_t pulse_off[4] = {}, pulse_amp[4] = {};
-    uint32_t n_filt[8] = {};
-    TnsFilter filt[8][4];
-    uint8_t sfb_cb[8][64] = {};
-    float scales[8][64] = {};
-    float coeffs[1024] = {};
-    const SubbandInfo* sb = nullptr;
-
-    void reset_info() {  // Ics::reset -> IcsInfo::new (ics/mod.rs:103-117, :229-232)
-        window_sequence = prev_window_sequence = 0;
-        window_shape = prev_window_shape = false;
-        std::memset(grouping, 0, sizeof grouping);
-        std::memset(group_start, 0, sizeof group_start);
-        window_groups = num_windows = max_sfb = 0;
-        long_win = true;
-    }
-    const Bands& bands() const { return long_win ? sb->lng : sb->shrt; }
-    void copy_from_common(const Ics& o) {
-        const uint8_t seq = window_sequence;
-        const bool shape = window_shape;
-        window_sequence = o.window_sequence, window_shape = o.window_shape;
-        std::memcpy(grouping, o.grouping, sizeof grouping);
-        std::memcpy(group_start, o.group_start, sizeof group_start);
-        window_groups = o.window_groups, num_windows = o.num_windows, max_sfb = o.max_sfb, long_win = o.long_win;
-        prev_window_sequence = seq, prev_window_shape = shape;
-    }
-    symgpu_status decode_info(Bits& bs) {  // ics/mod.rs:120-177, :292-300
-        prev_window_sequence = window_sequence, prev_window_shape = window_shape;
-        const bool reserved = bs.read_bool();
-        READ_OK();
-        CHECK(!reserved);
-        const uint32_t seq = bs.read(2);
-        READ_OK();
-        window_sequence = uint8_t(seq);
-        const bool shape = bs.read_bool();
-        READ_OK();
-        window_shape = shape;
-        window_groups = 1;
-        if (window_sequence == SYMGPU_AAC_EIGHT_SHORT) {
-            long_win = false, num_windows = 8;
-            const uint32_t v = bs.read(4);
-            READ_OK();
-            max_sfb = v;
-            for (uint32_t i = 0; i < 7; ++i) {
-                const bool g = bs.read_bool();
-                READ_OK();
-                grouping[i] = g;
-                if (!g) group_start[window_groups++] = i + 1;
-            }
-        } else {
-            long_win = true, num_windows = 1;
-            const uint32_t v = bs.read(6);
-            READ_OK();
-            max_sfb = v;
-            const bool predictor = bs.read_bool();
-            READ_OK();
-            if (predictor) return SYMGPU_ERR_UNSUPPORTED;  // ltp.rs:20-54
-        }
-        CHECK(max_sfb + 1 <= bands().len);
-        return SYMGPU_OK;
-    }
-    uint32_t get_group_start(uint32_t g) const { return g == 0 ? 0 : g >= window_groups ? (long_win ? 1u : 8u) : group_start[g]; }
-
-    symgpu_status decode_section_data(Bits& bs) {  // :234-275
-        const uint32_t bits = long_win ? 5 : 3, esc = (1u << bits) - 1;
-        for (uint32_t g = 0; g < window_groups; ++g) {
-            uint32_t k = 0, l = 0;
-            while (k < max_sfb) {
-                CHECK(l < 64);
-                const uint32_t cb = bs.read(4);
-                READ_OK();
-                CHECK(cb != RESERVED_HCB);
-                uint64_t len = 0;
-                for (;;) {
-                    const uint32_t inc = bs.read(bits);
-                    READ_OK();
-                    len += inc;
-                    if (inc < esc) break;
-                }
-                CHECK(k + len <= max_sfb);
-                for (uint32_t s = k; s < k + len; ++s) sfb_cb[g][s] = uint8_t(cb);
-                k += uint32_t(len), ++l;
-            }
-        }
-        return SYMGPU_OK;
-    }
-    symgpu_status decode_scale_factors(Bits& bs) {  // :302-354
-        const Tables& T = tables();
-        bool noise_pcm = true;
-        int32_t scf_int = 155, scf_noise = int32_t(global_gain) - 90 + 100, scf_normal = int32_t(global_gain);
-        for (uint32_t g = 0; g < window_groups; ++g)
-            for (uint32_t s = 0; s < max_sfb; ++s) {
-                const uint8_t cb = sfb_cb[g][s];
-                float v;
-                if (cb == ZERO_HCB) {
-                    v = 0.0f;
-                } else if (cb == INTENSITY_HCB || cb == INTENSITY_HCB2) {
-                    scf_int += int32_t(bs.codebook(T.scf)) - 60;
-                    READ_OK();
-                    CHECK(scf_int >= 0 && scf_int < 256);
-                    v = T.intensity_scf[scf_int];
-                } else if (cb == NOISE_HCB) {
-                    if (noise_pcm) noise_pcm = false, scf_noise += int32_t(bs.read(9)) - 256;
-                    else scf_noise += int32_t(bs.codebook(T.scf)) - 60;
-                    READ_OK();
-                    CHECK(scf_noise >= 0 && scf_noise < 256);
-                    v = T.normal_scf[scf_noise];
-                } else {
-                    scf_normal += int32_t(bs.codebook(T.scf)) - 60;
-                    READ_OK();
-                    CHECK(scf_normal >= 0 && scf_normal < 256);
-                    v = T.normal_scf[scf_normal];
-                }
-                scales[g][s] = v;
-            }
-        return SYMGPU_OK;
-    }
-    static float sign_of(uint32_t bit) { return 1.0f - 2.0f * float(bit); }
-    static symgpu_status read_escape(Bits& bs, uint32_t& out) {  // :598-607
-        const uint32_t n = bs.unary_ones();
-        READ_OK();
-        CHECK(n < 9);
-        const uint32_t w = bs.read(n + 4);
-        READ_OK();
-        out = (1u << (n + 4)) + w;
-        return SYMGPU_OK;
-    }
-    symgpu_status decode_spectrum(Bits& bs, Lcg& lcg) {  // :360-401, :466-596
-        const Tables& T = tables();
-        std::memset(coeffs, 0, sizeof coeffs);
-        const Bands& b = bands();
-        for (uint32_t g = 0; g < window_groups; ++g) {
-            const uint32_t cur_w = get_group_start(g), next_w = get_group_start(g + 1);
-            for (uint32_t s = 0; s < max_sfb; ++s) {
-                const uint8_t cb = sfb_cb[g][s];
-                const float scale = scales[g][s];
-                for (uint32_t w = cur_w; w < next_w; ++w) {
-                    float* dst = coeffs + b.v[s] + 128 * w;
-                    const uint32_t n = uint32_t(b.v[s + 1] - b.v[s]);
-                    if (cb == ZERO_HCB || cb == RESERVED_HCB || cb == INTENSITY_HCB || cb == INTENSITY_HCB2) continue;
-                    if (cb == NOISE_HCB) {  // decode_noise
-                        float energy = 0.0f;
-                        for (uint32_t i = 0; i < n; ++i) {
-                            dst[i] = float(int16_t(lcg.next() >> 16));
-                            energy += dst[i] * dst[i];
-                        }
-                        const float sc = scale / sqrtf(energy);
-                        for (uint32_t i = 0; i < n; ++i) dst[i] *= sc;
-                    } else if (cb <= 2) {
-                        const float iq[3] = {-scale, 0.0f, scale};
-                        for (uint32_t i = 0; i + 4 <= n; i += 4) {
-                            const uint32_t cw = bs.codebook(T.spec[cb - 1]);
-                            READ_OK();
-                            dst[i] = iq[cw / 27], dst[i + 1] = iq[cw / 9 % 3], dst[i + 2] = iq[cw / 3 % 3], dst[i + 3] = iq[cw % 3];
-                        }
-                    } else if (cb <= 4) {
-                        const float iq[3] = {0.0f, scale, 2.51984209978974632953f * scale};
-                        for (uint32_t i = 0; i + 4 <= n; i += 4) {
-                            const uint32_t cw = bs.codebook(T.spec[cb - 1]);
-                            READ_OK();
-                            const uint32_t d[4] = {cw / 27, cw / 9 % 3, cw / 3 % 3, cw % 3};
-                            for (int k = 0; k < 4; ++k)
-                                if (d[k]) {
-                                    const uint32_t bit = bs.read(1);
-                                    READ_OK();
-                                    dst[i + k] = sign_of(bit) * iq[d[k]];
-                                }
-                        }
-                    } else if (cb <= 6) {
-                        for (uint32_t i = 0; i + 2 <= n; i += 2) {
-                            const uint32_t cw = bs.codebook(T.spec[cb - 1]);
-                            READ_OK();
-                            const uint32_t a = cw / 9, c = cw % 9;
-                            const float x = a < 4 ? -T.pow43[4 - a] : T.pow43[a - 4], y = c < 4 ? -T.pow43[4 - c] : T.pow43[c - 4];
-                            dst[i] = x * scale, dst[i + 1] = y * scale;
-                        }
-                    } else if (cb <= 10) {
-                        const uint32_t mod = cb < 9 ? 8 : 13;
-                        for (uint32_t i = 0; i + 2 <= n; i += 2) {
-                            const uint32_t cw = bs.codebook(T.spec[cb - 1]);
-                            READ_OK();
-                            const float x = T.pow43[cw / mod], y = T.pow43[cw % mod];
-                            float sx = 1.0f, sy = 1.0f;
-                            if (x != 0.0f) sx = sign_of(bs.read(1));
-                            READ_OK();
-                            if (y != 0.0f) sy = sign_of(bs.read(1));
-                            READ_OK();
-                            dst[i] = sx * x * scale, dst[i + 1] = sy * y * scale;
-                        }
-                    } else {
-                        for (uint32_t i = 0; i + 2 <= n; i += 2) {
-                            const uint32_t cw = bs.codebook(T.spec[10]);
-                            READ_OK();
-                            uint32_t a = cw / 17, c = cw % 17;
-                            float sx = 1.0f, sy = 1.0f;
-                            if (a) sx = sign_of(bs.read(1));
-                            READ_OK();
-                            if (c) sy = sign_of(bs.read(1));
-                            READ_OK();
-                            if (a == 16) {
-                                const symgpu_status st = read_escape(bs, a);
-                                if (st != SYMGPU_OK) return st;
-                            }
-                            if (c == 16) {
-                                const symgpu_status st = read_escape(bs, c);
-                                if (st != SYMGPU_OK) return st;
-                            }
-                            dst[i] = sx * T.pow43[a] * scale, dst[i + 1] = sy * T.pow43[c] * scale;
-                        }
-                    }
-                }
-            }
-        }
-        return SYMGPU_OK;
-    }
-    symgpu_status read_tns(Bits& bs) {  // tns.rs:35-147
-        has_tns = bs.read_bool();
-        READ_OK();
-        if (!has_tns) return SYMGPU_OK;
-        const uint32_t max_order = long_win ? 12 : 7;
-        std::memset(n_filt, 0, sizeof n_filt);
-        for (uint32_t w = 0; w < num_windows; ++w) {
-            const uint32_t nf = bs.read(long_win ? 2 : 1);
-            READ_OK();
-            n_filt[w] = nf;
-            bool coef_res = false;
-            if (nf) coef_res = bs.read_bool();
-            READ_OK();
-            for (uint32_t f = 0; f < nf; ++f) {
-                TnsFilter& t = filt[w][f];
-                t = TnsFilter();
-                t.length = bs.read(long_win ? 6 : 4);
-                t.order = bs.read(long_win ? 5 : 3);
-                READ_OK();
-                CHECK(t.order <= max_order);
-                if (t.order == 0) continue;
-                t.direction = bs.read_bool();
-                const bool compress = bs.read_bool();
-                READ_OK();
-                const uint32_t res_bits = (coef_res ? 4u : 3u) - (compress ? 1u : 0u);
-                const uint32_t sign_mask = 1u << (res_bits - 1), full = 1u << res_bits;
-                const float fac = coef_res ? 8.0f : 4.0f;
-                const float half_pi = 1.57079632679489661923132169163975144f;
-                const float iqfac = (fac - 0.5f) / half_pi, iqfac_m = (fac + 0.5f) / half_pi;
-                float tmp[20] = {};
-                for (uint32_t k = 0; k < t.order; ++k) {
-                    const uint32_t val = bs.read(res_bits);
-                    READ_OK();
-                    const float c = float((val & sign_mask) ? int32_t(val) - int32_t(full) : int32_t(val));
-                    tmp[k] = sinf(c >= 0.0f ? c / iqfac : c / iqfac_m);
-                }
-                float b[21] = {};
-                for (uint32_t m = 1; m <= t.order; ++m) {
-                    for (uint32_t i = 1; i < m; ++i) b[i] = t.coef[i - 1] + tmp[m - 1] * t.coef[m - i - 1];
-                    for (uint32_t i = 1; i < m; ++i) t.coef[i - 1] = b[i];
-                    t.coef[m - 1] = tmp[m - 1];
-                }
-            }
-        }
-        return SYMGPU_OK;
-    }
-    symgpu_status decode(Bits& bs, Lcg& lcg, bool common_window) {  // Ics::decode, ics/mod.rs:403-447
-        symgpu_status st;
-        global_gain = bs.read(8);
-        READ_OK();
-        if (!common_window && (st = decode_info(bs)) != SYMGPU_OK) return st;
-        if ((st = decode_section_data(bs)) != SYMGPU_OK) return st;
-        if ((st = decode_scale_factors(bs)) != SYMGPU_OK) return st;
-        has_pulse = bs.read_bool();
-        READ_OK();
-        if (has_pulse) {
-            n_pulse = bs.read(2) + 1;
-            pulse_start = bs.read(6);
-            for (uint32_t i = 0; i < n_pulse; ++i) pulse_off[i] = uint8_t(bs.read(5)), pulse_amp[i] = uint8_t(bs.read(4));
-            READ_OK();
-        }
-        CHECK(!has_pulse || long_win);
-        if ((st = read_tns(bs)) != SYMGPU_OK) return st;
-        const bool gain_control = bs.read_bool();
-        READ_OK();
-        CHECK(!gain_control);
-        return decode_spectrum(bs, lcg);
-    }
-    void apply_pulse() {  // Pulse::synth, pulse.rs:60-105
-        if (!has_pulse) return;
-        const Bands& b = bands();
-        if (pulse_start >= b.len - 1) return;
-        uint32_t k = b.v[pulse_start], band = pulse_start;
-        const float p43 = 4.0f / 3.0f;
-        for (uint32_t i = 0; i < n_pulse; ++i) {
-            k += pulse_off[i];
-            if (k >= 1024) return;
-            while (b.v[band + 1] <= k) ++band;
-            if (band >= max_sfb) stale_scale_read = true;  // a band no section coded: the scale is whatever an earlier block left
-            const float scale = scales[0][band];
-            float base = coeffs[k];
-            if (base != 0.0f) {
-                if (scale == 0.0f) {
-                    base = 0.0f;
-                } else {
-                    const float bval = coeffs[k] / scale;
-                    base = bval >= 0.0f ? powf(coeffs[k], 0.75f) : -powf(-coeffs[k], 0.75f);
-                }
-            }
-            if (base > 0.0f) base += float(pulse_amp[i]);
-            else base -= float(pulse_amp[i]);
-            const float iq = base < 0.0f ? -powf(-base, p43) : powf(base, p43);
-            coeffs[k] = iq * scale;
-        }
-    }
-    // The filters Tns::synth walks (tns.rs:149-199), resolved to line ranges; order 0 left out.
-    uint32_t tns_filters(uint32_t rate_idx, symgpu_aac_tns* out) const {
-        if (!has_tns) return 0;
-        const Bands& b = bands();
-        uint32_t max_bands = long_win ? kTnsMaxLong[rate_idx] : kTnsMaxShort[rate_idx];
-        if (max_sfb < max_bands) max_bands = max_sfb;
-        uint32_t n = 0;
-        for (uint32_t w = 0; w < num_windows; ++w) {
-            uint32_t bottom = uint32_t(b.len - 1);
-            for (uint32_t f = 0; f < n_filt[w]; ++f) {
-                const TnsFilter& t = filt[w][f];
-                const uint32_t top = bottom;
-                bottom = top > t.length ? top - t.length : 0;
-                if (t.order == 0) continue;
-                symgpu_aac_tns& o = out[n++];
-                std::memset(&o, 0, sizeof o);
-                o.start = uint16_t(w * 128 + b.v[bottom < max_bands ? bottom : max_bands]);
-                o.end = uint16_t(w * 128 + b.v[top < max_bands ? top : max_bands]);
-                o.order = uint8_t(t.order), o.direction = t.direction ? 1 : 0;
-                std::memcpy(o.lpc, t.coef, sizeof o.lpc);
-            }
-        }
-        return n;
-    }
-};
-
-struct Pair {  // cpe.rs:25-49
-    bool is_pair;
-    uint32_t channel;
-    uint8_t ms_mask_present = 0;
-    bool ms_used[8][64] = {};
-    Ics ics[2];
-    Lcg lcg;
-    Pair(bool pair, uint32_t ch, const SubbandInfo* sb) : is_pair(pair), channel(ch) { ics[0].sb = ics[1].sb = sb; }
-
-    symgpu_status decode_cpe(Bits& bs) {  // cpe.rs:61-161
-        Ics &a = ics[0], &b = ics[1];
-        symgpu_status st;
-        const bool common = bs.read_bool();
-        READ_OK();
-        if (common) {
-            if ((st = a.decode_info(bs)) != SYMGPU_OK) return st;
-            ms_mask_present = uint8_t(bs.read(2));
-            READ_OK();
-            CHECK(ms_mask_present != 3);
-            for (uint32_t g = 0; g < a.window_groups; ++g)
-                for (uint32_t s = 0; s < a.max_sfb; ++s) {
-                    ms_used[g][s] = ms_mask_present == 1 ? bs.read_bool() : ms_mask_present == 2;
-                    READ_OK();
-                }
-            b.copy_from_common(a);
-        }
-        if ((st = a.decode(bs, lcg, common)) != SYMGPU_OK) return st;
-        if ((st = b.decode(bs, lcg, common)) != SYMGPU_OK) return st;
-        if (!common) return SYMGPU_OK;
-        const Bands& bd = a.bands();
-        uint32_t g = 0;
-        for (uint32_t w = 0; w < a.num_windows; ++w) {
-            if (w > 0 && !a.grouping[w - 1]) ++g;
-            for (uint32_t s = 0; s < a.max_sfb; ++s) {
-                const uint32_t lo = w * 128 + bd.v[s], hi = w * 128 + bd.v[s + 1];
-                const uint8_t c0 = a.sfb_cb[g][s], c1 = b.sfb_cb[g][s];
-                if (c1 == INTENSITY_HCB || c1 == INTENSITY_HCB2) {
-                    const bool invert = ms_mask_present == 1 && ms_used[g][s];
-                    const float dir = c1 == INTENSITY_HCB ? 1.0f : -1.0f, factor = invert ? -1.0f : 1.0f;
-                    const float scale = dir * factor * b.scales[g][s];
-                    for (uint32_t i = lo; i < hi; ++i) b.coeffs[i] = scale * a.coeffs[i];
-                } else if (c0 == NOISE_HCB || c1 == NOISE_HCB) {
-                } else if (ms_used[g][s]) {
-                    for (uint32_t i = lo; i < hi; ++i) {
-                        const float tmp = a.coeffs[i] - b.coeffs[i];
-                        a.coeffs[i] += b.coeffs[i];
-                        b.coeffs[i] = tmp;
-                    }
-                }
-            }
-        }
-        return SYMGPU_OK;
-    }
-};
-
 }  // namespace
+
+const symgpu::aace::Tables& symgpu::aac_tables_host() {
+    static const HostTables t;
+    return t.t;
+}
+
+uint32_t symgpu::aac_rate_index(uint32_t sample_rate) {
+    for (uint32_t i = 0; i < 12; ++i)
+        if (sample_rate >= kInfo[i].min_rate) return i;
+    return 11;
+}
 
 struct symgpu_aac_fe {
     uint32_t channels, rate_idx;
-    const SubbandInfo* sb;
+    bool stale = false;               // a pulse read a scale factor an earlier block left behind
     std::vector<std::unique_ptr<Pair>> pairs;
     std::vector<uint32_t> lcg_start;  // job mode: the noise generator's state when pair k is first seen
 
-    symgpu_status set_pair(size_t pair_no, uint32_t channel, bool pair) {  // mod.rs:114-126
+    // the stream's side of aac_entropy.h's decode_ga
+    int set_pair(uint32_t pair_no, uint32_t channel, bool pair) {  // mod.rs:114-126
         if (pairs.size() <= pair_no) {
-            pairs.emplace_back(new Pair(pair, channel, sb));
+            pairs.emplace_back(new Pair(pair, channel, rate_idx));
             if (pair_no < lcg_start.size()) pairs.back()->lcg.state = lcg_start[pair_no];
         } else {
             CHECK(pairs[pair_no]->channel == channel);
@@ -631,59 +195,19 @@ struct symgpu_aac_fe {
         CHECK((pair ? channel + 1 : channel) < channels);
         return SYMGPU_OK;
     }
-    symgpu_status decode_ga(Bits& bs, size_t& cur_pair, uint32_t& cur_ch) {  // mod.rs:128-229
-        symgpu_status st;
-        while (bs.left() > 3) {
-            const uint32_t id = bs.read(3);
-            switch (id) {
-                case 0:
-                case 3: {
-                    bs.read(4);
-                    READ_OK();
-                    if ((st = set_pair(cur_pair, cur_ch, false)) != SYMGPU_OK) return st;
-                    Pair& p = *pairs[cur_pair];
-                    if ((st = p.ics[0].decode(bs, p.lcg, false)) != SYMGPU_OK) return st;
-                    ++cur_pair, ++cur_ch;
-                    break;
-                }
-                case 1:
-                    bs.read(4);
-                    READ_OK();
-                    if ((st = set_pair(cur_pair, cur_ch, true)) != SYMGPU_OK) return st;
-                    if ((st = pairs[cur_pair]->decode_cpe(bs)) != SYMGPU_OK) return st;
-                    ++cur_pair, cur_ch += 2;
-                    break;
-                case 2: return SYMGPU_ERR_UNSUPPORTED;
-                case 4: {
-                    bs.read(4);
-                    const bool align = bs.read_bool();
-                    uint32_t count = bs.read(8);
-                    READ_OK();
-                    if (count == 255) count += bs.read(8);
-                    READ_OK();
-                    if (align) bs.realign();
-                    bs.ignore(uint64_t(count) * 8);
-                    READ_OK();
-                    break;
-                }
-                case 5: return SYMGPU_ERR_UNSUPPORTED;
-                case 6: {
-                    uint32_t count = bs.read(4);
-                    READ_OK();
-                    if (count == 15) count += bs.read(8) - 1;
-                    READ_OK();
-                    if (count > 0) {
-                        bs.read(4);
-                        bs.ignore(4);
-                        bs.ignore(uint64_t(count - 1) * 8);
-                        READ_OK();
-                    }
-                    break;
-                }
-                default: return SYMGPU_OK;  // ID_TERM
-            }
+    ae::Ics& ics(uint32_t k, uint32_t c) { return pairs[k]->ics[c]; }
+    ae::Lcg& lcg(uint32_t k) { return pairs[k]->lcg; }
+    bool (&ms_used(uint32_t k))[8][64] { return pairs[k]->ms_used; }
+
+    void apply_pulse(ae::Ics& s) {  // Pulse::synth, pulse.rs:60-105
+        const ae::PulseLines p = ae::pulse_lines(symgpu::aac_tables_host(), s);
+        float scale[4], value[4];
+        for (uint32_t i = 0; i < p.n; ++i) {
+            if (p.band[i] >= s.max_sfb) stale = true;
+            scale[i] = s.scales[0][p.band[i]], value[i] = s.coeffs[p.line[i]];
         }
-        return SYMGPU_OK;
+        ae::pulse_apply(p, scale, value);
+        for (uint32_t i = 0; i < p.n; ++i) s.coeffs[p.line[i]] = value[i];
     }
 };
 
@@ -696,13 +220,7 @@ symgpu_status symgpu_aac_fe_create(uint32_t sample_rate, uint32_t channels, symg
     symgpu_aac_fe* fe = new (std::nothrow) symgpu_aac_fe();
     if (!fe) return SYMGPU_ERR_LIMIT;
     fe->channels = channels;
-    fe->rate_idx = 11;
-    for (uint32_t i = 0; i < 12; ++i)
-        if (sample_rate >= kInfo[i].min_rate) {
-            fe->rate_idx = i;
-            break;
-        }
-    fe->sb = &kInfo[fe->rate_idx];
+    fe->rate_idx = symgpu::aac_rate_index(sample_rate);
     *out = fe;
     return SYMGPU_OK;
 }
@@ -831,18 +349,17 @@ void symgpu_aac_fe_destroy(symgpu_aac_fe* fe) { delete fe; }
 
 void symgpu_aac_fe_reset(symgpu_aac_fe* fe) {  // AudioDecoder::reset -> ChannelPair::reset (the delay lines live with the synthesis stage)
     if (!fe) return;
-    for (auto& p : fe->pairs) p->ics[0].reset_info(), p->ics[1].reset_info();
+    for (auto& p : fe->pairs) ae::reset_info(p->ics[0]), ae::reset_info(p->ics[1]);
 }
 
 symgpu_status symgpu_aac_fe_decode(symgpu_aac_fe* fe, const uint8_t* packet, size_t n, uint32_t tns_base, symgpu_aac_unit* units,
                                    symgpu_aac_tns* tns, uint32_t* n_tns, float* coeffs) {
     if (!fe || (!packet && n) || !units || !tns || !n_tns || !coeffs) return SYMGPU_ERR_ARG;
     *n_tns = 0;
-    Bits bs(packet, n);
-    size_t cur_pair = 0;
-    uint32_t cur_ch = 0;
-    const symgpu_status st = fe->decode_ga(bs, cur_pair, cur_ch);
-    if (st != SYMGPU_OK) return st;
+    symgpu::mp3e::Bits bs(packet, n);
+    uint32_t cur_pair = 0, cur_ch = 0;
+    const int st = ae::decode_ga(bs, symgpu::aac_tables_host(), *fe, cur_pair, cur_ch);
+    if (st != SYMGPU_OK) return symgpu_status(st);
     // the reference renders the channels its elements covered and leaves the others alone; the batch format carries every channel
     if (cur_ch != fe->channels) return SYMGPU_ERR_UNSUPPORTED;
     std::memset(units, 0, 2 * sizeof(symgpu_aac_unit));
@@ -851,15 +368,15 @@ symgpu_status symgpu_aac_fe_decode(symgpu_aac_fe* fe, const uint8_t* packet, siz
     for (size_t k = 0; k < cur_pair; ++k) {
         Pair& p = *fe->pairs[k];
         for (uint32_t c = 0; c < (p.is_pair ? 2u : 1u); ++c) {
-            Ics& ics = p.ics[c];
+            ae::Ics& ics = p.ics[c];
             const uint32_t ch = p.channel + c;
-            ics.apply_pulse();
+            fe->apply_pulse(ics);
             symgpu_aac_unit& u = units[ch];
             u.window_sequence = ics.window_sequence, u.window_shape = ics.window_shape, u.prev_window_shape = ics.prev_window_shape;
-            const uint32_t nf = ics.tns_filters(fe->rate_idx, tns + total);
-            u.n_tns = uint8_t(nf), u.tns_first = nf ? tns_base + total : 0;
-            total += nf;
-            std::memcpy(coeffs + 1024 * ch, ics.coeffs, sizeof ics.coeffs);
+            std::memcpy(tns + total, ics.tns, ics.n_tns * sizeof(symgpu_aac_tns));
+            u.n_tns = uint8_t(ics.n_tns), u.tns_first = ics.n_tns ? tns_base + total : 0;
+            total += ics.n_tns;
+            std::memcpy(coeffs + 1024 * ch, ics.coeffs, 1024 * sizeof(float));
         }
     }
     *n_tns = total;
@@ -921,8 +438,8 @@ symgpu_status symgpu_aac_fe_decode_packets_jobs(uint32_t sample_rate, uint32_t c
         for (uint32_t k = 0; k < j.n_pairs; ++k) {
             const Pair& p = *fe->pairs[k];
             j.is_pair[k] = p.is_pair, j.draws[k] = p.lcg.draws;
-            j.stale = j.stale || p.ics[0].stale_scale_read || p.ics[1].stale_scale_read;
         }
+        j.stale = fe->stale;
         symgpu_aac_fe_destroy(fe);
     };
     auto parallel = [&](bool second) {
@@ -940,7 +457,7 @@ symgpu_status symgpu_aac_fe_decode_packets_jobs(uint32_t sample_rate, uint32_t c
         const Job& j = jobs[i];
         if (j.st != SYMGPU_OK || j.stale || j.n_pairs != jobs[0].n_pairs || j.is_pair[0] != jobs[0].is_pair[0] || j.is_pair[1] != jobs[0].is_pair[1])
             return SYMGPU_ERR_RESET;
-        for (int k = 0; k < 2; ++k) jobs[i].start[k] = Lcg::jump(0x1f2e3d4c, total[k]), total[k] += j.draws[k];
+        for (int k = 0; k < 2; ++k) jobs[i].start[k] = ae::Lcg::jump(ae::kLcgSeed, total[k]), total[k] += j.draws[k];
     }
     parallel(true);
     size_t at = 0;
@@ -966,7 +483,7 @@ symgpu_status symgpu_aac_fe_decode_packets_jobs(uint32_t sample_rate, uint32_t c
 }
 
 void symgpu_aac_fe_tables(float* pow43, float* normal_scf, float* intensity_scf) {
-    const Tables& T = tables();
+    const ae::Tables& T = symgpu::aac_tables_host();
     if (pow43) std::memcpy(pow43, T.pow43, sizeof T.pow43);
     if (normal_scf) std::memcpy(normal_scf, T.normal_scf, sizeof T.normal_scf);
     if (intensity_scf) std::memcpy(intensity_scf, T.intensity_scf, sizeof T.intensity_scf);

@@ -73,6 +73,7 @@ struct symgpu_ctx {
     cudaEvent_t ev_units = nullptr;
     // ---- AAC / Vorbis ----
     symgpu::CodecTables* d_codec_tab = nullptr;
+    void* d_aac_fe_tab = nullptr;    // symgpu::aace::Tables: the AAC packet rules' tables (symgpu_aac_decode_*), on first use
     symgpu::CodecChunk* d_chunks = nullptr;
     symgpu::CodecChunk* h_chunks = nullptr;
     size_t chunks_cap = 0;

@@ -570,6 +570,7 @@ void symgpu_ctx_destroy(symgpu_ctx* ctx) {
     if (ctx->h_tiles) cudaFreeHost(ctx->h_tiles);
     if (ctx->d_stage) cudaFree(ctx->d_stage);
     if (ctx->d_codec_tab) cudaFree(ctx->d_codec_tab);
+    if (ctx->d_aac_fe_tab) cudaFree(ctx->d_aac_fe_tab);
     if (ctx->d_chunks) cudaFree(ctx->d_chunks);
     if (ctx->h_chunks) cudaFreeHost(ctx->h_chunks);
     if (ctx->d_aac_states) cudaFree(ctx->d_aac_states);

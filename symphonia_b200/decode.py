@@ -692,6 +692,93 @@ def decode_mp3_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False,
     return result
 
 
+# ---- ADTS AAC-LC, many files decoded on the device (elements, scale factors, Huffman spectra and noise in device code) ----------
+
+def aac_files_plan(files, threads=None, errors=None):
+    """Host half of decode_aac_files: every file indexed (adts_aac_index, on `threads` host threads), their bytes concatenated once,
+    one job per raw_data_block and one group per file (group i uses state slot i).  Returns dict(data, jobs, groups, out_samples,
+    failed).  A file that cannot be indexed or whose channel configuration is outside 1 / 2 (listed in `failed`) gets a group
+    without jobs; its message goes to errors[i] when `errors` is a dict."""
+    import concurrent.futures
+    import os
+    messages = {}
+
+    def index(i):
+        try:
+            return adts_aac_index(files[i])
+        except Exception as e:  # noqa: BLE001 -- one bad file must not abort the batch; its message is kept
+            messages[i] = f"{type(e).__name__}: {e}"
+            return None
+    with concurrent.futures.ThreadPoolExecutor(max_workers=threads or os.cpu_count()) as pool:
+        ix = list(pool.map(index, range(len(files))))
+    if errors is not None:
+        errors.update(messages)
+    bufs = [np.frombuffer(f, dtype=np.uint8) if not isinstance(f, np.ndarray) else np.ascontiguousarray(f, dtype=np.uint8) for f in files]
+    good = [i for i in range(len(files)) if ix[i] is not None]
+    data = np.concatenate([bufs[i] for i in good]) if good else np.zeros(0, dtype=np.uint8)
+    groups = np.zeros(len(files), dtype=nat.AAC_GROUP_DTYPE)
+    groups["slot"] = np.arange(len(files))
+    groups["channels"], groups["sample_rate"] = 1, 44100
+    jobs, byte_at, job_at, out_at = [], 0, 0, 0
+    for i in good:
+        packets, rate, channels = ix[i]
+        n = len(packets)
+        g = groups[i]
+        g["out_offset"], g["first_job"], g["n_jobs"], g["sample_rate"], g["channels"] = out_at, job_at, n, rate, channels
+        j = np.zeros(n, dtype=nat.PIECE_DTYPE)
+        j["offset"], j["len"] = packets["offset"] + np.uint64(byte_at), packets["size"]
+        jobs.append(j)
+        byte_at += bufs[i].size
+        job_at += n
+        out_at += n * 1024 * channels
+    failed = [i for i in range(len(files)) if ix[i] is None]
+    groups["out_offset"][failed] = out_at
+    groups["first_job"][failed] = job_at
+    jobs = np.concatenate(jobs) if jobs else np.zeros(0, dtype=nat.PIECE_DTYPE)
+    return dict(data=data, jobs=jobs, groups=groups, out_samples=out_at, failed=failed)
+
+
+def decode_aac_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False, errors=None, stats=None):
+    """[(samples [frames, channels] of `fmt`, sample_rate)] for a list of ADTS AAC-LC files, each equal to decode_adts_aac(engine, file,
+    fmt): the files are indexed on host threads, and ONE device call decodes every raw_data_block of every file -- elements, scale
+    factors, Huffman spectra, noise and TNS filters in device code, synthesis and the output stage on the GPU (pulses' new line
+    values on the host).  device=True: the bytes go to the device once and the samples are CUDA tensors, views of one output tensor.
+    A file that cannot be indexed, or whose channel configuration is outside 1 / 2, yields an empty result with sample rate 0 (its
+    message in errors[i] when `errors` is a dict).  stats: a dict that receives the per-packet `status` and `n_redecoded` (packets
+    decoded twice because they drew noise).  (Re)allocates the engine's AAC state slots, one per file, as decode_files does: a
+    streaming AAC decoder on the same engine loses its state.  At most 65 536 files per call (the state slot is 16 bits)."""
+    if len(files) > 1 << 16:
+        raise ValueError(f"decode_aac_files takes at most 65536 files per call, not {len(files)}")
+    plan = aac_files_plan(files, threads, errors)
+    groups, cap = plan["groups"], plan["out_samples"]
+    engine.aac_streams_alloc(max(len(files), 1))
+    if device:
+        import torch
+        dev = torch.device("cuda", engine.device)
+        as_t = lambda a: torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(-1)).to(dev)  # noqa: E731
+        out = torch.empty(cap, dtype=getattr(torch, _TORCH_DTYPES[fmt]), device=dev)
+        results_t = torch.empty(len(groups) * nat.AAC_RESULT_DTYPE.itemsize, dtype=torch.uint8, device=dev)
+        status_t = torch.empty(len(plan["jobs"]), dtype=torch.uint8, device=dev)
+        data_t, jobs_t = as_t(plan["data"]), as_t(plan["jobs"])
+        torch.cuda.current_stream(dev).synchronize()  # the copies above are on torch's stream, the decode on the engine's
+        redone = engine.aac_decode_dev(data_t, jobs_t, groups, fmt, out, results_t, status_t)
+        engine.sync()
+        results = results_t.cpu().numpy().view(nat.AAC_RESULT_DTYPE)
+        status = status_t.cpu().numpy()
+    else:
+        out, results, status, redone = engine.aac_decode_host(plan["data"], plan["jobs"], groups, fmt, cap)
+    if stats is not None:
+        stats.update(status=status, n_redecoded=redone)
+    result = []
+    for g in range(len(groups)):
+        if g in plan["failed"]:
+            result.append((out[:0].reshape(0, 0), 0))
+            continue
+        ch, at, n = int(groups[g]["channels"]), int(groups[g]["out_offset"]), int(results[g]["frames"])
+        result.append((out[at:at + n * ch].reshape(n, ch), int(groups[g]["sample_rate"])))
+    return result
+
+
 def decode_mpeg_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False, errors=None):
     """[(samples [frames, channels] of `fmt`, sample_rate)] for a list of MPEG audio files of any layer, each what
     decode_mpeg_audio(engine, file, fmt) returns: every file is indexed once, Layer III files go to decode_mp3_files and Layer I / II

@@ -312,6 +312,45 @@ class Engine:
                                                     out_t.numel() * out_t.element_size(), ptr(results_t), ptr(status_t), ctypes.byref(rounds)))
         return rounds.value
 
+    # -- AAC-LC decoded on the device -------------------------------------------------------------------
+    def aac_decode_host(self, data, jobs, groups, fmt, out_samples, out=None):
+        """Device AAC-LC decoding of many files in one call: `data` (bytes / uint8 array) holds the raw_data_blocks, jobs PIECE_DTYPE
+        (one per packet), groups AAC_GROUP_DTYPE (one per file: its jobs, sample rate, channels, state slot and output offset).
+        Returns (out [out_samples] of `fmt`, results AAC_RESULT_DTYPE [groups], status uint8 [jobs], n_redecoded); file g's samples
+        are out[out_offset:][:frames * channels]."""
+        from ._native import AAC_GROUP_DTYPE, AAC_RESULT_DTYPE, PIECE_DTYPE
+        a = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
+        jobs = np.ascontiguousarray(jobs, dtype=PIECE_DTYPE)
+        groups = np.ascontiguousarray(groups, dtype=AAC_GROUP_DTYPE)
+        if out is None:
+            out = np.zeros(int(out_samples), dtype=FMT_NUMPY[fmt])
+        assert out.flags.c_contiguous
+        results = np.zeros(len(groups), dtype=AAC_RESULT_DTYPE)
+        status = np.zeros(len(jobs), dtype=np.uint8)
+        redone = ctypes.c_uint32(0)
+        self._check(self._lib.symgpu_aac_decode_host(self._ctx, _np_ptr(a) if a.size else None, a.size, _np_ptr(jobs) if len(jobs) else None, len(jobs),
+                                                     _np_ptr(groups) if len(groups) else None, len(groups), int(fmt),
+                                                     _np_ptr(out) if out.nbytes else None, out.nbytes, _np_ptr(results) if len(groups) else None,
+                                                     _np_ptr(status) if len(jobs) else None, ctypes.byref(redone)))
+        return out, results, status, redone.value
+
+    def aac_decode_dev(self, data_t, jobs_t, groups, fmt, out_t, results_t, status_t):
+        """Device-resident variant: torch CUDA tensors (uint8 bytes, jobs / results as uint8 views of the records, `out` of the format's
+        element size, uint8 status); `groups` stays a host array.  Waits for the engine's stream for one 8-byte readback (and once
+        more when pulses need the host); the synthesis and the output stage are left queued on it.  Returns n_redecoded."""
+        from ._native import AAC_GROUP_DTYPE, AAC_RESULT_DTYPE, PIECE_DTYPE
+        ts = (data_t, jobs_t, out_t, results_t, status_t)
+        assert all(t.is_cuda and t.is_contiguous() for t in ts)
+        groups = np.ascontiguousarray(groups, dtype=AAC_GROUP_DTYPE)
+        n_jobs = jobs_t.numel() * jobs_t.element_size() // PIECE_DTYPE.itemsize
+        assert results_t.numel() * results_t.element_size() >= len(groups) * AAC_RESULT_DTYPE.itemsize and status_t.numel() >= n_jobs
+        ptr = lambda t: ctypes.c_void_p(t.data_ptr()) if t.numel() else None  # noqa: E731
+        redone = ctypes.c_uint32(0)
+        self._check(self._lib.symgpu_aac_decode_dev(self._ctx, ptr(data_t), data_t.numel(), ptr(jobs_t), n_jobs,
+                                                    _np_ptr(groups) if len(groups) else None, len(groups), int(fmt), ptr(out_t),
+                                                    out_t.numel() * out_t.element_size(), ptr(results_t), ptr(status_t), ctypes.byref(redone)))
+        return redone.value
+
     # -- output stage -------------------------------------------------------------------------
     def pcm_pack_host(self, pcm, spans, channels, fmt, out_frames, plane_stride=0, frames=0, n_spans=None, out=None):
         """Trim + interleave + convert planar f32 `pcm` (any shape, flat indexing) into [out_frames, channels]
