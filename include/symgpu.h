@@ -871,6 +871,81 @@ symgpu_status symgpu_aac_decode_dev(symgpu_ctx* ctx, const uint8_t* bytes, size_
                                     const symgpu_aac_group* groups, size_t n_groups, int format, void* out, size_t out_bytes,
                                     symgpu_aac_group_result* results, uint8_t* status, uint32_t* n_redecoded);
 
+/* Ogg Vorbis decoded on the device, many files per call: audio packets of the gathered logical streams -> interleaved samples of
+ * `format`.  The packet rules are those of symgpu_vorbis_fe_decode (vorbis_entropy.h, the same code): one device thread per
+ * packet decodes it with a fresh partition-class buffer, a scan by file over the decoded packets gives each its frame slot, its
+ * previous block flag and its trims, and the unchanged symgpu_vorbis_synth_dev and output stage of symgpu_pcm_pack_dev follow.
+ *   headers  host bytes holding the identification and setup packets the setups name.
+ *   setups   one per distinct (identification, setup) pair, HOST memory in both variants; each is built once, with exactly the
+ *            checks of symgpu_vorbis_fe_create.
+ *   jobs     one per audio packet: its byte range in `bytes`, and the reader's leading discard and page end trim for it
+ *            (what symgpu_vorbis_packet_durations and symgpu_ogg_page_end_trims give).
+ *   groups   one per file: jobs [first_job, first_job + n_jobs) in stream order and the setup they use.  HOST memory in both
+ *            variants.
+ *   out      samples of `format`: file g's output starts at groups[g].out_offset (in samples) and holds results[g].frames frames
+ *            of results[g].channels interleaved samples; its region is n_jobs x blocksize_1 / 2 x channels samples.
+ *   results  one per group;  status  one SYMGPU_VORBIS_JOB_* per job (a job that no group names is left undecoded: REFUSED).
+ * A packet is decoded exactly when symgpu_vorbis_fe_decode_packets decodes it, with the same units, floor values and residue
+ * bits.  Trims as decode.ogg_vorbis_plan applies them: trim_start = min(discard, frames), trim_end = min(trim_end, frames -
+ * trim_start), and a file's first decoded packet is silenced (frames = (prev_n + n) / 4).  The call registers one Vorbis stream
+ * per group and every setup's floors once, as symgpu_vorbis_streams_set / symgpu_vorbis_floors_set do: it REPLACES whatever
+ * Vorbis streams, slots or floors the context held.  The streams' overlap state after the call is unspecified.  Per call: at
+ * most SYMGPU_VORBIS_MAX_FILES groups, and the setups' floors together fewer than 0xffff.  The number of launches does not
+ * depend on the number of files. */
+#define SYMGPU_VORBIS_MAX_FILES 65536
+typedef struct symgpu_vorbis_job {          /* 24 bytes */
+    uint64_t offset;
+    uint32_t len;
+    uint32_t discard;                       /* leading frames the reader discards from this packet                             */
+    uint32_t trim_end;                      /* frames the reader trims from its end                                            */
+    uint32_t reserved;
+} symgpu_vorbis_job;
+typedef struct symgpu_vorbis_setup_ref {    /* 24 bytes */
+    uint64_t ident_offset;                  /* the 30-byte identification packet in `headers`                                  */
+    uint64_t setup_offset;                  /* the setup packet in `headers`                                                   */
+    uint32_t ident_len;
+    uint32_t setup_len;
+} symgpu_vorbis_setup_ref;
+typedef struct symgpu_vorbis_group {        /* 24 bytes */
+    uint64_t out_offset;                    /* first sample of the file's output in `out`; a multiple of the setup's channels   */
+    uint32_t first_job;
+    uint32_t n_jobs;
+    uint32_t setup;                         /* index into `setups`                                                              */
+    uint32_t reserved;
+} symgpu_vorbis_group;
+typedef struct symgpu_vorbis_group_result { /* 24 bytes */
+    uint64_t frames;                        /* interleaved frames written to the file's region                                  */
+    uint32_t sample_rate;                   /* the setup's                                                                      */
+    uint32_t packets;                       /* packets decoded                                                                  */
+    uint8_t channels;
+    uint8_t reserved[7];
+} symgpu_vorbis_group_result;
+enum {
+    SYMGPU_VORBIS_JOB_DECODED = 0,
+    SYMGPU_VORBIS_JOB_REFUSED = 1,          /* SYMGPU_ERR_DECODE in symgpu_vorbis_fe_decode, or no group names the job          */
+    SYMGPU_VORBIS_JOB_INVALID = 2           /* device variant only: the job's bytes lie outside `bytes`                          */
+};
+/* Host variant: every pointer is host memory.  Everything is validated before anything is launched: SYMGPU_ERR_ARG for a job
+ * outside `bytes`, a header outside `headers`, a group whose jobs lie outside the table or overlap another group's, a setup
+ * index out of range, an out_offset that is not a multiple of channels, an unknown format; what symgpu_vorbis_fe_create returns
+ * for a setup it refuses (SYMGPU_ERR_DECODE / _UNSUPPORTED); SYMGPU_ERR_LIMIT for more than SYMGPU_VORBIS_MAX_FILES groups,
+ * 0xffff floors or more, or a region that does not fit in `out` (out_bytes).  Stages through the context's staging buffer and
+ * returns when the results are in host memory; samples of `out` outside the written frames are left as they were. */
+symgpu_status symgpu_vorbis_decode_host(symgpu_ctx* ctx, const uint8_t* headers, size_t n_headers, const symgpu_vorbis_setup_ref* setups,
+                                        size_t n_setups, const uint8_t* bytes, size_t n_bytes, const symgpu_vorbis_job* jobs, size_t n_jobs,
+                                        const symgpu_vorbis_group* groups, size_t n_groups, int format, void* out, size_t out_bytes,
+                                        symgpu_vorbis_group_result* results, uint8_t* status);
+/* Device variant: bytes, jobs, out, results and status are device memory; headers, setups and groups host memory, validated on
+ * the host as above, and the kernels check each job's byte range (SYMGPU_VORBIS_JOB_INVALID).  The host waits for the context
+ * stream only where the stream and floor registration does (it replaces device buffers); everything after it is queued without
+ * a wait, and the call returns with the decode, the synthesis and the output stage still queued.  Scratch from the context's
+ * staging buffer: about 24 x slot + 600 bytes per job (slot = the largest blocksize_1 / 2 among the groups' setups) plus one
+ * partition-class buffer per job of its setup's size, and the setups' codebooks in flat form. */
+symgpu_status symgpu_vorbis_decode_dev(symgpu_ctx* ctx, const uint8_t* headers, size_t n_headers, const symgpu_vorbis_setup_ref* setups,
+                                       size_t n_setups, const uint8_t* bytes, size_t n_bytes, const symgpu_vorbis_job* jobs, size_t n_jobs,
+                                       const symgpu_vorbis_group* groups, size_t n_groups, int format, void* out, size_t out_bytes,
+                                       symgpu_vorbis_group_result* results, uint8_t* status);
+
 /* ===================================================================================================
  * MPEG Layer I / II sample decoders (SURVEY 8f N1 for the Layer I / II path): a packet becomes the sub-band samples
  * symgpu_mpa12_synth_* take.  CPU only, stateless apart from the stream's signal specification.

@@ -121,6 +121,15 @@ AAC_GROUP_DTYPE = np.dtype([("out_offset", "<u8"), ("first_job", "<u4"), ("n_job
 AAC_RESULT_DTYPE = np.dtype([("frames", "<u8"), ("sample_rate", "<u4"), ("packets", "<u4"), ("channels", "u1"), ("reserved", "u1", (7,))])
 assert AAC_GROUP_DTYPE.itemsize == 24 and AAC_RESULT_DTYPE.itemsize == 24
 AAC_JOB_DECODED, AAC_JOB_REFUSED, AAC_JOB_UNSUPPORTED, AAC_JOB_INVALID = 0, 1, 2, 3
+# device Vorbis decoding: `symgpu_vorbis_job`, `symgpu_vorbis_setup_ref`, `symgpu_vorbis_group`, `symgpu_vorbis_group_result` (24 bytes each)
+VORBIS_JOB_DTYPE = np.dtype([("offset", "<u8"), ("len", "<u4"), ("discard", "<u4"), ("trim_end", "<u4"), ("reserved", "<u4")])
+VORBIS_SETUP_REF_DTYPE = np.dtype([("ident_offset", "<u8"), ("setup_offset", "<u8"), ("ident_len", "<u4"), ("setup_len", "<u4")])
+VORBIS_GROUP_DTYPE = np.dtype([("out_offset", "<u8"), ("first_job", "<u4"), ("n_jobs", "<u4"), ("setup", "<u4"), ("reserved", "<u4")])
+VORBIS_RESULT_DTYPE = np.dtype([("frames", "<u8"), ("sample_rate", "<u4"), ("packets", "<u4"), ("channels", "u1"), ("reserved", "u1", (7,))])
+assert VORBIS_JOB_DTYPE.itemsize == 24 and VORBIS_SETUP_REF_DTYPE.itemsize == 24
+assert VORBIS_GROUP_DTYPE.itemsize == 24 and VORBIS_RESULT_DTYPE.itemsize == 24
+VORBIS_JOB_DECODED, VORBIS_JOB_REFUSED, VORBIS_JOB_INVALID = 0, 1, 2
+VORBIS_MAX_FILES = 65536
 MP3_FILE_DTYPE = np.dtype([("data", "<u8"), ("n", "<u8"), ("packets", "<u8"), ("n_packets", "<u8"), ("stream", "<u4"), ("reserved", "<u4")])
 assert MP3_FILE_DTYPE.itemsize == 40
 VORBIS_SETUP_INFO_DTYPE = np.dtype([("n_codebooks", "<u4"), ("n_floors", "<u4"), ("n_residues", "<u4"), ("n_mappings", "<u4"), ("n_modes", "<u4"),
@@ -290,6 +299,10 @@ def lib():
         fn = getattr(L, name)
         fn.restype = ctypes.c_int
         fn.argtypes = [vp, vp, sz, vp, sz, vp, sz, ctypes.c_int, vp, sz, vp, vp, ctypes.POINTER(ctypes.c_uint32)]
+    for name in ("symgpu_vorbis_decode_host", "symgpu_vorbis_decode_dev"):
+        fn = getattr(L, name)
+        fn.restype = ctypes.c_int
+        fn.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, sz, vp, sz, ctypes.c_int, vp, sz, vp, vp]
     L.symgpu_vorbis_fe_create.restype = ctypes.c_int
     L.symgpu_vorbis_fe_create.argtypes = [vp, sz, vp, sz, ctypes.POINTER(vp)]
     L.symgpu_vorbis_fe_destroy.restype = None

@@ -1,7 +1,8 @@
 // Vorbis entropy front-end (include/symgpu.h "Vorbis entropy front-end", SURVEY §8f N1): codebooks, floor-1 packet
 // decode, residue decode and the packet-level bookkeeping of VorbisDecoder::decode_inner up to -- not including --
 // inverse coupling (symphonia-codec-vorbis/src/{codebook,floor,residue,lib}.rs).  Output: what symgpu_vorbis_synth_*
-// reads.  CPU only.
+// reads.  The per-packet rules are those of vorbis_entropy.h (shared with the device decoder); this file builds the setup
+// (codebooks, canonical codes, VQ tables) in their flat form and runs them packet after packet.
 //
 // Floating point, bit-exact by construction: a VQ table value is `m * delta + min (+ last)` in f32 in that order, a
 // residue element the running f32 sum of the vectors laid over it in pass order -- the same single IEEE operations in
@@ -17,6 +18,7 @@
 
 #include "../../include/symgpu.h"
 #include "../../include/symgpu/packetizer.hpp"
+#include "vorbis_entropy.h"
 
 namespace {
 
@@ -38,85 +40,13 @@ float float32_unpack(uint32_t x) {  // codebook.rs:16-27
     return (x & 0x80000000u) ? -value : value;
 }
 
-// The reference's BitReaderRtl, state for state (symphonia-core/src/io/bit.rs:941-1027, :1211-1250, :1305-1370).  In a Vorbis audio
-// packet running out of bits is legal and decoding CONTINUES (the next channel's floor, the next sub-map's residue), so which
-// bits a failed read leaves behind is observable: the reference keeps a 64-bit cache that it refills 8 bytes at a time, a read
-// that fails on the FIRST refill consumes nothing, one that fails on a later refill has already dropped the cache it started
-// with.  A simpler reader would differ on truncated packets; this one follows the cache.
-struct PacketBits {
-    const uint8_t* p;
-    size_t n;         // bytes not yet fetched
-    uint64_t bits = 0;
-    uint32_t left = 0;
-    PacketBits(const uint8_t* data, size_t len) : p(data), n(len) {}
-    bool fetch() {  // fetch_bits: replace the cache with the next (up to) 8 bytes
-        const size_t k = n < 8 ? n : 8;
-        if (k == 0) return false;
-        uint64_t v = 0;
-        for (size_t i = 0; i < k; ++i) v |= uint64_t(p[i]) << (8 * i);
-        p += k, n -= k, bits = v, left = uint32_t(8 * k);
-        return true;
-    }
-    void top_up() {  // fetch_bits_partial: fill the free whole bytes of the cache
-        size_t k = (64 - left) >> 3;
-        if (k > n) k = n;
-        for (size_t i = 0; i < k; ++i) bits |= uint64_t(p[i]) << left, left += 8;
-        p += k, n -= k;
-    }
-    void consume(uint32_t w) { left -= w, bits = w < 64 ? bits >> w : 0; }
-    bool read(uint32_t width, uint32_t& out) {  // read_bits_leq32
-        uint64_t acc = bits;
-        uint32_t needed = width;
-        while (needed > left) {
-            needed -= left;
-            if (!fetch()) return false;
-            acc |= bits << (width - needed);
-        }
-        consume(needed);
-        out = uint32_t(acc & (width >= 32 ? 0xffffffffull : ((1ull << width) - 1)));
-        return true;
-    }
-    bool read_bool(bool& out) {
-        if (left < 1 && !fetch()) return false;
-        out = bits & 1;
-        consume(1);
-        return true;
-    }
-};
-
-struct Codebook {
+struct Codebook {  // as read_codebook builds it; appended to the setup's pools (vorbise::Book)
     uint16_t dims = 0;
     bool has_vq = false;
     std::vector<float> vq;           // [entries][dims]
     std::vector<int32_t> child;      // binary trie: child[2 * node + bit] = node index, or ~value for a leaf, or 0 = no such code
     uint32_t max_len = 0;
     uint32_t lut[1024] = {};         // next ten stream bits (first bit = bit 0) -> (value + 1) << 6 | length, 0 = a longer code
-    // One codeword, first stream bit = root of the tree (codebook.rs:366-369 "BitOrder::Reverse"; bit.rs:1211-1250): the cache is
-    // topped up, the code is matched against it padded with zeros, and must then fit in what the cache really holds -- else the
-    // packet has ended and nothing is consumed.
-    bool read(PacketBits& bs, uint32_t& value) const {
-        if (bs.left < max_len) bs.top_up();
-        const uint32_t e = lut[bs.bits & 1023];  // codes of up to ten bits: one look-up (the cache holds zeros above `left`)
-        if (e) {
-            const uint32_t len = e & 63;
-            if (len > bs.left) return false;
-            bs.consume(len);
-            return value = (e >> 6) - 1, true;
-        }
-        int32_t node = 0;
-        for (uint32_t depth = 0; depth < 64; ++depth) {
-            const uint32_t bit = uint32_t(bs.bits >> depth) & 1;
-            const int32_t next = child[size_t(2 * node) + bit];
-            if (next < 0) {
-                if (depth + 1 > bs.left) return false;
-                bs.consume(depth + 1);
-                return value = uint32_t(~next), true;
-            }
-            if (next == 0) return false;  // cannot happen in a fully specified tree
-            node = next;
-        }
-        return false;
-    }
 };
 
 // Canonical codeword assignment (Vorbis I 3.2.1): each entry, in order, takes the lowest-valued free leaf of its length.
@@ -250,140 +180,85 @@ int read_codebook(BitReaderRtl& bs, Codebook& cb) {
 
 }  // namespace
 
+namespace ve = symgpu::vorbise;
+
 struct symgpu_vorbis_fe {
     VorbisIdent ident{};
     VorbisSetup setup;
-    std::vector<Codebook> books;
+    // the setup in the flat form of vorbis_entropy.h
+    std::vector<ve::Book> books;
+    std::vector<uint32_t> lut;
+    std::vector<int32_t> child;
+    std::vector<float> vq;
+    std::vector<ve::Mapping> mappings;
+    std::vector<ve::Mode> modes;
+    uint32_t class_cap = 0;
+    ve::Setup view{};
     int prev_block_flag = -1;
-    std::vector<float> type2;
     std::vector<uint8_t> part_classes;  // persistent across packets, see read_residue
+    ve::ClassBuf classes{};
 };
 
 namespace {
 
-// floor.rs:655-722.  Returns false when the floor is unused (flag clear, or the packet ended inside it).
-bool read_floor1(const symgpu_vorbis_fe& fe, const VorbisFloor1Setup& f, PacketBits& bs, uint16_t* y) {
-    bool used;
-    if (!bs.read_bool(used) || !used) return false;
-    static const uint32_t ranges[4] = {256, 128, 86, 64};
-    const uint32_t bits = vorbis_ilog(ranges[f.multiplier - 1] - 1);
-    uint32_t v;
-    if (!bs.read(bits, v)) return false;
-    y[0] = uint16_t(v);
-    if (!bs.read(bits, v)) return false;
-    y[1] = uint16_t(v);
-    int offset = 2;
-    for (int p = 0; p < f.partitions; ++p) {
-        const auto& cl = f.classes[f.partition_class[p]];
-        const uint32_t cbits = cl.subclass_bits, csub = (1u << cbits) - 1;
-        uint32_t cval = 0;
-        if (cbits && !fe.books[cl.mainbook].read(bs, cval)) return false;
-        for (int d = 0; d < cl.dimensions; ++d) {
-            const uint32_t sub = cval & csub;
-            cval >>= cbits;
-            v = 0;
-            if (cl.subbook_used & (1u << sub))
-                if (!fe.books[cl.subbooks[sub]].read(bs, v)) return false;
-            y[offset + d] = uint16_t(v);
-        }
-        offset += cl.dimensions;
-    }
-    return true;
+void append_book(symgpu_vorbis_fe& fe, const Codebook& cb) {
+    ve::Book b{};
+    b.lut = uint32_t(fe.lut.size()), b.child = uint32_t(fe.child.size()), b.vq = uint32_t(fe.vq.size());
+    b.max_len = cb.max_len, b.dims = cb.dims, b.has_vq = cb.has_vq;
+    fe.lut.insert(fe.lut.end(), cb.lut, cb.lut + 1024);
+    fe.child.insert(fe.child.end(), cb.child.begin(), cb.child.end());
+    fe.vq.insert(fe.vq.end(), cb.vq.begin(), cb.vq.end());
+    fe.books.push_back(b);
 }
 
-// residue.rs:451-477
-void decode_classes(uint32_t val, unsigned per_word, uint32_t classifications, uint8_t* out, size_t n_out) {
-    unsigned skip = 0;
-    if (per_word > n_out) {
-        skip = unsigned(per_word - n_out);
-        for (unsigned k = 0; k < skip; ++k) val /= classifications;
+// Pools, mappings and modes in place: the pointers of fe.view, and the class vector sized for the setup's largest residue.
+void finish_setup(symgpu_vorbis_fe& fe) {
+    for (const auto& m : fe.setup.mappings) {
+        ve::Mapping o{};
+        o.n_submaps = m.n_submaps, o.coupled = uint8_t(m.couplings.empty() ? 0 : 1);
+        for (size_t c = 0; c < m.multiplex.size() && c < 2; ++c) o.multiplex[c] = m.multiplex[c];
+        std::memcpy(o.submap_floor, m.submap_floor, 16), std::memcpy(o.submap_residue, m.submap_residue, 16);
+        fe.mappings.push_back(o);
     }
-    for (size_t k = per_word - skip; k-- > 0;) out[k] = uint8_t(val % classifications), val /= classifications;
+    for (const auto& md : fe.setup.modes) fe.modes.push_back(ve::Mode{uint8_t(md.first), md.second});
+    const size_t n2 = (size_t(1) << fe.ident.bs1_exp) >> 1, ch = fe.ident.n_channels;
+    for (const VorbisResidueSetup& r : fe.setup.residues) {  // a short block's partitions are never more than a long block's
+        const size_t full = r.type == 2 ? n2 * ch : n2;
+        const size_t begin = std::min<size_t>(r.begin, full), end = std::min<size_t>(r.end, full);
+        const size_t parts = r.partition_size ? (end - begin) / r.partition_size : 0;
+        fe.class_cap = std::max<uint32_t>(fe.class_cap, uint32_t(r.type == 2 ? parts : parts * ch));
+    }
+    fe.part_classes.assign(std::max<uint32_t>(fe.class_cap, 1), 0);
+    fe.classes = ve::ClassBuf{fe.part_classes.data(), 0, fe.class_cap};
+    ve::Setup& v = fe.view;
+    v.books = fe.books.data(), v.lut = fe.lut.data(), v.child = fe.child.data(), v.vq = fe.vq.data();
+    v.floors = fe.setup.floor1.data(), v.residues = fe.setup.residues.data(), v.mappings = fe.mappings.data(), v.modes = fe.modes.data();
+    v.n_modes = uint32_t(fe.setup.modes.size()), v.bs0_exp = fe.ident.bs0_exp, v.bs1_exp = fe.ident.bs1_exp, v.channels = fe.ident.n_channels;
 }
 
-// One partition: residue.rs:479-543.  false: the packet ended (legal: decoding stops), `bad` set: malformed setup.
-bool read_partition(const Codebook& book, PacketBits& bs, float* out, size_t n, bool format0, bool& bad) {
-    if (!book.has_vq) return bad = true, false;  // "vorbis: not a vq codebook"
-    const size_t dim = book.dims;
-    if (format0) {
-        const size_t step = n / dim;
-        for (size_t i = 0; i < step; ++i) {
-            uint32_t e;
-            if (!book.read(bs, e)) return false;
-            const float* v = book.vq.data() + size_t(e) * dim;
-            for (size_t k = 0, o = i; k < dim && o < n; ++k, o += step) out[o] += v[k];
-        }
-    } else {
-        for (size_t o = 0; o + dim <= n; o += dim) {
-            uint32_t e;
-            if (!book.read(bs, e)) return false;
-            const float* v = book.vq.data() + size_t(e) * dim;
-            for (size_t k = 0; k < dim; ++k) out[o + k] += v[k];
-        }
-    }
-    return true;
-}
-
-// residue.rs:142-449 for the channels in `chans` (1 or 2 of them).  0 ok, 1 decode error.
-int read_residue(symgpu_vorbis_fe& fe, const VorbisResidueSetup& r, PacketBits& bs, unsigned bs_exp, const int* chans, int n_chans,
-                 const uint8_t* do_not_decode, float* residue, uint32_t slot) {
-    const Codebook& class_book = fe.books[r.classbook];
-    const size_t n2 = (size_t(1) << bs_exp) >> 1;
-    const size_t full = r.type == 2 ? n2 * size_t(n_chans) : n2;
-    const size_t begin = std::min<size_t>(r.begin, full), end = std::min<size_t>(r.end, full);
-    const size_t part_size = r.partition_size, per_word = class_book.dims, parts = (end - begin) / part_size;
-    bool any = false;
-    for (int c = 0; c < n_chans; ++c) any |= !do_not_decode[chans[c]];
-    float* target[2] = {nullptr, nullptr};
-    if (r.type == 2) {
-        fe.type2.assign(full, 0.0f);
-    } else {
-        for (int c = 0; c < n_chans; ++c) target[c] = residue + size_t(chans[c]) * slot;  // already zeroed by the caller
-    }
-    // the partition classes live in a vector that only ever grows and is never cleared (residue.rs:434-441): what a class word
-    // writes is bounded by the vector's END, not by this packet's partition count, so a class word of the last group can spill
-    // into the next channel's entries and stale entries of earlier packets stay behind -- reproduced, because later passes read them
-    {
-        const size_t class_slots = r.type == 2 ? parts : parts * size_t(n_chans);
-        if (fe.part_classes.size() < class_slots) fe.part_classes.resize(class_slots, 0);
-    }
-    if (any) {
-        bool bad = false, ended = false;
-        for (unsigned pass = 0; pass <= r.max_pass && !ended; ++pass)
-            for (size_t first = 0; first < parts && !ended; first += per_word) {
-                if (pass == 0)
-                    for (int c = 0; c < (r.type == 2 ? 1 : n_chans) && !ended; ++c) {
-                        if (r.type != 2 && do_not_decode[chans[c]]) continue;
-                        uint32_t code;
-                        if (!class_book.read(bs, code)) {
-                            ended = true;
-                            break;
-                        }
-                        const size_t base = first + size_t(c) * parts;
-                        decode_classes(code, unsigned(per_word), r.classifications, fe.part_classes.data() + base, fe.part_classes.size() - base);
-                    }
-                const size_t last = std::min(parts, first + per_word);
-                for (size_t part = first; part < last && !ended; ++part)
-                    for (int c = 0; c < (r.type == 2 ? 1 : n_chans) && !ended; ++c) {
-                        if (r.type != 2 && do_not_decode[chans[c]]) continue;
-                        const uint8_t cls = fe.part_classes[part + parts * size_t(c)];
-                        if (!(r.used[cls] & (1u << pass))) continue;
-                        const size_t start = begin + part_size * part;
-                        float* out = (r.type == 2 ? fe.type2.data() : target[c]) + start;
-                        if (!read_partition(fe.books[r.books[cls][pass]], bs, out, part_size, r.type == 0, bad)) ended = true;
-                    }
-            }
-        if (bad) return 1;
-    }
-    if (r.type == 2)  // de-interleave (residue.rs:177-218)
-        for (int c = 0; c < n_chans; ++c) {
-            float* out = residue + size_t(chans[c]) * slot;
-            for (size_t i = 0; i < n2; ++i) out[i] = fe.type2[i * size_t(n_chans) + size_t(c)];
-        }
-    return 0;
+template <class T>
+uint64_t put(std::vector<uint8_t>& blob, const T* p, size_t n) {
+    const uint64_t at = (blob.size() + 15) & ~uint64_t(15);
+    blob.resize(size_t(at) + n * sizeof(T));
+    if (n) std::memcpy(blob.data() + at, p, n * sizeof(T));
+    return at;
 }
 
 }  // namespace
+
+void symgpu::vorbise::setup_export(const symgpu_vorbis_fe* fe, std::vector<uint8_t>& blob, SetupHead& h) {
+    h = SetupHead{};
+    h.books = put(blob, fe->books.data(), fe->books.size());
+    h.lut = put(blob, fe->lut.data(), fe->lut.size());
+    h.child = put(blob, fe->child.data(), fe->child.size());
+    h.vq = put(blob, fe->vq.data(), fe->vq.size());
+    h.floors = put(blob, fe->setup.floor1.data(), fe->setup.floor1.size());
+    h.residues = put(blob, fe->setup.residues.data(), fe->setup.residues.size());
+    h.mappings = put(blob, fe->mappings.data(), fe->mappings.size());
+    h.modes = put(blob, fe->modes.data(), fe->modes.size());
+    h.n_modes = uint32_t(fe->modes.size()), h.class_cap = fe->class_cap;
+    h.bs0_exp = fe->ident.bs0_exp, h.bs1_exp = fe->ident.bs1_exp, h.channels = fe->ident.n_channels, h.sample_rate = fe->ident.sample_rate;
+}
 
 extern "C" symgpu_status symgpu_vorbis_fe_create(const uint8_t* ident, size_t n_ident, const uint8_t* setup, size_t n_setup, symgpu_vorbis_fe** out) {
     if (!ident || !setup || !out) return SYMGPU_ERR_ARG;
@@ -395,9 +270,11 @@ extern "C" symgpu_status symgpu_vorbis_fe_create(const uint8_t* ident, size_t n_
     // the codebooks once more, this time built (the walk above only checked their syntax)
     BitReaderRtl bs(setup + 7, n_setup - 7);
     const uint32_t n_books = bs.read(8) + 1;
-    fe->books.resize(n_books);
-    for (uint32_t k = 0; k < n_books; ++k)
-        if (read_codebook(bs, fe->books[k])) return SYMGPU_ERR_DECODE;
+    for (uint32_t k = 0; k < n_books; ++k) {
+        Codebook cb;
+        if (read_codebook(bs, cb)) return SYMGPU_ERR_DECODE;
+        append_book(*fe, cb);
+    }
     // residue partitions must fit the blocks they are laid over (the reference would panic slicing past the vector)
     // -- checked per packet; here: what the synthesis kernel cannot take
     if (fe->ident.n_channels > 2) return SYMGPU_ERR_UNSUPPORTED;
@@ -424,6 +301,7 @@ extern "C" symgpu_status symgpu_vorbis_fe_create(const uint8_t* ident, size_t n_
     for (size_t k = 1; k < fe->setup.modes.size(); ++k)
         if (fe->setup.mappings[fe->setup.modes[k].second].couplings.size() != fe->setup.mappings[fe->setup.modes[0].second].couplings.size())
             return SYMGPU_ERR_UNSUPPORTED;
+    finish_setup(*fe);
     *out = fe.release();
     return SYMGPU_OK;
 }
@@ -451,53 +329,9 @@ extern "C" symgpu_status symgpu_vorbis_fe_decode(symgpu_vorbis_fe* fe, const uin
                                                  symgpu_vorbis_unit* unit, uint16_t* floor_y, float* residue) {
     if (!fe || (!packet && n) || !unit || !floor_y || !residue) return SYMGPU_ERR_ARG;
     if (slot < ((1u << fe->ident.bs1_exp) >> 1)) return SYMGPU_ERR_ARG;
-    PacketBits bs(packet, n);
-    bool flag;
-    if (!bs.read_bool(flag) || flag) return SYMGPU_ERR_DECODE;  // lib.rs:151-154
-    const size_t n_modes = fe->setup.modes.size();
-    uint32_t mode_number;
-    if (!bs.read(vorbis_ilog(uint32_t(n_modes - 1)), mode_number) || mode_number >= n_modes) return SYMGPU_ERR_DECODE;
-    const bool long_block = fe->setup.modes[mode_number].first;
-    const VorbisMappingSetup& mapping = fe->setup.mappings[fe->setup.modes[mode_number].second];
-    if (long_block) {  // previous / next window flags: read, not used (lib.rs:168-173)
-        if (!bs.read_bool(flag) || !bs.read_bool(flag)) return SYMGPU_ERR_DECODE;
-    }
-    const unsigned bs_exp = long_block ? fe->ident.bs1_exp : fe->ident.bs0_exp;
-    const int n_ch = fe->ident.n_channels;
-    std::memset(unit, 0, sizeof *unit);
-    std::memset(floor_y, 0, sizeof(uint16_t) * 2 * 65);
-    std::memset(residue, 0, sizeof(float) * 2 * size_t(slot));
-    unit->block_flag = long_block;
-    unit->prev_block_flag = uint8_t(fe->prev_block_flag < 0 ? long_block : fe->prev_block_flag);
-    unit->floor[0] = unit->floor[1] = 0xffff, unit->do_not_decode[0] = unit->do_not_decode[1] = 1;
-    // floors, one per channel (lib.rs:184-207).  A packet that ends inside a floor leaves that floor unused and everything
-    // behind it unread -- which the reader reports by failing every later read, exactly the reference's behaviour.
-    for (int ch = 0; ch < n_ch; ++ch) {
-        const uint8_t floor_idx = mapping.submap_floor[mapping.multiplex[ch]];
-        if (uint64_t(floor_base) + floor_idx >= 0xffffu) return SYMGPU_ERR_LIMIT; // unit->floor is 16 bits, 0xffff = unused
-        const bool used = read_floor1(*fe, fe->setup.floor1[floor_idx], bs, floor_y + ch * 65);
-        unit->do_not_decode[ch] = !used;
-        unit->floor[ch] = used ? uint16_t(floor_base + floor_idx) : uint16_t(0xffff);
-        if (!used) std::memset(floor_y + ch * 65, 0, sizeof(uint16_t) * 65);
-    }
-    // non-zero vector propagate (lib.rs:213-225)
-    for (const auto& cp : mapping.couplings)
-        if (unit->do_not_decode[cp.first] != unit->do_not_decode[cp.second]) unit->do_not_decode[cp.first] = unit->do_not_decode[cp.second] = 0;
-    // residues, per sub-map (lib.rs:229-248)
-    for (int sm = 0; sm < mapping.n_submaps; ++sm) {
-        int chans[2], n_chans = 0;
-        for (int ch = 0; ch < n_ch; ++ch)
-            if (mapping.multiplex[ch] == sm) chans[n_chans++] = ch;
-        const VorbisResidueSetup& r = fe->setup.residues[mapping.submap_residue[sm]];
-        if (n_chans == 0) continue;  // (the reference still runs the residue over no channels: nothing is read for types 0 / 1;
-                                     //  type 2 divides by the channel count: a malformed setup, refuse it)
-        // the partitions must lie inside the vector they are added to
-        const size_t n2 = (size_t(1) << bs_exp) >> 1, full = r.type == 2 ? n2 * size_t(n_chans) : n2;
-        const size_t begin = std::min<size_t>(r.begin, full), end = std::min<size_t>(r.end, full);
-        if (fe->books[r.classbook].dims == 0 || begin + ((end - begin) / r.partition_size) * size_t(r.partition_size) > full) return SYMGPU_ERR_DECODE;
-        if (read_residue(*fe, r, bs, bs_exp, chans, n_chans, unit->do_not_decode, residue, slot)) return SYMGPU_ERR_DECODE;
-    }
-    fe->prev_block_flag = long_block;
+    const symgpu_status st = ve::decode_packet(fe->view, packet, n, slot, floor_base, fe->prev_block_flag, fe->classes, unit, floor_y, residue);
+    if (st != SYMGPU_OK) return st;
+    fe->prev_block_flag = unit->block_flag;
     return SYMGPU_OK;
 }
 

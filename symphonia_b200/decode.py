@@ -801,3 +801,105 @@ def decode_mpeg_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False
             empty = torch.empty((0, 0), dtype=getattr(torch, _TORCH_DTYPES[fmt]), device=torch.device("cuda", engine.device))
         result[i] = (empty, 0)
     return result
+
+
+# ---- Ogg Vorbis, many files decoded on the device (codebooks, floors, residues in device code) --------------------------------
+
+def vorbis_files_plan(files, threads=None, errors=None):
+    """Host half of decode_vorbis_files: every file indexed (ogg_vorbis_index, on `threads` host threads), the gathered logical
+    streams concatenated once, one job per audio packet with the reader's leading discard and page end trim, files with
+    byte-identical identification and setup headers sharing one setup, and one group per file.  Returns dict(data, headers,
+    setups, jobs, groups, out_samples, failed).  A file that cannot be indexed or opened -- not Ogg, more than two channels, floor
+    type 0, ... (listed in `failed`) -- gets a group without jobs; its message goes to errors[i] when `errors` is a dict."""
+    import concurrent.futures
+    import os
+    messages = {}
+
+    def index(i):
+        try:
+            ix = ogg_vorbis_index(files[i])
+            ix["fe"].close()   # (it checked the setup; the device call builds its own)
+            return ix
+        except Exception as e:  # noqa: BLE001 -- one bad file must not abort the batch; its message is kept
+            messages[i] = f"{type(e).__name__}: {e}"
+            return None
+    with concurrent.futures.ThreadPoolExecutor(max_workers=threads or os.cpu_count()) as pool:
+        ix = list(pool.map(index, range(len(files))))
+    if errors is not None:
+        errors.update(messages)
+    good = [i for i in range(len(files)) if ix[i] is not None]
+    data = np.concatenate([ix[i]["blob"] for i in good]) if good else np.zeros(0, dtype=np.uint8)
+    groups = np.zeros(len(files), dtype=nat.VORBIS_GROUP_DTYPE)
+    setup_of, headers, refs = {}, [], []
+    jobs, byte_at, job_at, out_at, head_at = [], 0, 0, 0, 0
+    for i in good:
+        x = ix[i]
+        ident_b, setup_b = x["headers"]
+        key = (ident_b, setup_b)
+        if key not in setup_of:
+            setup_of[key] = len(refs)
+            refs.append((head_at, head_at + len(ident_b), len(ident_b), len(setup_b)))
+            headers += [ident_b, setup_b]
+            head_at += len(ident_b) + len(setup_b)
+        n, channels = len(x["table"]), int(x["ident"]["channels"])
+        g = groups[i]
+        g["out_offset"], g["first_job"], g["n_jobs"], g["setup"] = out_at, job_at, n, setup_of[key]
+        j = np.zeros(n, dtype=nat.VORBIS_JOB_DTYPE)
+        j["offset"], j["len"] = x["table"]["offset"] + np.uint64(byte_at), x["table"]["len"]
+        j["discard"] = np.clip(x["discard"], 0, 0xffffffff)
+        j["trim_end"] = np.clip(x["trim_end"], 0, 0xffffffff)
+        jobs.append(j)
+        byte_at += x["blob"].size
+        job_at += n
+        out_at += n * ((1 << int(x["ident"]["bs1_exp"])) >> 1) * channels
+    failed = [i for i in range(len(files)) if ix[i] is None]
+    groups["out_offset"][failed] = out_at
+    groups["first_job"][failed] = job_at
+    setups = np.zeros(len(refs), dtype=nat.VORBIS_SETUP_REF_DTYPE)
+    for k, r in enumerate(refs):
+        setups[k] = r
+    jobs = np.concatenate(jobs) if jobs else np.zeros(0, dtype=nat.VORBIS_JOB_DTYPE)
+    return dict(data=data, headers=b"".join(headers), setups=setups, jobs=jobs, groups=groups, out_samples=out_at, failed=failed)
+
+
+def decode_vorbis_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False, errors=None, stats=None):
+    """[(samples [frames, channels] of `fmt`, sample_rate)] for a list of Ogg Vorbis files (mono / stereo, floor 1), each equal to
+    decode_ogg_vorbis(engine, file, fmt): the files are indexed on host threads, and ONE device call decodes every audio packet of
+    every file -- codebooks, floors and residues in device code, synthesis and the output stage on the GPU.  device=True: the
+    bytes go to the device once and the samples are CUDA tensors, views of one output tensor.  A file that cannot be indexed or
+    opened yields an empty result with sample rate 0 (its message in errors[i] when `errors` is a dict), and the others still
+    decode.  stats: a dict that receives the per-packet `status` and `n_setups`, the number of distinct setups.  Replaces the
+    engine's Vorbis stream and floor registration, as decode_ogg_vorbis does.  At most 65 536 files per call."""
+    if len(files) > nat.VORBIS_MAX_FILES:
+        raise ValueError(f"decode_vorbis_files takes at most {nat.VORBIS_MAX_FILES} files per call, not {len(files)}")
+    plan = vorbis_files_plan(files, threads, errors)
+    groups, cap, setups = plan["groups"], plan["out_samples"], plan["setups"]
+    if device:
+        import torch
+        dev = torch.device("cuda", engine.device)
+        out = torch.empty(cap, dtype=getattr(torch, _TORCH_DTYPES[fmt]), device=dev)
+        results_t = torch.zeros(len(groups) * nat.VORBIS_RESULT_DTYPE.itemsize, dtype=torch.uint8, device=dev)
+        status_t = torch.empty(len(plan["jobs"]), dtype=torch.uint8, device=dev)
+        if len(setups):
+            as_t = lambda a: torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(-1)).to(dev)  # noqa: E731
+            data_t, jobs_t = as_t(plan["data"]), as_t(plan["jobs"])
+            torch.cuda.current_stream(dev).synchronize()  # the copies above are on torch's stream, the decode on the engine's
+            engine.vorbis_decode_dev(plan["headers"], setups, data_t, jobs_t, groups, fmt, out, results_t, status_t)
+            engine.sync()
+        results = results_t.cpu().numpy().view(nat.VORBIS_RESULT_DTYPE)
+        status = status_t.cpu().numpy()
+    elif len(setups):
+        out, results, status = engine.vorbis_decode_host(plan["headers"], setups, plan["data"], plan["jobs"], groups, fmt, cap)
+    else:   # no file could be opened: nothing to decode
+        out, results, status = np.zeros(0, dtype=nat.FMT_NUMPY[fmt]), np.zeros(len(groups), dtype=nat.VORBIS_RESULT_DTYPE), np.zeros(0, dtype=np.uint8)
+    if stats is not None:
+        stats.update(status=status, n_setups=len(setups))
+    failed = set(plan["failed"])
+    result = []
+    for g in range(len(groups)):
+        if g in failed:
+            result.append((out[:0].reshape(0, 0), 0))
+            continue
+        ch, at, n = int(results[g]["channels"]), int(groups[g]["out_offset"]), int(results[g]["frames"])
+        result.append((out[at:at + n * ch].reshape(n, ch), int(results[g]["sample_rate"])))
+    return result

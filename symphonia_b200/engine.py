@@ -351,6 +351,47 @@ class Engine:
                                                     out_t.numel() * out_t.element_size(), ptr(results_t), ptr(status_t), ctypes.byref(redone)))
         return redone.value
 
+    def vorbis_decode_host(self, headers, setups, data, jobs, groups, fmt, out_samples, out=None):
+        """Device Ogg Vorbis decoding of many files in one call: `headers` (bytes) holds the identification / setup packets that
+        `setups` (VORBIS_SETUP_REF_DTYPE, one per distinct pair) name, `data` the audio packets, jobs VORBIS_JOB_DTYPE (one per
+        packet, with the reader's discard / end trim), groups VORBIS_GROUP_DTYPE (one per file: its jobs, setup and output
+        offset).  Returns (out [out_samples] of `fmt`, results VORBIS_RESULT_DTYPE [groups], status uint8 [jobs]); file g's
+        samples are out[out_offset:][:frames * channels].  Replaces the engine's Vorbis stream and floor registration."""
+        from ._native import VORBIS_GROUP_DTYPE, VORBIS_JOB_DTYPE, VORBIS_RESULT_DTYPE, VORBIS_SETUP_REF_DTYPE
+        h = np.frombuffer(headers, dtype=np.uint8) if not isinstance(headers, np.ndarray) else np.ascontiguousarray(headers, dtype=np.uint8)
+        a = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
+        setups = np.ascontiguousarray(setups, dtype=VORBIS_SETUP_REF_DTYPE)
+        jobs = np.ascontiguousarray(jobs, dtype=VORBIS_JOB_DTYPE)
+        groups = np.ascontiguousarray(groups, dtype=VORBIS_GROUP_DTYPE)
+        if out is None:
+            out = np.zeros(int(out_samples), dtype=FMT_NUMPY[fmt])
+        assert out.flags.c_contiguous
+        results = np.zeros(len(groups), dtype=VORBIS_RESULT_DTYPE)
+        status = np.zeros(len(jobs), dtype=np.uint8)
+        opt = lambda x, n: _np_ptr(x) if n else None  # noqa: E731
+        self._check(self._lib.symgpu_vorbis_decode_host(self._ctx, opt(h, h.size), h.size, opt(setups, len(setups)), len(setups), opt(a, a.size), a.size,
+                                                        opt(jobs, len(jobs)), len(jobs), opt(groups, len(groups)), len(groups), int(fmt),
+                                                        opt(out, out.nbytes), out.nbytes, opt(results, len(groups)), opt(status, len(jobs))))
+        return out, results, status
+
+    def vorbis_decode_dev(self, headers, setups, data_t, jobs_t, groups, fmt, out_t, results_t, status_t):
+        """Device-resident variant: torch CUDA tensors (uint8 bytes, jobs / results as uint8 views of the records, `out` of the
+        format's element size, uint8 status); `headers`, `setups` and `groups` stay on the host.  The host waits only for the
+        stream / floor registration; the decode, the synthesis and the output stage are left queued on the engine's stream."""
+        from ._native import VORBIS_GROUP_DTYPE, VORBIS_JOB_DTYPE, VORBIS_RESULT_DTYPE, VORBIS_SETUP_REF_DTYPE
+        ts = (data_t, jobs_t, out_t, results_t, status_t)
+        assert all(t.is_cuda and t.is_contiguous() for t in ts)
+        h = np.frombuffer(headers, dtype=np.uint8) if not isinstance(headers, np.ndarray) else np.ascontiguousarray(headers, dtype=np.uint8)
+        setups = np.ascontiguousarray(setups, dtype=VORBIS_SETUP_REF_DTYPE)
+        groups = np.ascontiguousarray(groups, dtype=VORBIS_GROUP_DTYPE)
+        n_jobs = jobs_t.numel() * jobs_t.element_size() // VORBIS_JOB_DTYPE.itemsize
+        assert results_t.numel() * results_t.element_size() >= len(groups) * VORBIS_RESULT_DTYPE.itemsize and status_t.numel() >= n_jobs
+        ptr = lambda t: ctypes.c_void_p(t.data_ptr()) if t.numel() else None  # noqa: E731
+        self._check(self._lib.symgpu_vorbis_decode_dev(self._ctx, _np_ptr(h) if h.size else None, h.size, _np_ptr(setups) if len(setups) else None,
+                                                       len(setups), ptr(data_t), data_t.numel(), ptr(jobs_t), n_jobs,
+                                                       _np_ptr(groups) if len(groups) else None, len(groups), int(fmt), ptr(out_t),
+                                                       out_t.numel() * out_t.element_size(), ptr(results_t), ptr(status_t)))
+
     # -- output stage -------------------------------------------------------------------------
     def pcm_pack_host(self, pcm, spans, channels, fmt, out_frames, plane_stride=0, frames=0, n_spans=None, out=None):
         """Trim + interleave + convert planar f32 `pcm` (any shape, flat indexing) into [out_frames, channels]

@@ -92,12 +92,13 @@ TARGETS = {
         ("if (asc.object_type != 2 || asc.sbr_present || asc.channels > 2 || asc.samples != 1024) return SYMGPU_ERR_UNSUPPORTED;", "if (asc.object_type != 2 || asc.sbr_present || asc.channels > 2) return SYMGPU_ERR_UNSUPPORTED;"),
         ("case 35: case 36: case 37: case 38: case 39: case 40: case 41:", "case 35: case 36: case 37: case 38: case 39: case 40:"),
     ]),
-    "vorbis": dict(src="vorbis_frontend.cpp", prefix="symgpu_vorbis_fe_", tests=["tests/test_vorbis_frontend.py", "tests/test_zz_ogg_vorbis_to_pcm.py"], mutants=[
+    "vorbis": dict(src="vorbis_frontend.cpp", header="vorbis_entropy.h", prefix="symgpu_vorbis_fe_", tests=["tests/test_vorbis_frontend.py", "tests/test_zz_ogg_vorbis_to_pcm.py",
+                                                                                     "tests/test_vorbis_codeword_fit.py"], mutants=[
         ("size_t k = (64 - left) >> 3;", "size_t k = (63 - left) >> 3;"),
         ("            needed -= left;\n            if (!fetch()) return false;", "            if (!fetch()) return false;\n            needed -= left > needed ? needed : left;"),
         ("if (left < 1 && !fetch()) return false;", "if (left < 2 && !fetch()) return false;"),
-        ("if (bs.left < max_len) bs.top_up();", "if (bs.left <= max_len) bs.top_up();"),
-        ("if (bs.left < max_len) bs.top_up();", "bs.top_up();"),
+        ("if (bs.left < b.max_len) bs.top_up();", "if (bs.left <= b.max_len) bs.top_up();"),
+        ("if (bs.left < b.max_len) bs.top_up();", "bs.top_up();"),
         ("if (depth + 1 > bs.left) return false;", "if (depth > bs.left) return false;"),
         ("if (free_nodes[k].depth > len) continue;", "if (free_nodes[k].depth >= len) continue;"),
         ("if (v < best_value) best_value = v, best = int(k);", "if (v <= best_value) best_value = v, best = int(k);"),
@@ -107,27 +108,27 @@ TARGETS = {
         ("if (lens.size() == 1 && lens[0] == 1)", "if (lens.size() == 1 && lens[0] == 2)"),
         ("if (!bs.ok() || lookup > 2) return 1;", "if (!bs.ok() || lookup > 3) return 1;"),
         ("if (sequence) last = v;", "if (!sequence) last = v;"),
-        ("static const uint32_t ranges[4] = {256, 128, 86, 64};", "static const uint32_t ranges[4] = {256, 128, 85, 64};"),
-        ("static const uint32_t ranges[4] = {256, 128, 86, 64};", "static const uint32_t ranges[4] = {256, 129, 86, 64};"),
-        ("if (cbits && !fe.books[cl.mainbook].read(bs, cval)) return false;", "if (!fe.books[cl.mainbook].read(bs, cval)) return false;"),
+        ("f.multiplier == 3 ? 86u", "f.multiplier == 3 ? 85u"),
+        ("f.multiplier == 2 ? 128u", "f.multiplier == 2 ? 129u"),
+        ("if (cbits && !read_code(S, S.books[cl.mainbook], bs, cval)) return false;", "if (!read_code(S, S.books[cl.mainbook], bs, cval)) return false;"),
         ("            cval >>= cbits;\n", ""),
         ("if (per_word > n_out) {", "if (per_word >= n_out) {"),
-        ("for (size_t k = 0, o = i; k < dim && o < n; ++k, o += step) out[o] += v[k];", "for (size_t k = 0, o = i; k < dim && o < n; ++k, o += step) out[o] = v[k];"),
+        ("element(rows, lanes, start + o) += v[k];", "element(rows, lanes, start + o) = v[k];"),
         ("for (size_t o = 0; o + dim <= n; o += dim) {", "for (size_t o = 0; o + dim < n; o += dim) {"),
-        ("const size_t begin = std::min<size_t>(r.begin, full), end = std::min<size_t>(r.end, full);", "const size_t begin = r.begin, end = std::min<size_t>(r.end, full);"),
-        ("const size_t begin = std::min<size_t>(r.begin, full), end = std::min<size_t>(r.end, full);", "const size_t begin = std::min<size_t>(r.begin, full), end = std::min<size_t>(r.end, n2);"),
+        ("const size_t begin = min_sz(r.begin, full), end = min_sz(r.end, full);", "const size_t begin = r.begin, end = min_sz(r.end, full);"),
+        ("const size_t begin = min_sz(r.begin, full), end = min_sz(r.end, full);", "const size_t begin = min_sz(r.begin, full), end = min_sz(r.end, n2);"),
         ("for (unsigned pass = 0; pass <= r.max_pass && !ended; ++pass)", "for (unsigned pass = 0; pass < r.max_pass && !ended; ++pass)"),
         ("                        if (r.type != 2 && do_not_decode[chans[c]]) continue;\n                        uint32_t code;", "                        uint32_t code;"),
         ("const size_t base = first + size_t(c) * parts;", "const size_t base = first;"),
-        ("fe.part_classes.size() - base);", "parts - first);"),
-        ("if (!(r.used[cls] & (1u << pass))) continue;", "if (!(r.used[cls] & (1u << pass)) && pass) continue;"),
-        ("out[i] = fe.type2[i * size_t(n_chans) + size_t(c)];", "out[i] = fe.type2[i + size_t(c) * n2];"),
+        ("cls.size - base);", "parts - first);"),
+        ("if (!(r.used[k] & (1u << pass))) continue;", "if (!(r.used[k] & (1u << pass)) && pass) continue;"),
+        ("rows[j & 1][j >> 1]", "rows[(j >> 1) & 1][j >> 1]"),
         ("if (fe) fe->prev_block_flag = -1;", ""),
         ("if (!bs.read_bool(flag) || flag) return SYMGPU_ERR_DECODE;  // lib.rs:151-154", "if (!bs.read_bool(flag)) return SYMGPU_ERR_DECODE;"),
         ("|| mode_number >= n_modes) return SYMGPU_ERR_DECODE;", ") return SYMGPU_ERR_DECODE;"),
         ("if (!bs.read_bool(flag) || !bs.read_bool(flag)) return SYMGPU_ERR_DECODE;", "if (!bs.read_bool(flag)) return SYMGPU_ERR_DECODE;"),
-        ("if (unit->do_not_decode[cp.first] != unit->do_not_decode[cp.second]) unit->do_not_decode[cp.first] = unit->do_not_decode[cp.second] = 0;", ""),
-        ("if (!used) std::memset(floor_y + ch * 65, 0, sizeof(uint16_t) * 65);", ""),
+        ("if (mapping.coupled && unit->do_not_decode[0] != unit->do_not_decode[1]) unit->do_not_decode[0] = unit->do_not_decode[1] = 0;", ""),
+        ("        if (!used)\n            for (int i = 0; i < 65; ++i) floor_y[ch * 65 + i] = 0;\n", ""),
     ]),
 }
 
@@ -154,19 +155,29 @@ sys.exit(pytest.main(["-x", "-q", "-p", "no:cacheprovider", "-m", "not gpu"] + {
 def main():
     t = TARGETS[sys.argv[1]]
     src = open(os.path.join(CSRC, t["src"])).read()
+    # rules shared with a device decoder live in a header the source includes: a mutant found there is applied to a copy of
+    # the header, and the source's copy includes that copy instead
+    header = open(os.path.join(CSRC, t["header"])).read() if "header" in t else ""
     survivors = []
     with tempfile.TemporaryDirectory() as tmp:
         for k, (old, new) in enumerate(t["mutants"]):
-            assert src.count(old) >= 1, old
+            in_src = src.count(old) >= 1
+            assert in_src or header.count(old) >= 1, old
             path = os.path.join(CSRC, f"_mutant_{k}.cpp")  # next to the original: relative includes
+            hpath = os.path.join(CSRC, f"_mutant_{k}.h")
             so = os.path.join(tmp, f"m{k}.so")
             with open(path, "w") as f:
-                f.write(src.replace(old, new, 1))
+                f.write(src.replace(old, new, 1) if in_src else src.replace(f'#include "{t["header"]}"', f'#include "_mutant_{k}.h"'))
+            if not in_src:
+                with open(hpath, "w") as f:
+                    f.write(header.replace(old, new, 1))
             try:
                 cc = subprocess.run(["g++", "-std=c++17", "-O1", "-ffp-contract=off", "-fPIC", "-shared", "-I/usr/local/cuda/include", "-o", so, path] +
                                     ([os.path.join(CSRC, "packetizer.cpp")] if sys.argv[1] == "vorbis" else []), capture_output=True, text=True)
             finally:
                 os.remove(path)
+                if os.path.exists(hpath):
+                    os.remove(hpath)
             if cc.returncode:
                 print(f"[{k}] does not compile: {old!r}")
                 continue
