@@ -28,7 +28,7 @@
 #include <vector>
 
 #include "aac_entropy.h"
-#include "ctx.h"
+#include "batch_call.h"
 #include "pack_kernel.h"
 
 using namespace symgpu_detail;
@@ -196,8 +196,6 @@ __global__ void __launch_bounds__(256) aac_place_kernel(const DevGroup* __restri
     }
 }
 
-size_t align256(size_t v) { return (v + 255) & ~size_t(255); }
-
 struct Layout {
     std::vector<DevGroup> dev;
     std::vector<symgpu_aac_run> runs;
@@ -208,25 +206,18 @@ symgpu_status check_groups(const symgpu_ctx* ctx, size_t n_jobs, const symgpu_aa
     const size_t sample = symgpu_sample_bytes(format);
     if (sample == 0) return SYMGPU_ERR_ARG;
     const uint64_t out_samples = out_bytes / sample;
-    std::vector<uint32_t> order, slots;
+    std::vector<JobRange> ranges;
+    std::vector<uint32_t> slots;
     for (size_t g = 0; g < n_groups; ++g) {
         const symgpu_aac_group& G = groups[g];
-        if ((G.channels != 1 && G.channels != 2) || G.sample_rate == 0) return SYMGPU_ERR_ARG;
-        if (uint64_t(G.first_job) + G.n_jobs > n_jobs || G.out_offset % G.channels) return SYMGPU_ERR_ARG;
-        if (G.n_jobs) order.push_back(uint32_t(g));
+        if ((G.channels != 1 && G.channels != 2) || G.sample_rate == 0 || G.out_offset % G.channels) return SYMGPU_ERR_ARG;
+        ranges.push_back({G.first_job, G.n_jobs});
         slots.push_back(G.slot);
     }
-    std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return groups[a].first_job < groups[b].first_job; });
-    for (size_t i = 1; i < order.size(); ++i)
-        if (uint64_t(groups[order[i - 1]].first_job) + groups[order[i - 1]].n_jobs > groups[order[i]].first_job) return SYMGPU_ERR_ARG;
-    std::sort(slots.begin(), slots.end());
-    if (std::adjacent_find(slots.begin(), slots.end()) != slots.end()) return SYMGPU_ERR_ARG;
-    for (size_t g = 0; g < n_groups; ++g) {
-        const symgpu_aac_group& G = groups[g];
-        if (G.slot >= ctx->n_aac_streams) return SYMGPU_ERR_LIMIT;
-        const uint64_t region = uint64_t(G.n_jobs) * 1024u * G.channels;
-        if (G.out_offset > out_samples || region > out_samples - G.out_offset) return SYMGPU_ERR_LIMIT;
-    }
+    symgpu_status e = check_job_ranges(ranges, n_jobs);
+    if (e == SYMGPU_OK) e = check_slots(slots, ctx->n_aac_streams);
+    for (size_t g = 0; g < n_groups && e == SYMGPU_OK; ++g) e = check_region(groups[g].out_offset, uint64_t(groups[g].n_jobs) * 1024u * groups[g].channels, out_samples);
+    if (e != SYMGPU_OK) return e;
     L.dev.resize(n_groups);
     for (size_t g = 0; g < n_groups; ++g) {
         const symgpu_aac_group& G = groups[g];
@@ -244,32 +235,27 @@ struct Scratch {
 
 Scratch scratch_layout(uint32_t n_jobs, size_t n_groups, const Layout& L) {
     Scratch s;
-    size_t at = 0;
-    auto take = [&](size_t bytes) {
-        const size_t here = at;
-        at += align256(bytes);
-        return here;
-    };
+    Carver c;
     const size_t J = n_jobs, F = L.n_frames;
-    s.groups = take(n_groups * sizeof(DevGroup));
-    s.keys = take(J * sizeof(uint32_t));
-    s.state = take(J * sizeof(ae::JobState));
-    s.units = take(J * 2 * sizeof(symgpu_aac_unit));
-    s.tns = take(J * 16 * sizeof(symgpu_aac_tns));
-    s.coeffs = take(J * 2048 * sizeof(float));
-    s.pulse = take(J * 2 * sizeof(ae::PulseLines));
-    s.scales0 = take(J * 128 * sizeof(float));
-    s.walk = take(J * sizeof(ae::WalkOut));
-    s.slot_job = take(F * sizeof(uint32_t));
-    s.spans1 = take(J * sizeof(symgpu_pcm_span));
-    s.spans2 = take(J * sizeof(symgpu_pcm_span));
-    s.counts = take(2 * sizeof(uint32_t));
-    s.fixes = take(J * 2 * sizeof(PulseFix));
-    s.p_units = take(F * 2 * sizeof(symgpu_aac_unit));
-    s.p_tns = take(F * 16 * sizeof(symgpu_aac_tns));
-    s.p_coeffs = take(F * 2048 * sizeof(float));
-    s.pcm = take(F * 2048 * sizeof(float));
-    s.total = at;
+    s.groups = c.take(n_groups * sizeof(DevGroup));
+    s.keys = c.take(J * sizeof(uint32_t));
+    s.state = c.take(J * sizeof(ae::JobState));
+    s.units = c.take(J * 2 * sizeof(symgpu_aac_unit));
+    s.tns = c.take(J * 16 * sizeof(symgpu_aac_tns));
+    s.coeffs = c.take(J * 2048 * sizeof(float));
+    s.pulse = c.take(J * 2 * sizeof(ae::PulseLines));
+    s.scales0 = c.take(J * 128 * sizeof(float));
+    s.walk = c.take(J * sizeof(ae::WalkOut));
+    s.slot_job = c.take(F * sizeof(uint32_t));
+    s.spans1 = c.take(J * sizeof(symgpu_pcm_span));
+    s.spans2 = c.take(J * sizeof(symgpu_pcm_span));
+    s.counts = c.take(2 * sizeof(uint32_t));
+    s.fixes = c.take(J * 2 * sizeof(PulseFix));
+    s.p_units = c.take(F * 2 * sizeof(symgpu_aac_unit));
+    s.p_tns = c.take(F * 16 * sizeof(symgpu_aac_tns));
+    s.p_coeffs = c.take(F * 2048 * sizeof(float));
+    s.pcm = c.take(F * 2048 * sizeof(float));
+    s.total = c.at;
     return s;
 }
 
@@ -363,18 +349,13 @@ symgpu_aac_group_result empty_result(const symgpu_aac_group& G) {
     return r;
 }
 
-bool bad_args(const symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_piece* jobs, size_t n_jobs, const symgpu_aac_group* groups,
-              size_t n_groups, const void* out, size_t out_bytes, const symgpu_aac_group_result* results, const uint8_t* status) {
-    return !ctx || (n_bytes && !bytes) || (n_jobs && (!jobs || !status)) || (n_groups && (!groups || !results)) || (out_bytes && !out) || n_jobs > kMaxJobs ||
-           n_groups > 0x7fffffff;
-}
-
 }  // namespace
 
 extern "C" symgpu_status symgpu_aac_decode_dev(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_piece* jobs, size_t n_jobs,
                                                const symgpu_aac_group* groups, size_t n_groups, int format, void* out, size_t out_bytes,
                                                symgpu_aac_group_result* results, uint8_t* status, uint32_t* n_redecoded) {
-    if (bad_args(ctx, bytes, n_bytes, jobs, n_jobs, groups, n_groups, out, out_bytes, results, status)) return SYMGPU_ERR_ARG;
+    if (bad_batch_args(ctx, bytes, n_bytes, jobs, n_jobs, groups, n_groups, out, out_bytes, results, status, kMaxJobs) || n_groups > 0x7fffffff)
+        return SYMGPU_ERR_ARG;
     Layout L;
     symgpu_status e = check_groups(ctx, n_jobs, groups, n_groups, format, out_bytes, L);
     if (e != SYMGPU_OK) return e;
@@ -399,10 +380,9 @@ extern "C" symgpu_status symgpu_aac_decode_dev(symgpu_ctx* ctx, const uint8_t* b
 extern "C" symgpu_status symgpu_aac_decode_host(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_piece* jobs, size_t n_jobs,
                                                 const symgpu_aac_group* groups, size_t n_groups, int format, void* out, size_t out_bytes,
                                                 symgpu_aac_group_result* results, uint8_t* status, uint32_t* n_redecoded) {
-    if (bad_args(ctx, bytes, n_bytes, jobs, n_jobs, groups, n_groups, out, out_bytes, results, status)) return SYMGPU_ERR_ARG;
-    // Everything is checked before anything is launched.
-    for (size_t k = 0; k < n_jobs; ++k)
-        if (jobs[k].offset > n_bytes || jobs[k].len > n_bytes - jobs[k].offset) return SYMGPU_ERR_ARG;
+    if (bad_batch_args(ctx, bytes, n_bytes, jobs, n_jobs, groups, n_groups, out, out_bytes, results, status, kMaxJobs) || n_groups > 0x7fffffff ||
+        !jobs_in_bytes(jobs, n_jobs, n_bytes))
+        return SYMGPU_ERR_ARG;
     Layout L;
     symgpu_status e = check_groups(ctx, n_jobs, groups, n_groups, format, out_bytes, L);
     if (e != SYMGPU_OK) return e;
@@ -412,35 +392,12 @@ extern "C" symgpu_status symgpu_aac_decode_host(symgpu_ctx* ctx, const uint8_t* 
     if (n_jobs == 0 || n_groups == 0) return SYMGPU_OK;
     DeviceGuard guard(ctx->device);
     const Scratch s = scratch_layout(uint32_t(n_jobs), n_groups, L);
-    const size_t o_bytes = s.total, o_jobs = o_bytes + align256(n_bytes), o_out = o_jobs + align256(n_jobs * sizeof(symgpu_piece));
-    const size_t o_results = o_out + align256(out_bytes), o_status = o_results + align256(n_groups * sizeof(symgpu_aac_group_result));
-    const size_t end = o_status + align256(n_jobs);
-    e = ensure_stage(ctx, end);
-    if (e != SYMGPU_OK) return e;
-    char* stage = static_cast<char*>(ctx->d_stage);
-    uint8_t* d_bytes = reinterpret_cast<uint8_t*>(stage + o_bytes);
-    symgpu_piece* d_jobs = reinterpret_cast<symgpu_piece*>(stage + o_jobs);
-    char* d_out = stage + o_out;
-    symgpu_aac_group_result* d_results = reinterpret_cast<symgpu_aac_group_result*>(stage + o_results);
-    uint8_t* d_status = reinterpret_cast<uint8_t*>(stage + o_status);
-    if (n_bytes) CU(ctx, cudaMemcpyAsync(d_bytes, bytes, n_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    CU(ctx, cudaMemcpyAsync(d_jobs, jobs, n_jobs * sizeof(symgpu_piece), cudaMemcpyHostToDevice, ctx->stream));
-    e = decode_on_device(ctx, s, L, d_bytes, n_bytes, d_jobs, uint32_t(n_jobs), format, d_out, d_results, d_status, n_redecoded);
-    if (e != SYMGPU_OK) return e;
-    CU(ctx, cudaMemcpyAsync(status, d_status, n_jobs, cudaMemcpyDeviceToHost, ctx->stream));
-    CU(ctx, cudaMemcpyAsync(results, d_results, n_groups * sizeof(symgpu_aac_group_result), cudaMemcpyDeviceToHost, ctx->stream));
-    CU(ctx, cudaStreamSynchronize(ctx->stream));
-    // only the written frames come back, in as few copies as the regions allow
-    const size_t sample = symgpu_sample_bytes(format);
-    std::vector<std::pair<size_t, size_t>> spans;
-    for (size_t g = 0; g < n_groups; ++g)
-        if (results[g].frames) spans.emplace_back(size_t(groups[g].out_offset) * sample, size_t(groups[g].out_offset + results[g].frames * results[g].channels) * sample);
-    std::sort(spans.begin(), spans.end());
-    for (size_t i = 0; i < spans.size();) {
-        size_t a = spans[i].first, b = spans[i].second;
-        for (++i; i < spans.size() && spans[i].first <= b; ++i) b = std::max(b, spans[i].second);
-        CU(ctx, cudaMemcpyAsync(static_cast<char*>(out) + a, d_out + a, b - a, cudaMemcpyDeviceToHost, ctx->stream));
-    }
-    CU(ctx, cudaStreamSynchronize(ctx->stream));
-    return SYMGPU_OK;
+    return decode_from_host(
+        ctx, s.total, std::array<HostIn, 2>{{{bytes, n_bytes}, {jobs, n_jobs * sizeof(symgpu_piece)}}}, out, out_bytes,
+        std::array<HostOut, 2>{{{status, n_jobs}, {results, n_groups * sizeof(symgpu_aac_group_result)}}},
+        [&](const std::array<void*, 2>& in, void* d_out, const std::array<void*, 2>& back) {
+            return decode_on_device(ctx, s, L, static_cast<const uint8_t*>(in[0]), n_bytes, static_cast<const symgpu_piece*>(in[1]), uint32_t(n_jobs), format,
+                                    d_out, static_cast<symgpu_aac_group_result*>(back[1]), static_cast<uint8_t*>(back[0]), n_redecoded);
+        },
+        [&] { return written_by_results(groups, results, n_groups, symgpu_sample_bytes(format)); });
 }

@@ -18,7 +18,7 @@
 #include <cub/device/device_scan.cuh>
 #include <vector>
 
-#include "ctx.h"
+#include "batch_call.h"
 #include "flac_entropy.h"
 #include "flac_kernel.h"
 
@@ -111,8 +111,6 @@ __global__ void __launch_bounds__(256) flac_interleave_kernel(const symgpu_flac_
     }
 }
 
-size_t align256(size_t v) { return (v + 255) & ~size_t(255); }
-
 // The two device-wide scans; the size query (temp == nullptr) and the run go through the same instantiation.
 cudaError_t scan_slots(void* temp, size_t& temp_bytes, const Slot* sizes, Slot* base, uint32_t n_jobs, cudaStream_t st) {
     return cub::DeviceScan::ExclusiveScan(temp, temp_bytes, sizes, base, SlotSum(), Slot{0, 0}, int(n_jobs), st);
@@ -135,22 +133,17 @@ cudaError_t scratch_layout(uint32_t n_jobs, size_t out_cap, Scratch& s) {
     e = scan_first(nullptr, t_first, nullptr, nullptr, nullptr, n_jobs, nullptr);
     if (e != cudaSuccess) return e;
     s.temp_bytes = t_slots > t_first ? t_slots : t_first;
-    size_t at = 0;
-    auto take = [&](size_t bytes) {
-        const size_t here = at;
-        at += align256(bytes);
-        return here;
-    };
-    s.sizes = take(n_jobs * sizeof(Slot));
-    s.base = take(n_jobs * sizeof(Slot));
-    s.keys = take(n_jobs * sizeof(uint32_t));
-    s.accepted = take(n_jobs * sizeof(unsigned long long));
-    s.first = take(n_jobs * sizeof(unsigned long long));
-    s.frames = take(n_jobs * sizeof(symgpu_flac_frame));
-    s.subs = take(size_t(n_jobs) * 8 * sizeof(symgpu_flac_subframe));
-    s.samples = take(out_cap * sizeof(int32_t));
-    s.temp = take(s.temp_bytes);
-    s.total = at;
+    Carver c;
+    s.sizes = c.take(n_jobs * sizeof(Slot));
+    s.base = c.take(n_jobs * sizeof(Slot));
+    s.keys = c.take(n_jobs * sizeof(uint32_t));
+    s.accepted = c.take(n_jobs * sizeof(unsigned long long));
+    s.first = c.take(n_jobs * sizeof(unsigned long long));
+    s.frames = c.take(n_jobs * sizeof(symgpu_flac_frame));
+    s.subs = c.take(size_t(n_jobs) * 8 * sizeof(symgpu_flac_subframe));
+    s.samples = c.take(out_cap * sizeof(int32_t));
+    s.temp = c.take(s.temp_bytes);
+    s.total = c.at;
     return cudaSuccess;
 }
 
@@ -192,8 +185,7 @@ constexpr size_t kMaxJobs = 0x1fffffff;  // eight sub-frame records per job are 
 extern "C" symgpu_status symgpu_flac_decode_dev(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_flac_job* jobs, size_t n_jobs,
                                                 const symgpu_flac_group* groups, size_t n_groups, int32_t* out, size_t out_cap, uint64_t* group_frames,
                                                 uint8_t* status) {
-    if (!ctx || (n_bytes && !bytes) || (n_jobs && (!jobs || !status)) || (n_groups && (!groups || !group_frames)) || (out_cap && !out) || n_jobs > kMaxJobs)
-        return SYMGPU_ERR_ARG;
+    if (bad_batch_args(ctx, bytes, n_bytes, jobs, n_jobs, groups, n_groups, out, out_cap, group_frames, status, kMaxJobs)) return SYMGPU_ERR_ARG;
     DeviceGuard guard(ctx->device);
     if (n_groups) CU(ctx, cudaMemsetAsync(group_frames, 0, n_groups * sizeof(uint64_t), ctx->stream));
     if (n_jobs == 0) return SYMGPU_OK;
@@ -207,9 +199,9 @@ extern "C" symgpu_status symgpu_flac_decode_dev(symgpu_ctx* ctx, const uint8_t* 
 extern "C" symgpu_status symgpu_flac_decode_host(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_flac_job* jobs, size_t n_jobs,
                                                  const symgpu_flac_group* groups, size_t n_groups, int32_t* out, size_t out_cap, uint64_t* group_frames,
                                                  uint8_t* status) {
-    if (!ctx || (n_bytes && !bytes) || (n_jobs && (!jobs || !status)) || (n_groups && (!groups || !group_frames)) || (out_cap && !out) || n_jobs > kMaxJobs)
+    if (bad_batch_args(ctx, bytes, n_bytes, jobs, n_jobs, groups, n_groups, out, out_cap, group_frames, status, kMaxJobs) ||
+        !jobs_in_bytes(jobs, n_jobs, n_bytes))
         return SYMGPU_ERR_ARG;
-    // Everything is checked before anything is launched.
     for (size_t g = 0; g < n_groups; ++g)
         if (groups[g].channels < 1 || groups[g].channels > 8 || groups[g].bits_per_sample > 32 || groups[g].out_offset > out_cap) return SYMGPU_ERR_ARG;
     std::vector<uint64_t> need(n_groups, 0);
@@ -217,7 +209,7 @@ extern "C" symgpu_status symgpu_flac_decode_host(symgpu_ctx* ctx, const uint8_t*
     uint64_t total = 0;
     for (size_t k = 0; k < n_jobs; ++k) {
         const symgpu_flac_job& j = jobs[k];
-        if (j.offset > n_bytes || j.len > n_bytes - j.offset || j.group >= n_groups) return SYMGPU_ERR_ARG;
+        if (j.group >= n_groups) return SYMGPU_ERR_ARG;
         if (k == 0 || jobs[k - 1].group != j.group) {
             if (seen[j.group]) return SYMGPU_ERR_ARG;  // the group's jobs are not consecutive
             seen[j.group] = 1;
@@ -226,48 +218,28 @@ extern "C" symgpu_status symgpu_flac_decode_host(symgpu_ctx* ctx, const uint8_t*
         need[j.group] += size, total += size;
     }
     for (size_t g = 0; g < n_groups; ++g)
-        if (need[g] > out_cap - groups[g].out_offset) return SYMGPU_ERR_LIMIT;
+        if (check_region(groups[g].out_offset, need[g], out_cap) != SYMGPU_OK) return SYMGPU_ERR_LIMIT;
     if (total > out_cap) return SYMGPU_ERR_LIMIT;
     for (size_t g = 0; g < n_groups; ++g) group_frames[g] = 0;
     if (n_jobs == 0) return SYMGPU_OK;
     DeviceGuard guard(ctx->device);
     Scratch s;
     CU(ctx, scratch_layout(uint32_t(n_jobs), out_cap, s));
-    const size_t o_bytes = s.total, o_jobs = o_bytes + align256(n_bytes), o_groups = o_jobs + align256(n_jobs * sizeof(symgpu_flac_job));
-    const size_t o_out = o_groups + align256(n_groups * sizeof(symgpu_flac_group)), o_frames = o_out + align256(out_cap * sizeof(int32_t));
-    const size_t o_status = o_frames + align256(n_groups * sizeof(uint64_t)), end = o_status + align256(n_jobs);
-    symgpu_status e = ensure_stage(ctx, end);
-    if (e != SYMGPU_OK) return e;
-    char* stage = static_cast<char*>(ctx->d_stage);
-    uint8_t* d_bytes = reinterpret_cast<uint8_t*>(stage + o_bytes);
-    symgpu_flac_job* d_jobs = reinterpret_cast<symgpu_flac_job*>(stage + o_jobs);
-    symgpu_flac_group* d_groups = reinterpret_cast<symgpu_flac_group*>(stage + o_groups);
-    int32_t* d_out = reinterpret_cast<int32_t*>(stage + o_out);
-    uint64_t* d_frames = reinterpret_cast<uint64_t*>(stage + o_frames);
-    uint8_t* d_status = reinterpret_cast<uint8_t*>(stage + o_status);
-    if (n_bytes) CU(ctx, cudaMemcpyAsync(d_bytes, bytes, n_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    CU(ctx, cudaMemcpyAsync(d_jobs, jobs, n_jobs * sizeof(symgpu_flac_job), cudaMemcpyHostToDevice, ctx->stream));
-    if (n_groups) {
-        CU(ctx, cudaMemcpyAsync(d_groups, groups, n_groups * sizeof(symgpu_flac_group), cudaMemcpyHostToDevice, ctx->stream));
-        CU(ctx, cudaMemsetAsync(d_frames, 0, n_groups * sizeof(uint64_t), ctx->stream));
-    }
-    e = decode_on_device(ctx, s, d_bytes, n_bytes, d_jobs, uint32_t(n_jobs), d_groups, n_groups, d_out, out_cap, d_frames, d_status);
-    if (e != SYMGPU_OK) return e;
-    CU(ctx, cudaMemcpyAsync(status, d_status, n_jobs, cudaMemcpyDeviceToHost, ctx->stream));
-    if (n_groups) CU(ctx, cudaMemcpyAsync(group_frames, d_frames, n_groups * sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
-    CU(ctx, cudaStreamSynchronize(ctx->stream));
-    // only the written frames come back, in as few copies as the regions allow
-    size_t run_a = 0, run_b = 0;
-    for (size_t g = 0; g <= n_groups; ++g) {
-        size_t a = 0, b = 0;
-        if (g < n_groups) a = groups[g].out_offset, b = a + size_t(group_frames[g]) * groups[g].channels;
-        if (g < n_groups && a == run_b && b > a) {
-            run_b = b;
-            continue;
-        }
-        if (run_b > run_a) CU(ctx, cudaMemcpyAsync(out + run_a, d_out + run_a, (run_b - run_a) * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
-        run_a = a, run_b = b;
-    }
-    CU(ctx, cudaStreamSynchronize(ctx->stream));
-    return SYMGPU_OK;
+    return decode_from_host(
+        ctx, s.total,
+        std::array<HostIn, 3>{{{bytes, n_bytes}, {jobs, n_jobs * sizeof(symgpu_flac_job)}, {groups, n_groups * sizeof(symgpu_flac_group)}}}, out,
+        out_cap * sizeof(int32_t), std::array<HostOut, 2>{{{status, n_jobs}, {group_frames, n_groups * sizeof(uint64_t)}}},
+        [&](const std::array<void*, 3>& in, void* d_out, const std::array<void*, 2>& back) {
+            uint64_t* d_frames = static_cast<uint64_t*>(back[1]);
+            if (n_groups) CU(ctx, cudaMemsetAsync(d_frames, 0, n_groups * sizeof(uint64_t), ctx->stream));
+            return decode_on_device(ctx, s, static_cast<const uint8_t*>(in[0]), n_bytes, static_cast<const symgpu_flac_job*>(in[1]), uint32_t(n_jobs),
+                                    static_cast<const symgpu_flac_group*>(in[2]), n_groups, static_cast<int32_t*>(d_out), out_cap, d_frames,
+                                    static_cast<uint8_t*>(back[0]));
+        },
+        [&] {
+            std::vector<ByteRange> w;
+            for (size_t g = 0; g < n_groups; ++g)
+                w.push_back({size_t(groups[g].out_offset) * sizeof(int32_t), size_t(groups[g].out_offset + group_frames[g] * groups[g].channels) * sizeof(int32_t)});
+            return w;
+        });
 }

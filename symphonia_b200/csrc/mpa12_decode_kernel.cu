@@ -22,7 +22,7 @@
 #include <numeric>
 #include <vector>
 
-#include "ctx.h"
+#include "batch_call.h"
 #include "mp3_kernel.h"
 #include "mpa12_entropy.h"
 
@@ -206,8 +206,6 @@ __global__ void __launch_bounds__(32 * kWarpsPerCta) mpa12_sample_kernel(const u
     }
 }
 
-size_t align256(size_t v) { return (v + 255) & ~size_t(255); }
-
 cudaError_t scan_place(void* temp, size_t& temp_bytes, const uint32_t* keys, const Place* in, Place* out, uint32_t n_jobs, cudaStream_t st) {
     return cub::DeviceScan::ExclusiveScanByKey(temp, temp_bytes, keys, in, out, PlaceSum(), Place{0, 0}, int(n_jobs), cuda::std::equal_to<>(), st);
 }
@@ -224,26 +222,19 @@ symgpu_status check_groups(const symgpu_ctx* ctx, size_t n_jobs, const symgpu_mp
     const size_t sample = symgpu_sample_bytes(format);
     if (sample == 0) return SYMGPU_ERR_ARG;
     const uint64_t out_samples = out_bytes / sample;
-    std::vector<uint32_t> order;
+    std::vector<JobRange> ranges;
     std::vector<uint32_t> slots;
     for (size_t g = 0; g < n_groups; ++g) {
         const symgpu_mpa12_group& G = groups[g];
-        if (G.layer != 1 && G.layer != 2) return SYMGPU_ERR_ARG;
-        if (uint64_t(G.first_job) + G.n_jobs > n_jobs || (G.out_offset & 1)) return SYMGPU_ERR_ARG;
-        if (G.n_jobs) order.push_back(uint32_t(g));
+        if ((G.layer != 1 && G.layer != 2) || (G.out_offset & 1)) return SYMGPU_ERR_ARG;
+        ranges.push_back({G.first_job, G.n_jobs});
         slots.push_back(G.slot);
     }
-    std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return groups[a].first_job < groups[b].first_job; });
-    for (size_t i = 1; i < order.size(); ++i)
-        if (uint64_t(groups[order[i - 1]].first_job) + groups[order[i - 1]].n_jobs > groups[order[i]].first_job) return SYMGPU_ERR_ARG;
-    std::sort(slots.begin(), slots.end());
-    if (std::adjacent_find(slots.begin(), slots.end()) != slots.end()) return SYMGPU_ERR_ARG;
-    for (size_t g = 0; g < n_groups; ++g) {
-        const symgpu_mpa12_group& G = groups[g];
-        if (G.slot >= ctx->n_mp3_streams) return SYMGPU_ERR_LIMIT;
-        const uint64_t region = 2ull * G.n_jobs * (G.layer == 1 ? 384u : 1152u);
-        if (G.out_offset > out_samples || region > out_samples - G.out_offset) return SYMGPU_ERR_LIMIT;
-    }
+    symgpu_status e = check_job_ranges(ranges, n_jobs);
+    if (e == SYMGPU_OK) e = check_slots(slots, ctx->n_mp3_streams);
+    for (size_t g = 0; g < n_groups && e == SYMGPU_OK; ++g)
+        e = check_region(groups[g].out_offset, 2ull * groups[g].n_jobs * (groups[g].layer == 1 ? 384u : 1152u), out_samples);
+    if (e != SYMGPU_OK) return e;
     for (size_t g = 0; g < n_groups; ++g) L.n_frames[groups[g].layer - 1] += groups[g].n_jobs;
     uint64_t base[2] = {0, L.n_frames[0]};
     L.dev.resize(n_groups);
@@ -266,25 +257,20 @@ struct Scratch {
 cudaError_t scratch_layout(uint32_t n_jobs, size_t n_groups, const Layout& L, Scratch& s) {
     cudaError_t e = scan_place(nullptr, s.temp_bytes, nullptr, nullptr, nullptr, n_jobs, nullptr);
     if (e != cudaSuccess) return e;
-    size_t at = 0;
-    auto take = [&](size_t bytes) {
-        const size_t here = at;
-        at += align256(bytes);
-        return here;
-    };
-    s.groups = take(n_groups * sizeof(DevGroup));
-    s.heads = take(n_jobs * sizeof(Head));
-    s.keys = take(n_jobs * sizeof(uint32_t));
-    s.spec = take(n_groups * sizeof(Spec));
-    s.sides = take(n_jobs * sizeof(me::Side));
-    s.place_in = take(n_jobs * sizeof(Place));
-    s.place = take(n_jobs * sizeof(Place));
-    s.sub = take((L.n_frames[0] * 64 * 12 + L.n_frames[1] * 64 * 36) * sizeof(float));
-    s.pcm = take(size_t(L.n_frames[0] + L.n_frames[1]) * SYMGPU_MP3_FRAME_FLOATS * sizeof(float));
-    s.spans1 = take(n_jobs * sizeof(symgpu_pcm_span));
-    s.spans2 = take(n_jobs * sizeof(symgpu_pcm_span));
-    s.temp = take(s.temp_bytes);
-    s.total = at;
+    Carver c;
+    s.groups = c.take(n_groups * sizeof(DevGroup));
+    s.heads = c.take(n_jobs * sizeof(Head));
+    s.keys = c.take(n_jobs * sizeof(uint32_t));
+    s.spec = c.take(n_groups * sizeof(Spec));
+    s.sides = c.take(n_jobs * sizeof(me::Side));
+    s.place_in = c.take(n_jobs * sizeof(Place));
+    s.place = c.take(n_jobs * sizeof(Place));
+    s.sub = c.take((L.n_frames[0] * 64 * 12 + L.n_frames[1] * 64 * 36) * sizeof(float));
+    s.pcm = c.take(size_t(L.n_frames[0] + L.n_frames[1]) * SYMGPU_MP3_FRAME_FLOATS * sizeof(float));
+    s.spans1 = c.take(n_jobs * sizeof(symgpu_pcm_span));
+    s.spans2 = c.take(n_jobs * sizeof(symgpu_pcm_span));
+    s.temp = c.take(s.temp_bytes);
+    s.total = c.at;
     return cudaSuccess;
 }
 
@@ -341,8 +327,7 @@ constexpr size_t kMaxJobs = 0x7fffffff;  // the device-wide scan counts items in
 extern "C" symgpu_status symgpu_mpa12_decode_dev(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_mpa12_job* jobs, size_t n_jobs,
                                                  const symgpu_mpa12_group* groups, size_t n_groups, int format, void* out, size_t out_bytes,
                                                  symgpu_mpa12_group_result* results, uint8_t* status) {
-    if (!ctx || (n_bytes && !bytes) || (n_jobs && (!jobs || !status)) || (n_groups && (!groups || !results)) || (out_bytes && !out) || n_jobs > kMaxJobs ||
-        n_groups > 0x7fffffff)
+    if (bad_batch_args(ctx, bytes, n_bytes, jobs, n_jobs, groups, n_groups, out, out_bytes, results, status, kMaxJobs) || n_groups > 0x7fffffff)
         return SYMGPU_ERR_ARG;
     Layout L;
     symgpu_status e = check_groups(ctx, n_jobs, groups, n_groups, format, out_bytes, L);
@@ -363,12 +348,9 @@ extern "C" symgpu_status symgpu_mpa12_decode_dev(symgpu_ctx* ctx, const uint8_t*
 extern "C" symgpu_status symgpu_mpa12_decode_host(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_mpa12_job* jobs, size_t n_jobs,
                                                   const symgpu_mpa12_group* groups, size_t n_groups, int format, void* out, size_t out_bytes,
                                                   symgpu_mpa12_group_result* results, uint8_t* status) {
-    if (!ctx || (n_bytes && !bytes) || (n_jobs && (!jobs || !status)) || (n_groups && (!groups || !results)) || (out_bytes && !out) || n_jobs > kMaxJobs ||
-        n_groups > 0x7fffffff)
+    if (bad_batch_args(ctx, bytes, n_bytes, jobs, n_jobs, groups, n_groups, out, out_bytes, results, status, kMaxJobs) || n_groups > 0x7fffffff ||
+        !jobs_in_bytes(jobs, n_jobs, n_bytes))
         return SYMGPU_ERR_ARG;
-    // Everything is checked before anything is launched.
-    for (size_t k = 0; k < n_jobs; ++k)
-        if (jobs[k].offset > n_bytes || jobs[k].len > n_bytes - jobs[k].offset) return SYMGPU_ERR_ARG;
     Layout L;
     symgpu_status e = check_groups(ctx, n_jobs, groups, n_groups, format, out_bytes, L);
     if (e != SYMGPU_OK) return e;
@@ -378,35 +360,12 @@ extern "C" symgpu_status symgpu_mpa12_decode_host(symgpu_ctx* ctx, const uint8_t
     DeviceGuard guard(ctx->device);
     Scratch s;
     CU(ctx, scratch_layout(uint32_t(n_jobs), n_groups, L, s));
-    const size_t o_bytes = s.total, o_jobs = o_bytes + align256(n_bytes), o_out = o_jobs + align256(n_jobs * sizeof(symgpu_mpa12_job));
-    const size_t o_results = o_out + align256(out_bytes), o_status = o_results + align256(n_groups * sizeof(symgpu_mpa12_group_result));
-    const size_t end = o_status + align256(n_jobs);
-    e = ensure_stage(ctx, end);
-    if (e != SYMGPU_OK) return e;
-    char* stage = static_cast<char*>(ctx->d_stage);
-    uint8_t* d_bytes = reinterpret_cast<uint8_t*>(stage + o_bytes);
-    symgpu_mpa12_job* d_jobs = reinterpret_cast<symgpu_mpa12_job*>(stage + o_jobs);
-    char* d_out = stage + o_out;
-    symgpu_mpa12_group_result* d_results = reinterpret_cast<symgpu_mpa12_group_result*>(stage + o_results);
-    uint8_t* d_status = reinterpret_cast<uint8_t*>(stage + o_status);
-    if (n_bytes) CU(ctx, cudaMemcpyAsync(d_bytes, bytes, n_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    CU(ctx, cudaMemcpyAsync(d_jobs, jobs, n_jobs * sizeof(symgpu_mpa12_job), cudaMemcpyHostToDevice, ctx->stream));
-    e = decode_on_device(ctx, s, L, d_bytes, n_bytes, d_jobs, uint32_t(n_jobs), format, d_out, d_results, d_status);
-    if (e != SYMGPU_OK) return e;
-    CU(ctx, cudaMemcpyAsync(status, d_status, n_jobs, cudaMemcpyDeviceToHost, ctx->stream));
-    CU(ctx, cudaMemcpyAsync(results, d_results, n_groups * sizeof(symgpu_mpa12_group_result), cudaMemcpyDeviceToHost, ctx->stream));
-    CU(ctx, cudaStreamSynchronize(ctx->stream));
-    // only the written frames come back, in as few copies as the regions allow
-    const size_t sample = symgpu_sample_bytes(format);
-    std::vector<std::pair<size_t, size_t>> spans;
-    for (size_t g = 0; g < n_groups; ++g)
-        if (results[g].frames) spans.emplace_back(size_t(groups[g].out_offset) * sample, size_t(groups[g].out_offset + results[g].frames * results[g].channels) * sample);
-    std::sort(spans.begin(), spans.end());
-    for (size_t i = 0; i < spans.size();) {
-        size_t a = spans[i].first, b = spans[i].second;
-        for (++i; i < spans.size() && spans[i].first <= b; ++i) b = std::max(b, spans[i].second);
-        CU(ctx, cudaMemcpyAsync(static_cast<char*>(out) + a, d_out + a, b - a, cudaMemcpyDeviceToHost, ctx->stream));
-    }
-    CU(ctx, cudaStreamSynchronize(ctx->stream));
-    return SYMGPU_OK;
+    return decode_from_host(
+        ctx, s.total, std::array<HostIn, 2>{{{bytes, n_bytes}, {jobs, n_jobs * sizeof(symgpu_mpa12_job)}}}, out, out_bytes,
+        std::array<HostOut, 2>{{{status, n_jobs}, {results, n_groups * sizeof(symgpu_mpa12_group_result)}}},
+        [&](const std::array<void*, 2>& in, void* d_out, const std::array<void*, 2>& back) {
+            return decode_on_device(ctx, s, L, static_cast<const uint8_t*>(in[0]), n_bytes, static_cast<const symgpu_mpa12_job*>(in[1]), uint32_t(n_jobs),
+                                    format, d_out, static_cast<symgpu_mpa12_group_result*>(back[1]), static_cast<uint8_t*>(back[0]));
+        },
+        [&] { return written_by_results(groups, results, n_groups, symgpu_sample_bytes(format)); });
 }

@@ -23,7 +23,7 @@
 #include <cub/device/device_scan.cuh>
 #include <vector>
 
-#include "ctx.h"
+#include "batch_call.h"
 #include "pack_kernel.h"
 #include "vorbis_entropy.h"
 
@@ -169,8 +169,6 @@ __global__ void __launch_bounds__(256) vorbis_place_kernel(const DevGroup* __res
     }
 }
 
-size_t align256(size_t v) { return (v + 255) & ~size_t(255); }
-
 cudaError_t scan_acc(void* temp, size_t& temp_bytes, const uint32_t* keys, const Acc* in, Acc* out, uint32_t n_jobs, cudaStream_t st) {
     return cub::DeviceScan::ExclusiveScanByKey(temp, temp_bytes, keys, in, out, AccOp(), Acc{0, -1}, int(n_jobs), cuda::std::equal_to<>(), st);
 }
@@ -226,22 +224,19 @@ symgpu_status check_groups(size_t n_jobs, const symgpu_vorbis_group* groups, siz
     const size_t sample = symgpu_sample_bytes(format);
     if (sample == 0) return SYMGPU_ERR_ARG;
     const uint64_t out_samples = out_bytes / sample;
-    std::vector<uint32_t> order;
+    std::vector<JobRange> ranges;
     for (size_t g = 0; g < n_groups; ++g) {
         const symgpu_vorbis_group& G = groups[g];
-        if (G.setup >= S.heads.size()) return SYMGPU_ERR_ARG;
-        if (uint64_t(G.first_job) + G.n_jobs > n_jobs || G.out_offset % S.heads[G.setup].channels) return SYMGPU_ERR_ARG;
-        if (G.n_jobs) order.push_back(uint32_t(g));
+        if (G.setup >= S.heads.size() || G.out_offset % S.heads[G.setup].channels) return SYMGPU_ERR_ARG;
+        ranges.push_back({G.first_job, G.n_jobs});
     }
-    std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return groups[a].first_job < groups[b].first_job; });
-    for (size_t i = 1; i < order.size(); ++i)
-        if (uint64_t(groups[order[i - 1]].first_job) + groups[order[i - 1]].n_jobs > groups[order[i]].first_job) return SYMGPU_ERR_ARG;
+    symgpu_status e = check_job_ranges(ranges, n_jobs);
+    if (e != SYMGPU_OK) return e;
     if (n_groups > SYMGPU_VORBIS_MAX_FILES) return SYMGPU_ERR_LIMIT;
     for (size_t g = 0; g < n_groups; ++g) {
-        const symgpu_vorbis_group& G = groups[g];
-        const ve::SetupHead& h = S.heads[G.setup];
-        const uint64_t region = uint64_t(G.n_jobs) * ((1u << h.bs1_exp) >> 1) * h.channels;
-        if (G.out_offset > out_samples || region > out_samples - G.out_offset) return SYMGPU_ERR_LIMIT;
+        const ve::SetupHead& h = S.heads[groups[g].setup];
+        e = check_region(groups[g].out_offset, uint64_t(groups[g].n_jobs) * ((1u << h.bs1_exp) >> 1) * h.channels, out_samples);
+        if (e != SYMGPU_OK) return e;
         L.row = std::max<uint32_t>(L.row, (1u << h.bs1_exp) >> 1);
     }
     L.dev.resize(n_groups);
@@ -273,34 +268,29 @@ cudaError_t scratch_layout(uint32_t n_jobs, const Setups& S, const Layout& L, Sc
     if (e == cudaSuccess) e = scan_first(nullptr, b, nullptr, nullptr, nullptr, n_jobs, nullptr);
     if (e != cudaSuccess) return e;
     s.temp_bytes = std::max(a, b);
-    size_t at = 0;
-    auto take = [&](size_t bytes) {
-        const size_t here = at;
-        at += align256(bytes);
-        return here;
-    };
+    Carver c;
     const size_t J = n_jobs, F = L.n_frames, R = L.row;
-    s.blob = take(S.blob.size());
-    s.heads = take(S.heads.size() * sizeof(ve::SetupHead));
-    s.groups = take(L.dev.size() * sizeof(DevGroup));
-    s.keys = take(J * sizeof(uint32_t));
-    s.units = take(J * sizeof(symgpu_vorbis_unit));
-    s.floor_y = take(J * 130 * sizeof(uint16_t));
-    s.residue = take(J * 2 * R * sizeof(float));
-    s.classes = take(L.class_bytes);
-    s.acc_in = take(J * sizeof(Acc));
-    s.acc = take(J * sizeof(Acc));
-    s.span = take(J * sizeof(Span));
-    s.left = take(J * sizeof(unsigned long long));
-    s.first = take(J * sizeof(unsigned long long));
-    s.p_units = take(F * sizeof(symgpu_vorbis_unit));
-    s.p_floor_y = take(F * 130 * sizeof(uint16_t));
-    s.p_residue = take(F * 2 * R * sizeof(float));
-    s.pcm = take(F * 2 * R * sizeof(float));
-    s.spans1 = take(J * sizeof(symgpu_pcm_span));
-    s.spans2 = take(J * sizeof(symgpu_pcm_span));
-    s.temp = take(s.temp_bytes);
-    s.total = at;
+    s.blob = c.take(S.blob.size());
+    s.heads = c.take(S.heads.size() * sizeof(ve::SetupHead));
+    s.groups = c.take(L.dev.size() * sizeof(DevGroup));
+    s.keys = c.take(J * sizeof(uint32_t));
+    s.units = c.take(J * sizeof(symgpu_vorbis_unit));
+    s.floor_y = c.take(J * 130 * sizeof(uint16_t));
+    s.residue = c.take(J * 2 * R * sizeof(float));
+    s.classes = c.take(L.class_bytes);
+    s.acc_in = c.take(J * sizeof(Acc));
+    s.acc = c.take(J * sizeof(Acc));
+    s.span = c.take(J * sizeof(Span));
+    s.left = c.take(J * sizeof(unsigned long long));
+    s.first = c.take(J * sizeof(unsigned long long));
+    s.p_units = c.take(F * sizeof(symgpu_vorbis_unit));
+    s.p_floor_y = c.take(F * 130 * sizeof(uint16_t));
+    s.p_residue = c.take(F * 2 * R * sizeof(float));
+    s.pcm = c.take(F * 2 * R * sizeof(float));
+    s.spans1 = c.take(J * sizeof(symgpu_pcm_span));
+    s.spans2 = c.take(J * sizeof(symgpu_pcm_span));
+    s.temp = c.take(s.temp_bytes);
+    s.total = c.at;
     return cudaSuccess;
 }
 
@@ -370,13 +360,6 @@ symgpu_status decode_on_device(symgpu_ctx* ctx, const Scratch& s, const Setups& 
 
 constexpr size_t kMaxJobs = 0x7fffffff;  // the device-wide scans count items in an int
 
-bool bad_args(const symgpu_ctx* ctx, const uint8_t* headers, size_t n_headers, const symgpu_vorbis_setup_ref* setups, size_t n_setups, const uint8_t* bytes,
-              size_t n_bytes, const symgpu_vorbis_job* jobs, size_t n_jobs, const symgpu_vorbis_group* groups, size_t n_groups, const void* out,
-              size_t out_bytes, const symgpu_vorbis_group_result* results, const uint8_t* status) {
-    return !ctx || (n_headers && !headers) || (n_setups && !setups) || (n_bytes && !bytes) || (n_jobs && (!jobs || !status)) ||
-           (n_groups && (!groups || !results)) || (out_bytes && !out) || n_jobs > kMaxJobs;
-}
-
 // Host-side preparation shared by both variants: setups, groups, registration and the staging buffer's size.
 symgpu_status prepare(symgpu_ctx* ctx, const uint8_t* headers, size_t n_headers, const symgpu_vorbis_setup_ref* setups, size_t n_setups, size_t n_jobs,
                       const symgpu_vorbis_group* groups, size_t n_groups, int format, size_t out_bytes, Setups& S, Layout& L) {
@@ -391,7 +374,8 @@ extern "C" symgpu_status symgpu_vorbis_decode_dev(symgpu_ctx* ctx, const uint8_t
                                                   size_t n_setups, const uint8_t* bytes, size_t n_bytes, const symgpu_vorbis_job* jobs, size_t n_jobs,
                                                   const symgpu_vorbis_group* groups, size_t n_groups, int format, void* out, size_t out_bytes,
                                                   symgpu_vorbis_group_result* results, uint8_t* status) {
-    if (bad_args(ctx, headers, n_headers, setups, n_setups, bytes, n_bytes, jobs, n_jobs, groups, n_groups, out, out_bytes, results, status))
+    if (bad_batch_args(ctx, bytes, n_bytes, jobs, n_jobs, groups, n_groups, out, out_bytes, results, status, kMaxJobs) || (n_headers && !headers) ||
+        (n_setups && !setups))
         return SYMGPU_ERR_ARG;
     Setups S;
     Layout L;
@@ -419,11 +403,9 @@ extern "C" symgpu_status symgpu_vorbis_decode_host(symgpu_ctx* ctx, const uint8_
                                                    size_t n_setups, const uint8_t* bytes, size_t n_bytes, const symgpu_vorbis_job* jobs, size_t n_jobs,
                                                    const symgpu_vorbis_group* groups, size_t n_groups, int format, void* out, size_t out_bytes,
                                                    symgpu_vorbis_group_result* results, uint8_t* status) {
-    if (bad_args(ctx, headers, n_headers, setups, n_setups, bytes, n_bytes, jobs, n_jobs, groups, n_groups, out, out_bytes, results, status))
+    if (bad_batch_args(ctx, bytes, n_bytes, jobs, n_jobs, groups, n_groups, out, out_bytes, results, status, kMaxJobs) || (n_headers && !headers) ||
+        (n_setups && !setups) || !jobs_in_bytes(jobs, n_jobs, n_bytes))
         return SYMGPU_ERR_ARG;
-    // Everything is checked before anything is launched.
-    for (size_t k = 0; k < n_jobs; ++k)
-        if (jobs[k].offset > n_bytes || jobs[k].len > n_bytes - jobs[k].offset) return SYMGPU_ERR_ARG;
     Setups S;
     Layout L;
     symgpu_status e = prepare(ctx, headers, n_headers, setups, n_setups, n_jobs, groups, n_groups, format, out_bytes, S, L);
@@ -436,36 +418,12 @@ extern "C" symgpu_status symgpu_vorbis_decode_host(symgpu_ctx* ctx, const uint8_
     if (e != SYMGPU_OK) return e;
     Scratch s;
     CU(ctx, scratch_layout(uint32_t(n_jobs), S, L, s));
-    const size_t o_bytes = s.total, o_jobs = o_bytes + align256(n_bytes), o_out = o_jobs + align256(n_jobs * sizeof(symgpu_vorbis_job));
-    const size_t o_results = o_out + align256(out_bytes), o_status = o_results + align256(n_groups * sizeof(symgpu_vorbis_group_result));
-    const size_t end = o_status + align256(n_jobs);
-    e = ensure_stage(ctx, end);
-    if (e != SYMGPU_OK) return e;
-    char* stage = static_cast<char*>(ctx->d_stage);
-    uint8_t* d_bytes = reinterpret_cast<uint8_t*>(stage + o_bytes);
-    symgpu_vorbis_job* d_jobs = reinterpret_cast<symgpu_vorbis_job*>(stage + o_jobs);
-    char* d_out = stage + o_out;
-    symgpu_vorbis_group_result* d_results = reinterpret_cast<symgpu_vorbis_group_result*>(stage + o_results);
-    uint8_t* d_status = reinterpret_cast<uint8_t*>(stage + o_status);
-    if (n_bytes) CU(ctx, cudaMemcpyAsync(d_bytes, bytes, n_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    CU(ctx, cudaMemcpyAsync(d_jobs, jobs, n_jobs * sizeof(symgpu_vorbis_job), cudaMemcpyHostToDevice, ctx->stream));
-    e = decode_on_device(ctx, s, S, L, d_bytes, n_bytes, d_jobs, uint32_t(n_jobs), format, d_out, d_results, d_status);
-    if (e != SYMGPU_OK) return e;
-    CU(ctx, cudaMemcpyAsync(status, d_status, n_jobs, cudaMemcpyDeviceToHost, ctx->stream));
-    CU(ctx, cudaMemcpyAsync(results, d_results, n_groups * sizeof(symgpu_vorbis_group_result), cudaMemcpyDeviceToHost, ctx->stream));
-    CU(ctx, cudaStreamSynchronize(ctx->stream));
-    // only the written frames come back, in as few copies as the regions allow
-    const size_t sample = symgpu_sample_bytes(format);
-    std::vector<std::pair<size_t, size_t>> spans;
-    for (size_t g = 0; g < n_groups; ++g)
-        if (results[g].frames)
-            spans.emplace_back(size_t(groups[g].out_offset) * sample, size_t(groups[g].out_offset + results[g].frames * results[g].channels) * sample);
-    std::sort(spans.begin(), spans.end());
-    for (size_t i = 0; i < spans.size();) {
-        size_t a = spans[i].first, b = spans[i].second;
-        for (++i; i < spans.size() && spans[i].first <= b; ++i) b = std::max(b, spans[i].second);
-        CU(ctx, cudaMemcpyAsync(static_cast<char*>(out) + a, d_out + a, b - a, cudaMemcpyDeviceToHost, ctx->stream));
-    }
-    CU(ctx, cudaStreamSynchronize(ctx->stream));
-    return SYMGPU_OK;
+    return decode_from_host(
+        ctx, s.total, std::array<HostIn, 2>{{{bytes, n_bytes}, {jobs, n_jobs * sizeof(symgpu_vorbis_job)}}}, out, out_bytes,
+        std::array<HostOut, 2>{{{status, n_jobs}, {results, n_groups * sizeof(symgpu_vorbis_group_result)}}},
+        [&](const std::array<void*, 2>& in, void* d_out, const std::array<void*, 2>& back) {
+            return decode_on_device(ctx, s, S, L, static_cast<const uint8_t*>(in[0]), n_bytes, static_cast<const symgpu_vorbis_job*>(in[1]), uint32_t(n_jobs),
+                                    format, d_out, static_cast<symgpu_vorbis_group_result*>(back[1]), static_cast<uint8_t*>(back[0]));
+        },
+        [&] { return written_by_results(groups, results, n_groups, symgpu_sample_bytes(format)); });
 }

@@ -428,45 +428,118 @@ def decode_flac(engine, data):
     return flac_interleave(plan, restored), plan["sample_rate"]
 
 
-def flac_files_plan(files, threads=None, errors=None):
-    """Host half of decode_flac_files: every file indexed (symgpu_flac_index, on `threads` host threads), their bytes concatenated
-    once, one job per packet and one group per file.  Returns dict(data, jobs, groups, rates, out_cap, failed).  A file that cannot
-    be indexed (listed in `failed`) gets a group without jobs; its message goes to errors[i] when `errors` is a dict."""
+# ---- many files per device call: the steps every codec's files path shares ---------------------------------------------------
+
+_TORCH_DTYPES = {nat.FMT_F32: "float32", nat.FMT_S16: "int16", nat.FMT_S24: "int32", nat.FMT_S32: "int32", nat.FMT_U8: "uint8"}
+
+
+def _index_files(files, index_fn, threads):
+    """index_fn(file) of every file on `threads` host threads: ([index | None], {i: message}).  A file whose index_fn raises
+    gets None and its message; the others are still indexed."""
     import concurrent.futures
     import os
     messages = {}
 
     def index(i):
         try:
-            return packetizer.flac_index(files[i])
+            return index_fn(files[i])
         except Exception as e:  # noqa: BLE001 -- one bad file must not abort the batch; its message is kept
             messages[i] = f"{type(e).__name__}: {e}"
             return None
     with concurrent.futures.ThreadPoolExecutor(max_workers=threads or os.cpu_count()) as pool:
         ix = list(pool.map(index, range(len(files))))
+    return ix, messages
+
+
+def _batch(groups, parts, job_dtype):
+    """One call's bytes, jobs and groups.  groups: one record per file, already holding what a failed file's group keeps;
+    parts: (i, bytes, jobs, fields, out samples) of every good file in order, its jobs' offsets relative to its bytes.  Each
+    good group gets `fields`, its out_offset and, when the group record has them, first_job / n_jobs; a failed file's group
+    gets no jobs, at the end of the output.  Returns (data, jobs, output total, failed files)."""
+    ranged = "first_job" in groups.dtype.names
+    srcs, jobs, byte_at, job_at, out_at = [], [], 0, 0, 0
+    for i, src, j, fields, n_out in parts:
+        src = np.frombuffer(src, dtype=np.uint8) if not isinstance(src, np.ndarray) else np.ascontiguousarray(src, dtype=np.uint8)
+        g = groups[i]
+        for k, v in fields.items():
+            g[k] = v
+        g["out_offset"] = out_at
+        if ranged:
+            g["first_job"], g["n_jobs"] = job_at, len(j)
+        j["offset"] += np.uint64(byte_at)
+        srcs.append(src)
+        jobs.append(j)
+        byte_at += src.size
+        job_at += len(j)
+        out_at += n_out
+    good = {p[0] for p in parts}
+    failed = [i for i in range(len(groups)) if i not in good]
+    groups["out_offset"][failed] = out_at
+    if ranged:
+        groups["first_job"][failed] = job_at
+    data = np.concatenate(srcs) if srcs else np.zeros(0, dtype=np.uint8)
+    jobs = np.concatenate(jobs) if jobs else np.zeros(0, dtype=job_dtype)
+    return data, jobs, out_at, failed
+
+
+def _decode_batch(engine, device, inputs, cap, out_dtype, n_groups, result_dtype, host, dev):
+    """One device call: host() -> (out, results, status, extra) on numpy arrays, or with device=True the `inputs` copied to the
+    device and dev(*inputs_t, out_t, results_t, status_t) -> extra on torch CUDA tensors (out_t: `cap` elements of torch's
+    `out_dtype`; results_t: the bytes of n_groups result_dtype records), read back after the engine's stream is done.  Returns
+    (out, results, status, extra)."""
+    if not device:
+        return host()
+    import torch
+    d = torch.device("cuda", engine.device)
+    out = torch.empty(cap, dtype=getattr(torch, out_dtype), device=d)
+    results_t = torch.empty(n_groups * result_dtype.itemsize, dtype=torch.uint8, device=d)
+    status_t = torch.empty(len(inputs[1]), dtype=torch.uint8, device=d)
+    staged = [torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(-1)).to(d) for a in inputs]
+    torch.cuda.current_stream(d).synchronize()  # the copies above are on torch's stream, the decode on the engine's
+    extra = dev(*staged, out, results_t, status_t)
+    engine.sync()
+    return out, results_t.cpu().numpy().view(result_dtype), status_t.cpu().numpy(), extra
+
+
+def _per_file(out, groups, failed, shape):
+    """[(samples [frames, channels], sample_rate)] cut from `out` at each group's out_offset; shape(g) -> (frames, channels,
+    sample_rate).  A failed file gives (out[:0].reshape(0, 0), 0)."""
+    failed = set(failed)
+    result = []
+    for g in range(len(groups)):
+        if g in failed:
+            result.append((out[:0].reshape(0, 0), 0))
+            continue
+        n, ch, rate = shape(g)
+        at = int(groups[g]["out_offset"])
+        result.append((out[at:at + n * ch].reshape(n, ch), rate))
+    return result
+
+
+# ---- native FLAC, many files decoded on the device (frame headers and Rice residuals in device code) --------------------------
+
+def flac_files_plan(files, threads=None, errors=None):
+    """Host half of decode_flac_files: every file indexed (symgpu_flac_index, on `threads` host threads), their bytes concatenated
+    once, one job per packet and one group per file.  Returns dict(data, jobs, groups, rates, out_cap, failed).  A file that cannot
+    be indexed (listed in `failed`) gets a group without jobs; its message goes to errors[i] when `errors` is a dict."""
+    ix, messages = _index_files(files, packetizer.flac_index, threads)
     if errors is not None:
         errors.update(messages)
-    bufs = [np.frombuffer(f, dtype=np.uint8) if not isinstance(f, np.ndarray) else np.ascontiguousarray(f, dtype=np.uint8) for f in files]
-    good = [i for i in range(len(files)) if ix[i] is not None]
-    data = np.concatenate([bufs[i] for i in good]) if good else np.zeros(0, dtype=np.uint8)
     groups = np.zeros(len(files), dtype=nat.FLAC_GROUP_DTYPE)
     groups["channels"] = 1
     rates = np.zeros(len(files), dtype=np.int64)
-    jobs, byte_at, out_at = [], 0, 0
-    for i in good:
-        info, packets = ix[i]
-        g = groups[i]
-        g["out_offset"], g["max_block"], g["bits_per_sample"], g["channels"] = out_at, int(info["block_max"]), int(info["bits_per_sample"]), int(info["channels"])
+    parts = []
+    for i, x in enumerate(ix):
+        if x is None:
+            continue
+        info, packets = x
         rates[i] = int(info["sample_rate"])
         j = np.zeros(len(packets), dtype=nat.FLAC_JOB_DTYPE)
-        j["offset"], j["len"], j["group"], j["slot"] = packets["offset"] + byte_at, packets["size"], i, packets["dur"]
-        jobs.append(j)
-        byte_at += bufs[i].size
-        out_at += int(packets["dur"].astype(np.int64).sum()) * int(info["channels"])
-    failed = [i for i in range(len(files)) if ix[i] is None]
-    groups["out_offset"][failed] = out_at
-    jobs = np.concatenate(jobs) if jobs else np.zeros(0, dtype=nat.FLAC_JOB_DTYPE)
-    return dict(data=data, jobs=jobs, groups=groups, rates=rates, out_cap=out_at, failed=failed)
+        j["offset"], j["len"], j["group"], j["slot"] = packets["offset"], packets["size"], i, packets["dur"]
+        fields = dict(max_block=int(info["block_max"]), bits_per_sample=int(info["bits_per_sample"]), channels=int(info["channels"]))
+        parts.append((i, files[i], j, fields, int(packets["dur"].astype(np.int64).sum()) * int(info["channels"])))
+    data, jobs, cap, failed = _batch(groups, parts, nat.FLAC_JOB_DTYPE)
+    return dict(data=data, jobs=jobs, groups=groups, rates=rates, out_cap=cap, failed=failed)
 
 
 def decode_flac_files(engine, files, threads=None, device=False, errors=None):
@@ -477,50 +550,20 @@ def decode_flac_files(engine, files, threads=None, device=False, errors=None):
     result with sample rate 0 (its message in errors[i] when `errors` is a dict)."""
     plan = flac_files_plan(files, threads, errors)
     groups, rates, cap = plan["groups"], plan["rates"], plan["out_cap"]
-    if device:
+    def dev(data_t, jobs_t, groups_t, out_t, frames_t, status_t):
         import torch
-        dev = torch.device("cuda", engine.device)
-        as_t = lambda a: torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(-1)).to(dev)  # noqa: E731
-        out = torch.empty(cap, dtype=torch.int32, device=dev)
-        frames_t = torch.empty(len(groups), dtype=torch.int64, device=dev)
-        status_t = torch.empty(len(plan["jobs"]), dtype=torch.uint8, device=dev)
-        data_t, jobs_t, groups_t = as_t(plan["data"]), as_t(plan["jobs"]), as_t(groups)
-        torch.cuda.current_stream(dev).synchronize()  # the copies above are on torch's stream, the decode on the engine's
-        engine.flac_decode_dev(data_t, jobs_t, groups_t, out, frames_t, status_t)
-        engine.sync()
-        group_frames = frames_t.cpu().numpy()
-    else:
-        out, group_frames, _ = engine.flac_decode_host(plan["data"], plan["jobs"], groups, cap)
-    result = []
-    for g in range(len(groups)):
-        ch, at, n = int(groups[g]["channels"]), int(groups[g]["out_offset"]), int(group_frames[g])
-        if g in plan["failed"]:
-            ch = 0
-        result.append((out[at:at + n * ch].reshape(n, ch), int(rates[g])))
-    return result
+        engine.flac_decode_dev(data_t, jobs_t, groups_t, out_t, frames_t.view(torch.int64), status_t)
+    out, group_frames, _, _ = _decode_batch(engine, device, (plan["data"], plan["jobs"], groups), cap, "int32", len(groups), np.dtype(np.int64),
+                                            lambda: (*engine.flac_decode_host(plan["data"], plan["jobs"], groups, cap), None), dev)
+    return _per_file(out, groups, plan["failed"], lambda g: (int(group_frames[g]), int(groups[g]["channels"]), int(rates[g])))
 
 
 # ---- MPEG Layer I / II, many files decoded on the device (header, side information and samples in device code) ----------------
 
-_TORCH_DTYPES = {nat.FMT_F32: "float32", nat.FMT_S16: "int16", nat.FMT_S24: "int32", nat.FMT_S32: "int32", nat.FMT_U8: "uint8"}
-
-
 def mpa_index_files(files, threads=None):
     """symgpu_mpa_index of every file on `threads` host threads: [(track, packets) | None], {i: message} for the files that cannot be
     indexed."""
-    import concurrent.futures
-    import os
-    messages = {}
-
-    def index(i):
-        try:
-            return packetizer.mpa_index(files[i])
-        except Exception as e:  # noqa: BLE001 -- one bad file must not abort the batch; its message is kept
-            messages[i] = f"{type(e).__name__}: {e}"
-            return None
-    with concurrent.futures.ThreadPoolExecutor(max_workers=threads or os.cpu_count()) as pool:
-        ix = list(pool.map(index, range(len(files))))
-    return ix, messages
+    return _index_files(files, packetizer.mpa_index, threads)
 
 
 def _keep_layers(ix, messages, layers, what):
@@ -533,6 +576,22 @@ def _keep_layers(ix, messages, layers, what):
     return ix
 
 
+def _mpa_jobs(packets, job_dtype):
+    """One job per indexed MPEG packet, its offset within the file and its trims (the end trim saturated to 32 bits)."""
+    j = np.zeros(len(packets), dtype=job_dtype)
+    j["offset"], j["len"] = packets["offset"], packets["size"]
+    j["trim_start"] = packets["trim_start"]
+    j["trim_end"] = np.minimum(packets["trim_end"].astype(np.uint64), np.uint64(0xFFFFFFFF))
+    return j
+
+
+def _mpa_shape(r, track):
+    """(frames, channels, sample_rate) of an MPEG file's group result."""
+    if int(r["packets"]) == 0:   # no frame survived: the track's parameters, as decode_mpeg_audio reports them
+        return 0, int(track["channels"]), int(track["sample_rate"])
+    return int(r["frames"]), int(r["channels"]), int(r["sample_rate"])
+
+
 def mpa12_files_plan(files, threads=None, errors=None, index=None):
     """Host half of decode_mpa12_files: every file indexed (symgpu_mpa_index, on `threads` host threads), their bytes concatenated
     once, one job per packet and one group per file (group i uses state slot i).  Returns dict(data, jobs, groups, tracks, out_samples,
@@ -542,33 +601,18 @@ def mpa12_files_plan(files, threads=None, errors=None, index=None):
     ix = _keep_layers(ix, messages, (1, 2), "decode_mpa12_files takes Layer I / II files")
     if errors is not None:
         errors.update(messages)
-    bufs = [np.frombuffer(f, dtype=np.uint8) if not isinstance(f, np.ndarray) else np.ascontiguousarray(f, dtype=np.uint8) for f in files]
-    good = [i for i in range(len(files)) if ix[i] is not None]
-    data = np.concatenate([bufs[i] for i in good]) if good else np.zeros(0, dtype=np.uint8)
     groups = np.zeros(len(files), dtype=nat.MPA12_GROUP_DTYPE)
     groups["slot"] = np.arange(len(files))
     groups["layer"] = 1
-    jobs, byte_at, job_at, out_at = [], 0, 0, 0
-    sat = np.uint64(0xFFFFFFFF)
-    for i in good:
-        track, packets = ix[i]
-        layer, n = int(track["layer"]), len(packets)
-        g = groups[i]
-        g["out_offset"], g["first_job"], g["n_jobs"], g["layer"] = out_at, job_at, n, layer
-        j = np.zeros(n, dtype=nat.MPA12_JOB_DTYPE)
-        j["offset"], j["len"] = packets["offset"] + np.uint64(byte_at), packets["size"]
-        j["trim_start"] = packets["trim_start"]
-        j["trim_end"] = np.minimum(packets["trim_end"].astype(np.uint64), sat)
-        jobs.append(j)
-        byte_at += bufs[i].size
-        job_at += n
-        out_at += 2 * n * (384 if layer == 1 else 1152)
-    failed = [i for i in range(len(files)) if ix[i] is None]
-    groups["out_offset"][failed] = out_at
-    groups["first_job"][failed] = job_at
-    jobs = np.concatenate(jobs) if jobs else np.zeros(0, dtype=nat.MPA12_JOB_DTYPE)
+    parts = []
+    for i, x in enumerate(ix):
+        if x is not None:
+            track, packets = x
+            layer = int(track["layer"])
+            parts.append((i, files[i], _mpa_jobs(packets, nat.MPA12_JOB_DTYPE), dict(layer=layer), 2 * len(packets) * (384 if layer == 1 else 1152)))
+    data, jobs, cap, failed = _batch(groups, parts, nat.MPA12_JOB_DTYPE)
     tracks = [None if t is None else t[0] for t in ix]
-    return dict(data=data, jobs=jobs, groups=groups, tracks=tracks, out_samples=out_at, failed=failed)
+    return dict(data=data, jobs=jobs, groups=groups, tracks=tracks, out_samples=cap, failed=failed)
 
 
 def decode_mpa12_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False, errors=None, index=None):
@@ -581,32 +625,11 @@ def decode_mpa12_files(engine, files, fmt=nat.FMT_S16, threads=None, device=Fals
     plan = mpa12_files_plan(files, threads, errors, index)
     groups, cap = plan["groups"], plan["out_samples"]
     engine.mp3_streams_alloc(max(len(files), 1))
-    if device:
-        import torch
-        dev = torch.device("cuda", engine.device)
-        as_t = lambda a: torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(-1)).to(dev)  # noqa: E731
-        out = torch.empty(cap, dtype=getattr(torch, _TORCH_DTYPES[fmt]), device=dev)
-        results_t = torch.empty(len(groups) * nat.MPA12_RESULT_DTYPE.itemsize, dtype=torch.uint8, device=dev)
-        status_t = torch.empty(len(plan["jobs"]), dtype=torch.uint8, device=dev)
-        data_t, jobs_t = as_t(plan["data"]), as_t(plan["jobs"])
-        torch.cuda.current_stream(dev).synchronize()  # the copies above are on torch's stream, the decode on the engine's
-        engine.mpa12_decode_dev(data_t, jobs_t, groups, fmt, out, results_t, status_t)
-        engine.sync()
-        results = results_t.cpu().numpy().view(nat.MPA12_RESULT_DTYPE)
-    else:
-        out, results, _ = engine.mpa12_decode_host(plan["data"], plan["jobs"], groups, fmt, cap)
-    result = []
-    for g in range(len(groups)):
-        if g in plan["failed"]:
-            result.append((out[:0].reshape(0, 0), 0))
-            continue
-        r, track = results[g], plan["tracks"][g]
-        if int(r["packets"]) == 0:   # no frame survived: the track's parameters, as decode_mpeg_audio reports them
-            result.append((out[:0].reshape(0, int(track["channels"])), int(track["sample_rate"])))
-            continue
-        ch, at, n = int(r["channels"]), int(groups[g]["out_offset"]), int(r["frames"])
-        result.append((out[at:at + n * ch].reshape(n, ch), int(r["sample_rate"])))
-    return result
+    out, results, _, _ = _decode_batch(
+        engine, device, (plan["data"], plan["jobs"]), cap, _TORCH_DTYPES[fmt], len(groups), nat.MPA12_RESULT_DTYPE,
+        lambda: (*engine.mpa12_decode_host(plan["data"], plan["jobs"], groups, fmt, cap), None),
+        lambda data_t, jobs_t, out_t, results_t, status_t: engine.mpa12_decode_dev(data_t, jobs_t, groups, fmt, out_t, results_t, status_t))
+    return _per_file(out, groups, plan["failed"], lambda g: _mpa_shape(results[g], plan["tracks"][g]))
 
 
 # ---- MPEG Layer III, many files decoded on the device (side information, bit reservoir and Huffman data in device code) ---------
@@ -620,33 +643,19 @@ def mp3_files_plan(files, threads=None, errors=None, index=None):
     ix = _keep_layers(ix, messages, (3,), "decode_mp3_files takes Layer III files")
     if errors is not None:
         errors.update(messages)
-    bufs = [np.frombuffer(f, dtype=np.uint8) if not isinstance(f, np.ndarray) else np.ascontiguousarray(f, dtype=np.uint8) for f in files]
-    good = [i for i in range(len(files)) if ix[i] is not None]
-    data = np.concatenate([bufs[i] for i in good]) if good else np.zeros(0, dtype=np.uint8)
     groups = np.zeros(len(files), dtype=nat.MP3_GROUP_DTYPE)
     groups["slot"] = np.arange(len(files))
     groups["granules"], groups["channels"] = 2, 2
-    jobs, byte_at, job_at, out_at = [], 0, 0, 0
-    sat = np.uint64(0xFFFFFFFF)
-    for i in good:
-        track, packets = ix[i]
-        n, granules, channels = len(packets), 2 if int(track["version"]) == 0 else 1, int(track["channels"])
-        g = groups[i]
-        g["out_offset"], g["first_job"], g["n_jobs"], g["granules"], g["channels"] = out_at, job_at, n, granules, channels
-        j = np.zeros(n, dtype=nat.MP3_JOB_DTYPE)
-        j["offset"], j["len"] = packets["offset"] + np.uint64(byte_at), packets["size"]
-        j["trim_start"] = packets["trim_start"]
-        j["trim_end"] = np.minimum(packets["trim_end"].astype(np.uint64), sat)
-        jobs.append(j)
-        byte_at += bufs[i].size
-        job_at += n
-        out_at += n * granules * 576 * channels
-    failed = [i for i in range(len(files)) if ix[i] is None]
-    groups["out_offset"][failed] = out_at
-    groups["first_job"][failed] = job_at
-    jobs = np.concatenate(jobs) if jobs else np.zeros(0, dtype=nat.MP3_JOB_DTYPE)
+    parts = []
+    for i, x in enumerate(ix):
+        if x is not None:
+            track, packets = x
+            granules, channels = 2 if int(track["version"]) == 0 else 1, int(track["channels"])
+            parts.append((i, files[i], _mpa_jobs(packets, nat.MP3_JOB_DTYPE), dict(granules=granules, channels=channels),
+                          len(packets) * granules * 576 * channels))
+    data, jobs, cap, failed = _batch(groups, parts, nat.MP3_JOB_DTYPE)
     tracks = [None if t is None else t[0] for t in ix]
-    return dict(data=data, jobs=jobs, groups=groups, tracks=tracks, out_samples=out_at, failed=failed)
+    return dict(data=data, jobs=jobs, groups=groups, tracks=tracks, out_samples=cap, failed=failed)
 
 
 def decode_mp3_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False, errors=None, index=None, stats=None):
@@ -661,35 +670,13 @@ def decode_mp3_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False,
     plan = mp3_files_plan(files, threads, errors, index)
     groups, cap = plan["groups"], plan["out_samples"]
     engine.mp3_streams_alloc(max(len(files), 1))
-    if device:
-        import torch
-        dev = torch.device("cuda", engine.device)
-        as_t = lambda a: torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(-1)).to(dev)  # noqa: E731
-        out = torch.empty(cap, dtype=getattr(torch, _TORCH_DTYPES[fmt]), device=dev)
-        results_t = torch.empty(len(groups) * nat.MP3_RESULT_DTYPE.itemsize, dtype=torch.uint8, device=dev)
-        status_t = torch.empty(len(plan["jobs"]), dtype=torch.uint8, device=dev)
-        data_t, jobs_t = as_t(plan["data"]), as_t(plan["jobs"])
-        torch.cuda.current_stream(dev).synchronize()  # the copies above are on torch's stream, the decode on the engine's
-        rounds = engine.mp3_decode_dev(data_t, jobs_t, groups, fmt, out, results_t, status_t)
-        engine.sync()
-        results = results_t.cpu().numpy().view(nat.MP3_RESULT_DTYPE)
-        status = status_t.cpu().numpy()
-    else:
-        out, results, status, rounds = engine.mp3_decode_host(plan["data"], plan["jobs"], groups, fmt, cap)
+    out, results, status, rounds = _decode_batch(
+        engine, device, (plan["data"], plan["jobs"]), cap, _TORCH_DTYPES[fmt], len(groups), nat.MP3_RESULT_DTYPE,
+        lambda: engine.mp3_decode_host(plan["data"], plan["jobs"], groups, fmt, cap),
+        lambda data_t, jobs_t, out_t, results_t, status_t: engine.mp3_decode_dev(data_t, jobs_t, groups, fmt, out_t, results_t, status_t))
     if stats is not None:
         stats.update(rounds=rounds, status=status)
-    result = []
-    for g in range(len(groups)):
-        if g in plan["failed"]:
-            result.append((out[:0].reshape(0, 0), 0))
-            continue
-        r, track = results[g], plan["tracks"][g]
-        if int(r["packets"]) == 0:   # no frame survived: the track's parameters, as decode_mpeg_audio reports them
-            result.append((out[:0].reshape(0, int(track["channels"])), int(track["sample_rate"])))
-            continue
-        ch, at, n = int(r["channels"]), int(groups[g]["out_offset"]), int(r["frames"])
-        result.append((out[at:at + n * ch].reshape(n, ch), int(r["sample_rate"])))
-    return result
+    return _per_file(out, groups, plan["failed"], lambda g: _mpa_shape(results[g], plan["tracks"][g]))
 
 
 # ---- ADTS AAC-LC, many files decoded on the device (elements, scale factors, Huffman spectra and noise in device code) ----------
@@ -699,43 +686,21 @@ def aac_files_plan(files, threads=None, errors=None):
     one job per raw_data_block and one group per file (group i uses state slot i).  Returns dict(data, jobs, groups, out_samples,
     failed).  A file that cannot be indexed or whose channel configuration is outside 1 / 2 (listed in `failed`) gets a group
     without jobs; its message goes to errors[i] when `errors` is a dict."""
-    import concurrent.futures
-    import os
-    messages = {}
-
-    def index(i):
-        try:
-            return adts_aac_index(files[i])
-        except Exception as e:  # noqa: BLE001 -- one bad file must not abort the batch; its message is kept
-            messages[i] = f"{type(e).__name__}: {e}"
-            return None
-    with concurrent.futures.ThreadPoolExecutor(max_workers=threads or os.cpu_count()) as pool:
-        ix = list(pool.map(index, range(len(files))))
+    ix, messages = _index_files(files, adts_aac_index, threads)
     if errors is not None:
         errors.update(messages)
-    bufs = [np.frombuffer(f, dtype=np.uint8) if not isinstance(f, np.ndarray) else np.ascontiguousarray(f, dtype=np.uint8) for f in files]
-    good = [i for i in range(len(files)) if ix[i] is not None]
-    data = np.concatenate([bufs[i] for i in good]) if good else np.zeros(0, dtype=np.uint8)
     groups = np.zeros(len(files), dtype=nat.AAC_GROUP_DTYPE)
     groups["slot"] = np.arange(len(files))
     groups["channels"], groups["sample_rate"] = 1, 44100
-    jobs, byte_at, job_at, out_at = [], 0, 0, 0
-    for i in good:
-        packets, rate, channels = ix[i]
-        n = len(packets)
-        g = groups[i]
-        g["out_offset"], g["first_job"], g["n_jobs"], g["sample_rate"], g["channels"] = out_at, job_at, n, rate, channels
-        j = np.zeros(n, dtype=nat.PIECE_DTYPE)
-        j["offset"], j["len"] = packets["offset"] + np.uint64(byte_at), packets["size"]
-        jobs.append(j)
-        byte_at += bufs[i].size
-        job_at += n
-        out_at += n * 1024 * channels
-    failed = [i for i in range(len(files)) if ix[i] is None]
-    groups["out_offset"][failed] = out_at
-    groups["first_job"][failed] = job_at
-    jobs = np.concatenate(jobs) if jobs else np.zeros(0, dtype=nat.PIECE_DTYPE)
-    return dict(data=data, jobs=jobs, groups=groups, out_samples=out_at, failed=failed)
+    parts = []
+    for i, x in enumerate(ix):
+        if x is not None:
+            packets, rate, channels = x
+            j = np.zeros(len(packets), dtype=nat.PIECE_DTYPE)
+            j["offset"], j["len"] = packets["offset"], packets["size"]
+            parts.append((i, files[i], j, dict(sample_rate=rate, channels=channels), len(packets) * 1024 * channels))
+    data, jobs, cap, failed = _batch(groups, parts, nat.PIECE_DTYPE)
+    return dict(data=data, jobs=jobs, groups=groups, out_samples=cap, failed=failed)
 
 
 def decode_aac_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False, errors=None, stats=None):
@@ -752,31 +717,14 @@ def decode_aac_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False,
     plan = aac_files_plan(files, threads, errors)
     groups, cap = plan["groups"], plan["out_samples"]
     engine.aac_streams_alloc(max(len(files), 1))
-    if device:
-        import torch
-        dev = torch.device("cuda", engine.device)
-        as_t = lambda a: torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(-1)).to(dev)  # noqa: E731
-        out = torch.empty(cap, dtype=getattr(torch, _TORCH_DTYPES[fmt]), device=dev)
-        results_t = torch.empty(len(groups) * nat.AAC_RESULT_DTYPE.itemsize, dtype=torch.uint8, device=dev)
-        status_t = torch.empty(len(plan["jobs"]), dtype=torch.uint8, device=dev)
-        data_t, jobs_t = as_t(plan["data"]), as_t(plan["jobs"])
-        torch.cuda.current_stream(dev).synchronize()  # the copies above are on torch's stream, the decode on the engine's
-        redone = engine.aac_decode_dev(data_t, jobs_t, groups, fmt, out, results_t, status_t)
-        engine.sync()
-        results = results_t.cpu().numpy().view(nat.AAC_RESULT_DTYPE)
-        status = status_t.cpu().numpy()
-    else:
-        out, results, status, redone = engine.aac_decode_host(plan["data"], plan["jobs"], groups, fmt, cap)
+    out, results, status, redone = _decode_batch(
+        engine, device, (plan["data"], plan["jobs"]), cap, _TORCH_DTYPES[fmt], len(groups), nat.AAC_RESULT_DTYPE,
+        lambda: engine.aac_decode_host(plan["data"], plan["jobs"], groups, fmt, cap),
+        lambda data_t, jobs_t, out_t, results_t, status_t: engine.aac_decode_dev(data_t, jobs_t, groups, fmt, out_t, results_t, status_t))
     if stats is not None:
         stats.update(status=status, n_redecoded=redone)
-    result = []
-    for g in range(len(groups)):
-        if g in plan["failed"]:
-            result.append((out[:0].reshape(0, 0), 0))
-            continue
-        ch, at, n = int(groups[g]["channels"]), int(groups[g]["out_offset"]), int(results[g]["frames"])
-        result.append((out[at:at + n * ch].reshape(n, ch), int(groups[g]["sample_rate"])))
-    return result
+    return _per_file(out, groups, plan["failed"],
+                     lambda g: (int(results[g]["frames"]), int(groups[g]["channels"]), int(groups[g]["sample_rate"])))
 
 
 def decode_mpeg_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False, errors=None):
@@ -811,29 +759,18 @@ def vorbis_files_plan(files, threads=None, errors=None):
     byte-identical identification and setup headers sharing one setup, and one group per file.  Returns dict(data, headers,
     setups, jobs, groups, out_samples, failed).  A file that cannot be indexed or opened -- not Ogg, more than two channels, floor
     type 0, ... (listed in `failed`) -- gets a group without jobs; its message goes to errors[i] when `errors` is a dict."""
-    import concurrent.futures
-    import os
-    messages = {}
-
-    def index(i):
-        try:
-            ix = ogg_vorbis_index(files[i])
-            ix["fe"].close()   # (it checked the setup; the device call builds its own)
-            return ix
-        except Exception as e:  # noqa: BLE001 -- one bad file must not abort the batch; its message is kept
-            messages[i] = f"{type(e).__name__}: {e}"
-            return None
-    with concurrent.futures.ThreadPoolExecutor(max_workers=threads or os.cpu_count()) as pool:
-        ix = list(pool.map(index, range(len(files))))
+    def index(f):
+        ix = ogg_vorbis_index(f)
+        ix["fe"].close()   # (it checked the setup; the device call builds its own)
+        return ix
+    ix, messages = _index_files(files, index, threads)
     if errors is not None:
         errors.update(messages)
-    good = [i for i in range(len(files)) if ix[i] is not None]
-    data = np.concatenate([ix[i]["blob"] for i in good]) if good else np.zeros(0, dtype=np.uint8)
     groups = np.zeros(len(files), dtype=nat.VORBIS_GROUP_DTYPE)
-    setup_of, headers, refs = {}, [], []
-    jobs, byte_at, job_at, out_at, head_at = [], 0, 0, 0, 0
-    for i in good:
-        x = ix[i]
+    setup_of, headers, refs, parts, head_at = {}, [], [], [], 0
+    for i, x in enumerate(ix):
+        if x is None:
+            continue
         ident_b, setup_b = x["headers"]
         key = (ident_b, setup_b)
         if key not in setup_of:
@@ -842,24 +779,16 @@ def vorbis_files_plan(files, threads=None, errors=None):
             headers += [ident_b, setup_b]
             head_at += len(ident_b) + len(setup_b)
         n, channels = len(x["table"]), int(x["ident"]["channels"])
-        g = groups[i]
-        g["out_offset"], g["first_job"], g["n_jobs"], g["setup"] = out_at, job_at, n, setup_of[key]
         j = np.zeros(n, dtype=nat.VORBIS_JOB_DTYPE)
-        j["offset"], j["len"] = x["table"]["offset"] + np.uint64(byte_at), x["table"]["len"]
+        j["offset"], j["len"] = x["table"]["offset"], x["table"]["len"]
         j["discard"] = np.clip(x["discard"], 0, 0xffffffff)
         j["trim_end"] = np.clip(x["trim_end"], 0, 0xffffffff)
-        jobs.append(j)
-        byte_at += x["blob"].size
-        job_at += n
-        out_at += n * ((1 << int(x["ident"]["bs1_exp"])) >> 1) * channels
-    failed = [i for i in range(len(files)) if ix[i] is None]
-    groups["out_offset"][failed] = out_at
-    groups["first_job"][failed] = job_at
+        parts.append((i, x["blob"], j, dict(setup=setup_of[key]), n * ((1 << int(x["ident"]["bs1_exp"])) >> 1) * channels))
+    data, jobs, cap, failed = _batch(groups, parts, nat.VORBIS_JOB_DTYPE)
     setups = np.zeros(len(refs), dtype=nat.VORBIS_SETUP_REF_DTYPE)
     for k, r in enumerate(refs):
         setups[k] = r
-    jobs = np.concatenate(jobs) if jobs else np.zeros(0, dtype=nat.VORBIS_JOB_DTYPE)
-    return dict(data=data, headers=b"".join(headers), setups=setups, jobs=jobs, groups=groups, out_samples=out_at, failed=failed)
+    return dict(data=data, headers=b"".join(headers), setups=setups, jobs=jobs, groups=groups, out_samples=cap, failed=failed)
 
 
 def decode_vorbis_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False, errors=None, stats=None):
@@ -874,32 +803,18 @@ def decode_vorbis_files(engine, files, fmt=nat.FMT_S16, threads=None, device=Fal
         raise ValueError(f"decode_vorbis_files takes at most {nat.VORBIS_MAX_FILES} files per call, not {len(files)}")
     plan = vorbis_files_plan(files, threads, errors)
     groups, cap, setups = plan["groups"], plan["out_samples"], plan["setups"]
-    if device:
-        import torch
-        dev = torch.device("cuda", engine.device)
-        out = torch.empty(cap, dtype=getattr(torch, _TORCH_DTYPES[fmt]), device=dev)
-        results_t = torch.zeros(len(groups) * nat.VORBIS_RESULT_DTYPE.itemsize, dtype=torch.uint8, device=dev)
-        status_t = torch.empty(len(plan["jobs"]), dtype=torch.uint8, device=dev)
-        if len(setups):
-            as_t = lambda a: torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(-1)).to(dev)  # noqa: E731
-            data_t, jobs_t = as_t(plan["data"]), as_t(plan["jobs"])
-            torch.cuda.current_stream(dev).synchronize()  # the copies above are on torch's stream, the decode on the engine's
-            engine.vorbis_decode_dev(plan["headers"], setups, data_t, jobs_t, groups, fmt, out, results_t, status_t)
-            engine.sync()
-        results = results_t.cpu().numpy().view(nat.VORBIS_RESULT_DTYPE)
-        status = status_t.cpu().numpy()
-    elif len(setups):
-        out, results, status = engine.vorbis_decode_host(plan["headers"], setups, plan["data"], plan["jobs"], groups, fmt, cap)
-    else:   # no file could be opened: nothing to decode
-        out, results, status = np.zeros(0, dtype=nat.FMT_NUMPY[fmt]), np.zeros(len(groups), dtype=nat.VORBIS_RESULT_DTYPE), np.zeros(0, dtype=np.uint8)
+
+    def host():
+        if not len(setups):   # no file could be opened: nothing to decode
+            return np.zeros(0, dtype=nat.FMT_NUMPY[fmt]), np.zeros(len(groups), dtype=nat.VORBIS_RESULT_DTYPE), np.zeros(0, dtype=np.uint8), None
+        return (*engine.vorbis_decode_host(plan["headers"], setups, plan["data"], plan["jobs"], groups, fmt, cap), None)
+
+    def dev(data_t, jobs_t, out_t, results_t, status_t):
+        if len(setups):       # (else every file failed: no result is read)
+            engine.vorbis_decode_dev(plan["headers"], setups, data_t, jobs_t, groups, fmt, out_t, results_t, status_t)
+    out, results, status, _ = _decode_batch(engine, device, (plan["data"], plan["jobs"]), cap, _TORCH_DTYPES[fmt], len(groups),
+                                            nat.VORBIS_RESULT_DTYPE, host, dev)
     if stats is not None:
         stats.update(status=status, n_setups=len(setups))
-    failed = set(plan["failed"])
-    result = []
-    for g in range(len(groups)):
-        if g in failed:
-            result.append((out[:0].reshape(0, 0), 0))
-            continue
-        ch, at, n = int(results[g]["channels"]), int(groups[g]["out_offset"]), int(results[g]["frames"])
-        result.append((out[at:at + n * ch].reshape(n, ch), int(results[g]["sample_rate"])))
-    return result
+    return _per_file(out, groups, plan["failed"],
+                     lambda g: (int(results[g]["frames"]), int(results[g]["channels"]), int(results[g]["sample_rate"])))

@@ -24,6 +24,21 @@ def _np_ptr(a):
     return a.ctypes.data_as(ctypes.c_void_p)
 
 
+def _byte_view(data):
+    """bytes, or any array, as a contiguous uint8 array."""
+    return np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
+
+
+def _host_ptr(a):
+    """A numpy array's pointer, or None (NULL) for an empty one."""
+    return _np_ptr(a) if a.size else None
+
+
+def _dev_ptr(t):
+    """A torch CUDA tensor's pointer, or None (NULL) for an empty one."""
+    return ctypes.c_void_p(t.data_ptr()) if t.numel() else None
+
+
 class Engine:
     def __init__(self, device=0):
         self._lib = _native.lib()
@@ -212,7 +227,7 @@ class Engine:
         [out_cap], group_frames uint64 [groups], status uint8 [jobs]); file g's PCM is out[out_offset:][:group_frames[g] * channels]
         as [frames, channels]."""
         from ._native import FLAC_GROUP_DTYPE, FLAC_JOB_DTYPE
-        a = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
+        a = _byte_view(data)
         jobs = np.ascontiguousarray(jobs, dtype=FLAC_JOB_DTYPE)
         groups = np.ascontiguousarray(groups, dtype=FLAC_GROUP_DTYPE)
         if out is None:
@@ -220,10 +235,8 @@ class Engine:
         assert out.dtype == np.int32 and out.flags.c_contiguous and out.size >= out_cap
         group_frames = np.zeros(len(groups), dtype=np.uint64)
         status = np.zeros(len(jobs), dtype=np.uint8)
-        self._check(self._lib.symgpu_flac_decode_host(self._ctx, _np_ptr(a) if a.size else None, a.size, _np_ptr(jobs) if len(jobs) else None, len(jobs),
-                                                      _np_ptr(groups) if len(groups) else None, len(groups), _np_ptr(out) if out_cap else None,
-                                                      int(out_cap), _np_ptr(group_frames) if len(groups) else None,
-                                                      _np_ptr(status) if len(jobs) else None))
+        self._check(self._lib.symgpu_flac_decode_host(self._ctx, _host_ptr(a), a.size, _host_ptr(jobs), len(jobs), _host_ptr(groups), len(groups),
+                                                      _host_ptr(out), int(out_cap), _host_ptr(group_frames), _host_ptr(status)))
         return out, group_frames, status
 
     def flac_decode_dev(self, data_t, jobs_t, groups_t, out_t, group_frames_t, status_t):
@@ -235,9 +248,8 @@ class Engine:
         n_jobs = jobs_t.numel() * jobs_t.element_size() // FLAC_JOB_DTYPE.itemsize
         n_groups = groups_t.numel() * groups_t.element_size() // FLAC_GROUP_DTYPE.itemsize
         assert group_frames_t.numel() >= n_groups and group_frames_t.element_size() == 8 and status_t.numel() >= n_jobs
-        ptr = lambda t: ctypes.c_void_p(t.data_ptr()) if t.numel() else None  # noqa: E731
-        self._check(self._lib.symgpu_flac_decode_dev(self._ctx, ptr(data_t), data_t.numel(), ptr(jobs_t), n_jobs, ptr(groups_t), n_groups, ptr(out_t),
-                                                     out_t.numel(), ptr(group_frames_t), ptr(status_t)))
+        self._check(self._lib.symgpu_flac_decode_dev(self._ctx, _dev_ptr(data_t), data_t.numel(), _dev_ptr(jobs_t), n_jobs, _dev_ptr(groups_t), n_groups,
+                                                     _dev_ptr(out_t), out_t.numel(), _dev_ptr(group_frames_t), _dev_ptr(status_t)))
 
     # -- MPEG Layer I / II decoded on the device ----------------------------------------------------------
     def mpa12_decode_host(self, data, jobs, groups, fmt, out_samples, out=None):
@@ -245,7 +257,7 @@ class Engine:
         (one per packet), groups MPA12_GROUP_DTYPE (one per file: its jobs, layer, state slot and output offset).  Returns (out [out_samples]
         of `fmt`, results MPA12_RESULT_DTYPE [groups], status uint8 [jobs]); file g's samples are out[out_offset:][:frames * channels]."""
         from ._native import MPA12_GROUP_DTYPE, MPA12_JOB_DTYPE, MPA12_RESULT_DTYPE
-        a = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
+        a = _byte_view(data)
         jobs = np.ascontiguousarray(jobs, dtype=MPA12_JOB_DTYPE)
         groups = np.ascontiguousarray(groups, dtype=MPA12_GROUP_DTYPE)
         if out is None:
@@ -253,10 +265,8 @@ class Engine:
         assert out.flags.c_contiguous
         results = np.zeros(len(groups), dtype=MPA12_RESULT_DTYPE)
         status = np.zeros(len(jobs), dtype=np.uint8)
-        self._check(self._lib.symgpu_mpa12_decode_host(self._ctx, _np_ptr(a) if a.size else None, a.size, _np_ptr(jobs) if len(jobs) else None, len(jobs),
-                                                       _np_ptr(groups) if len(groups) else None, len(groups), int(fmt),
-                                                       _np_ptr(out) if out.nbytes else None, out.nbytes, _np_ptr(results) if len(groups) else None,
-                                                       _np_ptr(status) if len(jobs) else None))
+        self._check(self._lib.symgpu_mpa12_decode_host(self._ctx, _host_ptr(a), a.size, _host_ptr(jobs), len(jobs), _host_ptr(groups), len(groups),
+                                                       int(fmt), _host_ptr(out), out.nbytes, _host_ptr(results), _host_ptr(status)))
         return out, results, status
 
     def mpa12_decode_dev(self, data_t, jobs_t, groups, fmt, out_t, results_t, status_t):
@@ -268,10 +278,9 @@ class Engine:
         groups = np.ascontiguousarray(groups, dtype=MPA12_GROUP_DTYPE)
         n_jobs = jobs_t.numel() * jobs_t.element_size() // MPA12_JOB_DTYPE.itemsize
         assert results_t.numel() * results_t.element_size() >= len(groups) * MPA12_RESULT_DTYPE.itemsize and status_t.numel() >= n_jobs
-        ptr = lambda t: ctypes.c_void_p(t.data_ptr()) if t.numel() else None  # noqa: E731
-        self._check(self._lib.symgpu_mpa12_decode_dev(self._ctx, ptr(data_t), data_t.numel(), ptr(jobs_t), n_jobs,
-                                                      _np_ptr(groups) if len(groups) else None, len(groups), int(fmt), ptr(out_t),
-                                                      out_t.numel() * out_t.element_size(), ptr(results_t), ptr(status_t)))
+        self._check(self._lib.symgpu_mpa12_decode_dev(self._ctx, _dev_ptr(data_t), data_t.numel(), _dev_ptr(jobs_t), n_jobs,
+                                                      _host_ptr(groups), len(groups), int(fmt), _dev_ptr(out_t),
+                                                      out_t.numel() * out_t.element_size(), _dev_ptr(results_t), _dev_ptr(status_t)))
 
     # -- MPEG Layer III decoded on the device -------------------------------------------------------------
     def mp3_decode_host(self, data, jobs, groups, fmt, out_samples, out=None):
@@ -280,7 +289,7 @@ class Engine:
         [out_samples] of `fmt`, results MP3_RESULT_DTYPE [groups], status uint8 [jobs], rounds); file g's samples are
         out[out_offset:][:frames * channels]."""
         from ._native import MP3_GROUP_DTYPE, MP3_JOB_DTYPE, MP3_RESULT_DTYPE
-        a = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
+        a = _byte_view(data)
         jobs = np.ascontiguousarray(jobs, dtype=MP3_JOB_DTYPE)
         groups = np.ascontiguousarray(groups, dtype=MP3_GROUP_DTYPE)
         if out is None:
@@ -289,10 +298,8 @@ class Engine:
         results = np.zeros(len(groups), dtype=MP3_RESULT_DTYPE)
         status = np.zeros(len(jobs), dtype=np.uint8)
         rounds = ctypes.c_uint32(0)
-        self._check(self._lib.symgpu_mp3_decode_host(self._ctx, _np_ptr(a) if a.size else None, a.size, _np_ptr(jobs) if len(jobs) else None, len(jobs),
-                                                     _np_ptr(groups) if len(groups) else None, len(groups), int(fmt),
-                                                     _np_ptr(out) if out.nbytes else None, out.nbytes, _np_ptr(results) if len(groups) else None,
-                                                     _np_ptr(status) if len(jobs) else None, ctypes.byref(rounds)))
+        self._check(self._lib.symgpu_mp3_decode_host(self._ctx, _host_ptr(a), a.size, _host_ptr(jobs), len(jobs), _host_ptr(groups), len(groups),
+                                                     int(fmt), _host_ptr(out), out.nbytes, _host_ptr(results), _host_ptr(status), ctypes.byref(rounds)))
         return out, results, status, rounds.value
 
     def mp3_decode_dev(self, data_t, jobs_t, groups, fmt, out_t, results_t, status_t):
@@ -305,11 +312,10 @@ class Engine:
         groups = np.ascontiguousarray(groups, dtype=MP3_GROUP_DTYPE)
         n_jobs = jobs_t.numel() * jobs_t.element_size() // MP3_JOB_DTYPE.itemsize
         assert results_t.numel() * results_t.element_size() >= len(groups) * MP3_RESULT_DTYPE.itemsize and status_t.numel() >= n_jobs
-        ptr = lambda t: ctypes.c_void_p(t.data_ptr()) if t.numel() else None  # noqa: E731
         rounds = ctypes.c_uint32(0)
-        self._check(self._lib.symgpu_mp3_decode_dev(self._ctx, ptr(data_t), data_t.numel(), ptr(jobs_t), n_jobs,
-                                                    _np_ptr(groups) if len(groups) else None, len(groups), int(fmt), ptr(out_t),
-                                                    out_t.numel() * out_t.element_size(), ptr(results_t), ptr(status_t), ctypes.byref(rounds)))
+        self._check(self._lib.symgpu_mp3_decode_dev(self._ctx, _dev_ptr(data_t), data_t.numel(), _dev_ptr(jobs_t), n_jobs,
+                                                    _host_ptr(groups), len(groups), int(fmt), _dev_ptr(out_t),
+                                                    out_t.numel() * out_t.element_size(), _dev_ptr(results_t), _dev_ptr(status_t), ctypes.byref(rounds)))
         return rounds.value
 
     # -- AAC-LC decoded on the device -------------------------------------------------------------------
@@ -319,7 +325,7 @@ class Engine:
         Returns (out [out_samples] of `fmt`, results AAC_RESULT_DTYPE [groups], status uint8 [jobs], n_redecoded); file g's samples
         are out[out_offset:][:frames * channels]."""
         from ._native import AAC_GROUP_DTYPE, AAC_RESULT_DTYPE, PIECE_DTYPE
-        a = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
+        a = _byte_view(data)
         jobs = np.ascontiguousarray(jobs, dtype=PIECE_DTYPE)
         groups = np.ascontiguousarray(groups, dtype=AAC_GROUP_DTYPE)
         if out is None:
@@ -328,10 +334,8 @@ class Engine:
         results = np.zeros(len(groups), dtype=AAC_RESULT_DTYPE)
         status = np.zeros(len(jobs), dtype=np.uint8)
         redone = ctypes.c_uint32(0)
-        self._check(self._lib.symgpu_aac_decode_host(self._ctx, _np_ptr(a) if a.size else None, a.size, _np_ptr(jobs) if len(jobs) else None, len(jobs),
-                                                     _np_ptr(groups) if len(groups) else None, len(groups), int(fmt),
-                                                     _np_ptr(out) if out.nbytes else None, out.nbytes, _np_ptr(results) if len(groups) else None,
-                                                     _np_ptr(status) if len(jobs) else None, ctypes.byref(redone)))
+        self._check(self._lib.symgpu_aac_decode_host(self._ctx, _host_ptr(a), a.size, _host_ptr(jobs), len(jobs), _host_ptr(groups), len(groups),
+                                                     int(fmt), _host_ptr(out), out.nbytes, _host_ptr(results), _host_ptr(status), ctypes.byref(redone)))
         return out, results, status, redone.value
 
     def aac_decode_dev(self, data_t, jobs_t, groups, fmt, out_t, results_t, status_t):
@@ -344,11 +348,10 @@ class Engine:
         groups = np.ascontiguousarray(groups, dtype=AAC_GROUP_DTYPE)
         n_jobs = jobs_t.numel() * jobs_t.element_size() // PIECE_DTYPE.itemsize
         assert results_t.numel() * results_t.element_size() >= len(groups) * AAC_RESULT_DTYPE.itemsize and status_t.numel() >= n_jobs
-        ptr = lambda t: ctypes.c_void_p(t.data_ptr()) if t.numel() else None  # noqa: E731
         redone = ctypes.c_uint32(0)
-        self._check(self._lib.symgpu_aac_decode_dev(self._ctx, ptr(data_t), data_t.numel(), ptr(jobs_t), n_jobs,
-                                                    _np_ptr(groups) if len(groups) else None, len(groups), int(fmt), ptr(out_t),
-                                                    out_t.numel() * out_t.element_size(), ptr(results_t), ptr(status_t), ctypes.byref(redone)))
+        self._check(self._lib.symgpu_aac_decode_dev(self._ctx, _dev_ptr(data_t), data_t.numel(), _dev_ptr(jobs_t), n_jobs,
+                                                    _host_ptr(groups), len(groups), int(fmt), _dev_ptr(out_t),
+                                                    out_t.numel() * out_t.element_size(), _dev_ptr(results_t), _dev_ptr(status_t), ctypes.byref(redone)))
         return redone.value
 
     def vorbis_decode_host(self, headers, setups, data, jobs, groups, fmt, out_samples, out=None):
@@ -358,8 +361,8 @@ class Engine:
         offset).  Returns (out [out_samples] of `fmt`, results VORBIS_RESULT_DTYPE [groups], status uint8 [jobs]); file g's
         samples are out[out_offset:][:frames * channels].  Replaces the engine's Vorbis stream and floor registration."""
         from ._native import VORBIS_GROUP_DTYPE, VORBIS_JOB_DTYPE, VORBIS_RESULT_DTYPE, VORBIS_SETUP_REF_DTYPE
-        h = np.frombuffer(headers, dtype=np.uint8) if not isinstance(headers, np.ndarray) else np.ascontiguousarray(headers, dtype=np.uint8)
-        a = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
+        h = _byte_view(headers)
+        a = _byte_view(data)
         setups = np.ascontiguousarray(setups, dtype=VORBIS_SETUP_REF_DTYPE)
         jobs = np.ascontiguousarray(jobs, dtype=VORBIS_JOB_DTYPE)
         groups = np.ascontiguousarray(groups, dtype=VORBIS_GROUP_DTYPE)
@@ -368,10 +371,9 @@ class Engine:
         assert out.flags.c_contiguous
         results = np.zeros(len(groups), dtype=VORBIS_RESULT_DTYPE)
         status = np.zeros(len(jobs), dtype=np.uint8)
-        opt = lambda x, n: _np_ptr(x) if n else None  # noqa: E731
-        self._check(self._lib.symgpu_vorbis_decode_host(self._ctx, opt(h, h.size), h.size, opt(setups, len(setups)), len(setups), opt(a, a.size), a.size,
-                                                        opt(jobs, len(jobs)), len(jobs), opt(groups, len(groups)), len(groups), int(fmt),
-                                                        opt(out, out.nbytes), out.nbytes, opt(results, len(groups)), opt(status, len(jobs))))
+        self._check(self._lib.symgpu_vorbis_decode_host(self._ctx, _host_ptr(h), h.size, _host_ptr(setups), len(setups), _host_ptr(a), a.size,
+                                                        _host_ptr(jobs), len(jobs), _host_ptr(groups), len(groups), int(fmt),
+                                                        _host_ptr(out), out.nbytes, _host_ptr(results), _host_ptr(status)))
         return out, results, status
 
     def vorbis_decode_dev(self, headers, setups, data_t, jobs_t, groups, fmt, out_t, results_t, status_t):
@@ -381,16 +383,14 @@ class Engine:
         from ._native import VORBIS_GROUP_DTYPE, VORBIS_JOB_DTYPE, VORBIS_RESULT_DTYPE, VORBIS_SETUP_REF_DTYPE
         ts = (data_t, jobs_t, out_t, results_t, status_t)
         assert all(t.is_cuda and t.is_contiguous() for t in ts)
-        h = np.frombuffer(headers, dtype=np.uint8) if not isinstance(headers, np.ndarray) else np.ascontiguousarray(headers, dtype=np.uint8)
+        h = _byte_view(headers)
         setups = np.ascontiguousarray(setups, dtype=VORBIS_SETUP_REF_DTYPE)
         groups = np.ascontiguousarray(groups, dtype=VORBIS_GROUP_DTYPE)
         n_jobs = jobs_t.numel() * jobs_t.element_size() // VORBIS_JOB_DTYPE.itemsize
         assert results_t.numel() * results_t.element_size() >= len(groups) * VORBIS_RESULT_DTYPE.itemsize and status_t.numel() >= n_jobs
-        ptr = lambda t: ctypes.c_void_p(t.data_ptr()) if t.numel() else None  # noqa: E731
-        self._check(self._lib.symgpu_vorbis_decode_dev(self._ctx, _np_ptr(h) if h.size else None, h.size, _np_ptr(setups) if len(setups) else None,
-                                                       len(setups), ptr(data_t), data_t.numel(), ptr(jobs_t), n_jobs,
-                                                       _np_ptr(groups) if len(groups) else None, len(groups), int(fmt), ptr(out_t),
-                                                       out_t.numel() * out_t.element_size(), ptr(results_t), ptr(status_t)))
+        self._check(self._lib.symgpu_vorbis_decode_dev(self._ctx, _host_ptr(h), h.size, _host_ptr(setups), len(setups), _dev_ptr(data_t), data_t.numel(),
+                                                       _dev_ptr(jobs_t), n_jobs, _host_ptr(groups), len(groups), int(fmt), _dev_ptr(out_t),
+                                                       out_t.numel() * out_t.element_size(), _dev_ptr(results_t), _dev_ptr(status_t)))
 
     # -- output stage -------------------------------------------------------------------------
     def pcm_pack_host(self, pcm, spans, channels, fmt, out_frames, plane_stride=0, frames=0, n_spans=None, out=None):
