@@ -1080,7 +1080,8 @@ symgpu_status symgpu_flac_index(const uint8_t* data, size_t n, symgpu_flac_strea
  * stream order, as [frames][channels] into the file's region of `out` (channels a frame does not carry are 0).
  *   jobs    one per packet; the jobs of one group are consecutive in the table, in stream order
  *   groups  one per file
- *   out     int32 [out_cap]: file g's output starts at groups[g].out_offset and holds group_frames[g] * channels samples
+ *   out     [out_cap] samples, int32 unless a format is given: file g's output starts at sample groups[g].out_offset and holds
+ *           group_frames[g] * channels samples
  *   group_frames[g]  frames written for group g;  status[j]  one SYMGPU_FLAC_JOB_* per job
  * A packet is refused in exactly the cases where symgpu_flac_fe_decode_packets refuses it with the group's stream facts.
  * Nothing outside [offset, offset + len) of a job is read and nothing outside the file's region of `out` is written. */
@@ -1093,7 +1094,7 @@ typedef struct symgpu_flac_job {    /* 24 bytes */
     uint32_t reserved;
 } symgpu_flac_job;
 typedef struct symgpu_flac_group {  /* 16 bytes */
-    uint64_t out_offset;            /* first int32 of the file's [frames][channels] output in `out`                              */
+    uint64_t out_offset;            /* first sample of the file's [frames][channels] output in `out`                             */
     uint32_t max_block;             /* STREAMINFO block_max (0 = unknown)                                                        */
     uint8_t bits_per_sample;        /* STREAMINFO (0 = unknown: a frame without its own is refused)                               */
     uint8_t channels;               /* STREAMINFO channels, 1..8: the output's columns; a frame with more is refused             */
@@ -1120,6 +1121,20 @@ symgpu_status symgpu_flac_decode_host(symgpu_ctx* ctx, const uint8_t* bytes, siz
 symgpu_status symgpu_flac_decode_dev(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_flac_job* jobs, size_t n_jobs,
                                      const symgpu_flac_group* groups, size_t n_groups, int32_t* out, size_t out_cap, uint64_t* group_frames,
                                      uint8_t* status);
+/* The same two calls with the output stage in the caller's sample format: `out` holds out_cap samples of `format`
+ * (SYMGPU_FMT_*; symgpu_sample_bytes(format) bytes each), out_cap and out_offset stay in samples, and the interleaving kernel
+ * writes the reference's FromSample<i32> (symphonia-core/src/audio/conv.rs:516-531) of the 32-bit-scaled sample s, all exact:
+ *   SYMGPU_FMT_S32  s                                        SYMGPU_FMT_S24  s >> 8, in an int32 as the f32 output stage stores s24
+ *   SYMGPU_FMT_S16  (s >> 16) as i16                         SYMGPU_FMT_U8   ((s as u32).wrapping_add(0x8000_0000) >> 24) as u8
+ *   SYMGPU_FMT_F32  (s as f64 / 2147483648.0) as f32
+ * An unknown format is SYMGPU_ERR_ARG before anything is launched.  symgpu_flac_decode_host / _dev are these calls with
+ * SYMGPU_FMT_S32. */
+symgpu_status symgpu_flac_decode_fmt_host(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_flac_job* jobs, size_t n_jobs,
+                                          const symgpu_flac_group* groups, size_t n_groups, int format, void* out, size_t out_cap,
+                                          uint64_t* group_frames, uint8_t* status);
+symgpu_status symgpu_flac_decode_fmt_dev(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_flac_job* jobs, size_t n_jobs,
+                                         const symgpu_flac_group* groups, size_t n_groups, int format, void* out, size_t out_cap,
+                                         uint64_t* group_frames, uint8_t* status);
 
 /* ===================================================================================================
  * Vorbis entropy front-end (SURVEY 8f N1): audio packets -> the batch format of symgpu_vorbis_synth_* (unit, floor-1 Y

@@ -291,6 +291,10 @@ def lib():
         fn = getattr(L, name)
         fn.restype = ctypes.c_int
         fn.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, sz, vp, vp]
+    for name in ("symgpu_flac_decode_fmt_host", "symgpu_flac_decode_fmt_dev"):
+        fn = getattr(L, name)
+        fn.restype = ctypes.c_int
+        fn.argtypes = [vp, vp, sz, vp, sz, vp, sz, ctypes.c_int, vp, sz, vp, vp]
     for name in ("symgpu_mpa12_decode_host", "symgpu_mpa12_decode_dev"):
         fn = getattr(L, name)
         fn.restype = ctypes.c_int

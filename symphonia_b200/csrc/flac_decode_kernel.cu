@@ -6,7 +6,8 @@
 //                            runs, writes the frame record, its sub-frame records and the warm-up samples / residuals
 //   flac_launch              prediction + decorrelation + scaling (flac_kernel.cu, unchanged) over all jobs' records
 //   scan by group            accepted block sizes -> each frame's first output frame within its file
-//   flac_interleave_kernel   one CTA per packet: the restored planes -> [frames][channels] int32 in the file's region
+//   flac_interleave_kernel   one CTA per packet: the restored planes -> [frames][channels] of the caller's sample format in
+//                            the file's region (one instantiation per SYMGPU_FMT_*, chosen once on the host)
 //
 // A refused packet keeps neutral records: a frame with 0 channels (flac_finish_kernel returns at once) and sub-frames
 // with n = 0 (flac_predict_kernel leaves them alone), so the restoration kernels run on every job unchanged.
@@ -16,6 +17,7 @@
 #include <cuda_runtime.h>
 
 #include <cub/device/device_scan.cuh>
+#include <type_traits>
 #include <vector>
 
 #include "batch_call.h"
@@ -84,12 +86,44 @@ __global__ void __launch_bounds__(128) flac_decode_kernel(const uint8_t* __restr
     status[k] = st;
 }
 
+// The reference's FromSample<i32> (symphonia-core/src/audio/conv.rs:516-531) applied to the decoder's 32-bit-scaled sample: what
+// copy_to_slice_interleaved::<S> makes of the FLAC decoder's AudioBuffer<i32>.  Every conversion is exact; f32 is the double
+// quotient rounded once.
+template <int Format>
+struct FlacSample;
+template <>
+struct FlacSample<SYMGPU_FMT_S32> {
+    using type = int32_t;
+    static __device__ __forceinline__ type from(int32_t s) { return s; }
+};
+template <>
+struct FlacSample<SYMGPU_FMT_S24> {
+    using type = int32_t;  // an s24 sample in an int32, as the f32 output stage stores it
+    static __device__ __forceinline__ type from(int32_t s) { return s >> 8; }
+};
+template <>
+struct FlacSample<SYMGPU_FMT_S16> {
+    using type = int16_t;
+    static __device__ __forceinline__ type from(int32_t s) { return int16_t(s >> 16); }
+};
+template <>
+struct FlacSample<SYMGPU_FMT_U8> {
+    using type = uint8_t;
+    static __device__ __forceinline__ type from(int32_t s) { return uint8_t((uint32_t(s) + 0x80000000u) >> 24); }
+};
+template <>
+struct FlacSample<SYMGPU_FMT_F32> {
+    using type = float;
+    static __device__ __forceinline__ type from(int32_t s) { return __double2float_rn(double(s) / 2147483648.0); }
+};
+
+template <int Format>
 __global__ void __launch_bounds__(256) flac_interleave_kernel(const symgpu_flac_job* __restrict__ jobs, uint32_t n_jobs, const symgpu_flac_group* __restrict__ groups,
                                                               size_t n_groups, const symgpu_flac_frame* __restrict__ frames,
                                                               const symgpu_flac_subframe* __restrict__ subs, const int32_t* __restrict__ samples,
                                                               const uint8_t* __restrict__ status, const unsigned long long* __restrict__ accepted,
-                                                              const unsigned long long* __restrict__ first, int32_t* __restrict__ out, unsigned long long out_cap,
-                                                              uint64_t* __restrict__ group_frames) {
+                                                              const unsigned long long* __restrict__ first, typename FlacSample<Format>::type* __restrict__ out,
+                                                              unsigned long long out_cap, uint64_t* __restrict__ group_frames) {
     __shared__ unsigned long long plane_s[8];
     const uint32_t k = blockIdx.x;
     const uint32_t gi = jobs[k].group;
@@ -104,10 +138,11 @@ __global__ void __launch_bounds__(256) flac_interleave_kernel(const symgpu_flac_
     if (g.out_offset > out_cap || at > out_cap || count > out_cap - at) return;
     if (threadIdx.x < have) plane_s[threadIdx.x] = subs[fr.first_subframe + threadIdx.x].offset;
     __syncthreads();
-    for (unsigned long long i = threadIdx.x; i < count; i += blockDim.x) {
-        const unsigned long long t = i / ch;
-        const unsigned c = unsigned(i - t * ch);
-        out[at + i] = c < have ? samples[plane_s[c] + t] : 0;
+    // a block has at most 65 536 samples in at most 8 channels: the element index and its divide fit 32 bits
+    for (uint32_t i = threadIdx.x; i < uint32_t(count); i += blockDim.x) {
+        const uint32_t t = i / ch;
+        const unsigned c = i - t * ch;
+        out[at + i] = FlacSample<Format>::from(c < have ? samples[plane_s[c] + t] : 0);
     }
 }
 
@@ -147,9 +182,10 @@ cudaError_t scratch_layout(uint32_t n_jobs, size_t out_cap, Scratch& s) {
     return cudaSuccess;
 }
 
-// Everything after the staging: device pointers, n_jobs > 0, ctx->d_stage holds `s`.
+// Everything after the staging: device pointers, n_jobs > 0, a format symgpu_sample_bytes knows, ctx->d_stage holds `s`.
 symgpu_status decode_on_device(symgpu_ctx* ctx, const Scratch& s, const uint8_t* bytes, size_t n_bytes, const symgpu_flac_job* jobs, uint32_t n_jobs,
-                               const symgpu_flac_group* groups, size_t n_groups, int32_t* out, size_t out_cap, uint64_t* group_frames, uint8_t* status) {
+                               const symgpu_flac_group* groups, size_t n_groups, int format, void* out, size_t out_cap, uint64_t* group_frames,
+                               uint8_t* status) {
     char* stage = static_cast<char*>(ctx->d_stage);
     Slot* sizes = reinterpret_cast<Slot*>(stage + s.sizes);
     Slot* base = reinterpret_cast<Slot*>(stage + s.base);
@@ -172,7 +208,18 @@ symgpu_status decode_on_device(symgpu_ctx* ctx, const Scratch& s, const uint8_t*
     CU(ctx, symgpu::flac_launch(frames, n_jobs, subs, n_jobs * 8, samples, out_cap, st));
     temp_bytes = s.temp_bytes;
     CU(ctx, scan_first(temp, temp_bytes, keys, accepted, first, n_jobs, st));
-    flac_interleave_kernel<<<n_jobs, 256, 0, st>>>(jobs, n_jobs, groups, n_groups, frames, subs, samples, status, accepted, first, out, out_cap, group_frames);
+    auto interleave = [&](auto fmt) {
+        constexpr int F = decltype(fmt)::value;
+        flac_interleave_kernel<F><<<n_jobs, 256, 0, st>>>(jobs, n_jobs, groups, n_groups, frames, subs, samples, status, accepted, first,
+                                                          static_cast<typename FlacSample<F>::type*>(out), out_cap, group_frames);
+    };
+    switch (format) {
+    case SYMGPU_FMT_F32: interleave(std::integral_constant<int, SYMGPU_FMT_F32>{}); break;
+    case SYMGPU_FMT_S16: interleave(std::integral_constant<int, SYMGPU_FMT_S16>{}); break;
+    case SYMGPU_FMT_S24: interleave(std::integral_constant<int, SYMGPU_FMT_S24>{}); break;
+    case SYMGPU_FMT_S32: interleave(std::integral_constant<int, SYMGPU_FMT_S32>{}); break;
+    default: interleave(std::integral_constant<int, SYMGPU_FMT_U8>{}); break;
+    }
     CU(ctx, cudaGetLastError());
     ctx->launches += 9;  // three kernels here, predict + finish, and two per device-wide scan
     return SYMGPU_OK;
@@ -182,9 +229,10 @@ constexpr size_t kMaxJobs = 0x1fffffff;  // eight sub-frame records per job are 
 
 }  // namespace
 
-extern "C" symgpu_status symgpu_flac_decode_dev(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_flac_job* jobs, size_t n_jobs,
-                                                const symgpu_flac_group* groups, size_t n_groups, int32_t* out, size_t out_cap, uint64_t* group_frames,
-                                                uint8_t* status) {
+extern "C" symgpu_status symgpu_flac_decode_fmt_dev(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_flac_job* jobs, size_t n_jobs,
+                                                    const symgpu_flac_group* groups, size_t n_groups, int format, void* out, size_t out_cap,
+                                                    uint64_t* group_frames, uint8_t* status) {
+    if (symgpu_sample_bytes(format) == 0) return SYMGPU_ERR_ARG;
     if (bad_batch_args(ctx, bytes, n_bytes, jobs, n_jobs, groups, n_groups, out, out_cap, group_frames, status, kMaxJobs)) return SYMGPU_ERR_ARG;
     DeviceGuard guard(ctx->device);
     if (n_groups) CU(ctx, cudaMemsetAsync(group_frames, 0, n_groups * sizeof(uint64_t), ctx->stream));
@@ -193,12 +241,20 @@ extern "C" symgpu_status symgpu_flac_decode_dev(symgpu_ctx* ctx, const uint8_t* 
     CU(ctx, scratch_layout(uint32_t(n_jobs), out_cap, s));
     const symgpu_status e = ensure_stage(ctx, s.total);
     if (e != SYMGPU_OK) return e;
-    return decode_on_device(ctx, s, bytes, n_bytes, jobs, uint32_t(n_jobs), groups, n_groups, out, out_cap, group_frames, status);
+    return decode_on_device(ctx, s, bytes, n_bytes, jobs, uint32_t(n_jobs), groups, n_groups, format, out, out_cap, group_frames, status);
 }
 
-extern "C" symgpu_status symgpu_flac_decode_host(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_flac_job* jobs, size_t n_jobs,
-                                                 const symgpu_flac_group* groups, size_t n_groups, int32_t* out, size_t out_cap, uint64_t* group_frames,
-                                                 uint8_t* status) {
+extern "C" symgpu_status symgpu_flac_decode_dev(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_flac_job* jobs, size_t n_jobs,
+                                                const symgpu_flac_group* groups, size_t n_groups, int32_t* out, size_t out_cap, uint64_t* group_frames,
+                                                uint8_t* status) {
+    return symgpu_flac_decode_fmt_dev(ctx, bytes, n_bytes, jobs, n_jobs, groups, n_groups, SYMGPU_FMT_S32, out, out_cap, group_frames, status);
+}
+
+extern "C" symgpu_status symgpu_flac_decode_fmt_host(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_flac_job* jobs, size_t n_jobs,
+                                                     const symgpu_flac_group* groups, size_t n_groups, int format, void* out, size_t out_cap,
+                                                     uint64_t* group_frames, uint8_t* status) {
+    const size_t sample = symgpu_sample_bytes(format);
+    if (sample == 0) return SYMGPU_ERR_ARG;
     if (bad_batch_args(ctx, bytes, n_bytes, jobs, n_jobs, groups, n_groups, out, out_cap, group_frames, status, kMaxJobs) ||
         !jobs_in_bytes(jobs, n_jobs, n_bytes))
         return SYMGPU_ERR_ARG;
@@ -228,18 +284,24 @@ extern "C" symgpu_status symgpu_flac_decode_host(symgpu_ctx* ctx, const uint8_t*
     return decode_from_host(
         ctx, s.total,
         std::array<HostIn, 3>{{{bytes, n_bytes}, {jobs, n_jobs * sizeof(symgpu_flac_job)}, {groups, n_groups * sizeof(symgpu_flac_group)}}}, out,
-        out_cap * sizeof(int32_t), std::array<HostOut, 2>{{{status, n_jobs}, {group_frames, n_groups * sizeof(uint64_t)}}},
+        out_cap * sample, std::array<HostOut, 2>{{{status, n_jobs}, {group_frames, n_groups * sizeof(uint64_t)}}},
         [&](const std::array<void*, 3>& in, void* d_out, const std::array<void*, 2>& back) {
             uint64_t* d_frames = static_cast<uint64_t*>(back[1]);
             if (n_groups) CU(ctx, cudaMemsetAsync(d_frames, 0, n_groups * sizeof(uint64_t), ctx->stream));
             return decode_on_device(ctx, s, static_cast<const uint8_t*>(in[0]), n_bytes, static_cast<const symgpu_flac_job*>(in[1]), uint32_t(n_jobs),
-                                    static_cast<const symgpu_flac_group*>(in[2]), n_groups, static_cast<int32_t*>(d_out), out_cap, d_frames,
+                                    static_cast<const symgpu_flac_group*>(in[2]), n_groups, format, d_out, out_cap, d_frames,
                                     static_cast<uint8_t*>(back[0]));
         },
         [&] {
             std::vector<ByteRange> w;
             for (size_t g = 0; g < n_groups; ++g)
-                w.push_back({size_t(groups[g].out_offset) * sizeof(int32_t), size_t(groups[g].out_offset + group_frames[g] * groups[g].channels) * sizeof(int32_t)});
+                w.push_back({size_t(groups[g].out_offset) * sample, size_t(groups[g].out_offset + group_frames[g] * groups[g].channels) * sample});
             return w;
         });
+}
+
+extern "C" symgpu_status symgpu_flac_decode_host(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_flac_job* jobs, size_t n_jobs,
+                                                 const symgpu_flac_group* groups, size_t n_groups, int32_t* out, size_t out_cap, uint64_t* group_frames,
+                                                 uint8_t* status) {
+    return symgpu_flac_decode_fmt_host(ctx, bytes, n_bytes, jobs, n_jobs, groups, n_groups, SYMGPU_FMT_S32, out, out_cap, group_frames, status);
 }

@@ -390,7 +390,7 @@ def decode_files(engine, files, fmt=nat.FMT_S16, threads=None):
     return pack_files(plans, batches, pcm, engine.pcm_pack_host, fmt)
 
 
-# ---- FLAC (integer path: restoration on the GPU, samples stay int32 as in the reference's AudioBuffer<i32>) ----------------------
+# ---- FLAC (integer path: restoration on the GPU, samples int32 as in the reference's AudioBuffer<i32> until the output stage) -----
 
 def flac_plan(data):
     """CPU half for a native FLAC file: marker + STREAMINFO + checksum-validated frame split (symgpu_flac_index), frame / sub-frame / Rice
@@ -419,13 +419,32 @@ def flac_interleave(plan, restored):
     return out
 
 
-def decode_flac(engine, data):
-    """(samples [frames, channels] int32 scaled to 32 bits as the reference's FLAC decoder leaves them, sample_rate)."""
+def flac_convert(samples, fmt):
+    """The decoder's int32 samples (scaled to 32 bits) as `fmt`, as the reference's FromSample<i32> converts them
+    (symphonia-core/src/audio/conv.rs:516-531) -- every case exact:  s32: s;  s24: s >> 8 (in an int32, as the f32 output stage
+    stores s24);  s16: (s >> 16) as i16;  u8: ((s as u32).wrapping_add(0x8000_0000) >> 24) as u8;  f32: (s as f64 / 2^31) as f32."""
+    s = np.asarray(samples, dtype=np.int32)
+    if fmt == nat.FMT_S32:
+        return s
+    if fmt == nat.FMT_S24:
+        return s >> 8
+    if fmt == nat.FMT_S16:
+        return (s >> 16).astype(np.int16)
+    if fmt == nat.FMT_U8:
+        return ((s.view(np.uint32) + np.uint32(0x80000000)) >> np.uint32(24)).astype(np.uint8)
+    if fmt == nat.FMT_F32:
+        return (s.astype(np.float64) / 2147483648.0).astype(np.float32)
+    raise ValueError(f"unknown sample format {fmt}")
+
+
+def decode_flac(engine, data, fmt=nat.FMT_S32):
+    """(samples [frames, channels] of `fmt`, sample_rate): int32 scaled to 32 bits as the reference's FLAC decoder leaves them by
+    default, any other format by flac_convert."""
     plan = flac_plan(data)
     if len(plan["frames"]) == 0:
-        return np.zeros((0, plan["channels"]), dtype=np.int32), plan["sample_rate"]
+        return np.zeros((0, plan["channels"]), dtype=nat.FMT_NUMPY[fmt]), plan["sample_rate"]
     restored = engine.flac_restore_host(plan["frames"], plan["subframes"], plan["samples"].copy())
-    return flac_interleave(plan, restored), plan["sample_rate"]
+    return flac_convert(flac_interleave(plan, restored), fmt), plan["sample_rate"]
 
 
 # ---- many files per device call: the steps every codec's files path shares ---------------------------------------------------
@@ -542,19 +561,20 @@ def flac_files_plan(files, threads=None, errors=None):
     return dict(data=data, jobs=jobs, groups=groups, rates=rates, out_cap=cap, failed=failed)
 
 
-def decode_flac_files(engine, files, threads=None, device=False, errors=None):
-    """[(samples [frames, channels] int32, sample_rate)] for a list of native FLAC files, each equal to decode_flac(engine, file):
-    the files are indexed on host threads, and ONE device call decodes every packet of every file -- frame headers and Rice
-    residuals in device code (one thread per packet), restoration and interleaving on the GPU.  device=True: the bytes go to the
-    device once and the samples are int32 CUDA tensors, views of one output tensor.  A file that cannot be indexed yields an empty
-    result with sample rate 0 (its message in errors[i] when `errors` is a dict)."""
+def decode_flac_files(engine, files, threads=None, device=False, errors=None, fmt=nat.FMT_S32):
+    """[(samples [frames, channels] of `fmt`, sample_rate)] for a list of native FLAC files, each equal to decode_flac(engine, file,
+    fmt): the files are indexed on host threads, and ONE device call decodes every packet of every file -- frame headers and Rice
+    residuals in device code (one thread per packet), restoration, and interleaving with the conversion to `fmt` (int32 scaled to
+    32 bits by default) on the GPU.  device=True: the bytes go to the device once and the samples are CUDA tensors, views of one
+    output tensor.  A file that cannot be indexed yields an empty result with sample rate 0 (its message in errors[i] when
+    `errors` is a dict)."""
     plan = flac_files_plan(files, threads, errors)
     groups, rates, cap = plan["groups"], plan["rates"], plan["out_cap"]
     def dev(data_t, jobs_t, groups_t, out_t, frames_t, status_t):
         import torch
-        engine.flac_decode_dev(data_t, jobs_t, groups_t, out_t, frames_t.view(torch.int64), status_t)
-    out, group_frames, _, _ = _decode_batch(engine, device, (plan["data"], plan["jobs"], groups), cap, "int32", len(groups), np.dtype(np.int64),
-                                            lambda: (*engine.flac_decode_host(plan["data"], plan["jobs"], groups, cap), None), dev)
+        engine.flac_decode_dev(data_t, jobs_t, groups_t, out_t, frames_t.view(torch.int64), status_t, fmt)
+    out, group_frames, _, _ = _decode_batch(engine, device, (plan["data"], plan["jobs"], groups), cap, _TORCH_DTYPES[fmt], len(groups), np.dtype(np.int64),
+                                            lambda: (*engine.flac_decode_host(plan["data"], plan["jobs"], groups, cap, fmt=fmt), None), dev)
     return _per_file(out, groups, plan["failed"], lambda g: (int(group_frames[g]), int(groups[g]["channels"]), int(rates[g])))
 
 
@@ -727,19 +747,20 @@ def decode_aac_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False,
                      lambda g: (int(results[g]["frames"]), int(groups[g]["channels"]), int(groups[g]["sample_rate"])))
 
 
-def decode_mpeg_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False, errors=None):
+def decode_mpeg_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False, errors=None, stats=None):
     """[(samples [frames, channels] of `fmt`, sample_rate)] for a list of MPEG audio files of any layer, each what
     decode_mpeg_audio(engine, file, fmt) returns: every file is indexed once, Layer III files go to decode_mp3_files and Layer I / II
     files to decode_mpa12_files (one device call each).  A file that cannot be indexed yields an empty result with sample rate 0 (its
-    message in errors[i] when `errors` is a dict)."""
+    message in errors[i] when `errors` is a dict).  stats: a dict that receives what decode_mp3_files' `stats` does, when there is a
+    Layer III file."""
     ix, messages = mpa_index_files(files, threads)
     if errors is not None:
         errors.update(messages)
     result = [None] * len(files)
-    for layers, decode in (((3,), decode_mp3_files), ((1, 2), decode_mpa12_files)):
+    for layers, decode, more in (((3,), decode_mp3_files, dict(stats=stats)), ((1, 2), decode_mpa12_files, {})):
         mine = [i for i, t in enumerate(ix) if t is not None and int(t[0]["layer"]) in layers]
         if mine:
-            got = decode(engine, [files[i] for i in mine], fmt, threads, device, None, ([ix[i] for i in mine], {}))
+            got = decode(engine, [files[i] for i in mine], fmt, threads, device, None, ([ix[i] for i in mine], {}), **more)
             for i, r in zip(mine, got):
                 result[i] = r
     for i in messages:
@@ -818,3 +839,40 @@ def decode_vorbis_files(engine, files, fmt=nat.FMT_S16, threads=None, device=Fal
         stats.update(status=status, n_setups=len(setups))
     return _per_file(out, groups, plan["failed"],
                      lambda g: (int(results[g]["frames"]), int(results[g]["channels"]), int(results[g]["sample_rate"])))
+
+
+# ---- a mixed list: every file to the device decoder of its kind ----------------------------------------------------------------
+
+def decode_any_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False, errors=None, stats=None):
+    """[(samples [frames, channels] of `fmt`, sample_rate)], one per file in input order, for a list of native FLAC, ADTS AAC-LC,
+    Ogg Vorbis and MPEG audio (Layers I-III) files in any mix: every file is sniffed, and the files of each kind go, at most once
+    per kind, to decode_flac_files, decode_aac_files, decode_vorbis_files and decode_mpeg_files; a kind without a file makes no
+    call.  Every result is what that decoder returns for the file alone with the same `fmt` and `device`.  device=True: the
+    samples are CUDA tensors, views of their kind's output tensor.  A file its decoder cannot index or open yields an empty [0, 0]
+    result with sample rate 0, and its message goes to errors[i], i its place in `files`, when `errors` is a dict.  stats: a dict
+    that receives `calls`, the kinds that ran ('flac', 'aac', 'vorbis', 'mpa'), and under each such kind a dict of what that
+    decoder's `stats` gives (`status`, `n_redecoded`, `n_setups`, `rounds`).  The decoders' limits hold per kind: more than
+    65 536 AAC or Vorbis files is their ValueError.  As those decoders do, the call (re)allocates the engine's MP3 and AAC state
+    slots and replaces its Vorbis stream and floor registration: streaming decoders on the same engine lose their state."""
+    decoders = (("flac", lambda fs, e, st: decode_flac_files(engine, fs, threads, device, e, fmt)),
+                ("aac", lambda fs, e, st: decode_aac_files(engine, fs, fmt, threads, device, e, st)),
+                ("vorbis", lambda fs, e, st: decode_vorbis_files(engine, fs, fmt, threads, device, e, st)),
+                ("mpa", lambda fs, e, st: decode_mpeg_files(engine, fs, fmt, threads, device, e, st)))
+    kinds = [sniff(f) for f in files]
+    result, calls = [None] * len(files), []
+    for kind, decode in decoders:
+        mine = [i for i, k in enumerate(kinds) if k == kind]
+        if not mine:
+            continue
+        messages, kind_stats = {}, {}
+        got = decode([files[i] for i in mine], messages, kind_stats)
+        for i, r in zip(mine, got):
+            result[i] = r
+        if errors is not None:
+            errors.update({mine[k]: m for k, m in messages.items()})
+        calls.append(kind)
+        if stats is not None:
+            stats[kind] = kind_stats
+    if stats is not None:
+        stats["calls"] = calls
+    return result

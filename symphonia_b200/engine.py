@@ -221,35 +221,38 @@ class Engine:
                                                       ctypes.c_void_p(subframes_t.data_ptr()), n_subframes,
                                                       ctypes.c_void_p(samples_t.data_ptr()), samples_t.numel()))
 
-    def flac_decode_host(self, data, jobs, groups, out_cap, out=None):
+    def flac_decode_host(self, data, jobs, groups, out_cap, out=None, fmt=_native.FMT_S32):
         """Device FLAC decoding of many files in one call: `data` (bytes / uint8 array) holds the packets, jobs FLAC_JOB_DTYPE
-        (one per packet, a group's jobs consecutive in stream order), groups FLAC_GROUP_DTYPE (one per file).  Returns (out int32
-        [out_cap], group_frames uint64 [groups], status uint8 [jobs]); file g's PCM is out[out_offset:][:group_frames[g] * channels]
-        as [frames, channels]."""
+        (one per packet, a group's jobs consecutive in stream order), groups FLAC_GROUP_DTYPE (one per file).  Returns (out
+        [out_cap] of `fmt`: int32 scaled to 32 bits by default, group_frames uint64 [groups], status uint8 [jobs]); file g's PCM is
+        out[out_offset:][:group_frames[g] * channels] as [frames, channels].  A format the library does not know is its to
+        refuse (give `out` then)."""
         from ._native import FLAC_GROUP_DTYPE, FLAC_JOB_DTYPE
         a = _byte_view(data)
         jobs = np.ascontiguousarray(jobs, dtype=FLAC_JOB_DTYPE)
         groups = np.ascontiguousarray(groups, dtype=FLAC_GROUP_DTYPE)
         if out is None:
-            out = np.zeros(int(out_cap), dtype=np.int32)
-        assert out.dtype == np.int32 and out.flags.c_contiguous and out.size >= out_cap
+            out = np.zeros(int(out_cap), dtype=FMT_NUMPY[fmt])
+        assert out.flags.c_contiguous and out.size >= out_cap and (fmt not in FMT_NUMPY or out.dtype == FMT_NUMPY[fmt])
         group_frames = np.zeros(len(groups), dtype=np.uint64)
         status = np.zeros(len(jobs), dtype=np.uint8)
-        self._check(self._lib.symgpu_flac_decode_host(self._ctx, _host_ptr(a), a.size, _host_ptr(jobs), len(jobs), _host_ptr(groups), len(groups),
-                                                      _host_ptr(out), int(out_cap), _host_ptr(group_frames), _host_ptr(status)))
+        self._check(self._lib.symgpu_flac_decode_fmt_host(self._ctx, _host_ptr(a), a.size, _host_ptr(jobs), len(jobs), _host_ptr(groups), len(groups),
+                                                          int(fmt), _host_ptr(out), int(out_cap), _host_ptr(group_frames), _host_ptr(status)))
         return out, group_frames, status
 
-    def flac_decode_dev(self, data_t, jobs_t, groups_t, out_t, group_frames_t, status_t):
-        """Device-resident variant: torch CUDA tensors (uint8 bytes, jobs / groups as uint8 views of the records, int32 out, int64
-        group_frames, uint8 status); asynchronous on the engine's stream."""
+    def flac_decode_dev(self, data_t, jobs_t, groups_t, out_t, group_frames_t, status_t, fmt=_native.FMT_S32):
+        """Device-resident variant: torch CUDA tensors (uint8 bytes, jobs / groups as uint8 views of the records, out of `fmt`'s
+        element type: int32 by default, int64 group_frames, uint8 status); asynchronous on the engine's stream."""
         from ._native import FLAC_GROUP_DTYPE, FLAC_JOB_DTYPE
         ts = (data_t, jobs_t, groups_t, out_t, group_frames_t, status_t)
         assert all(t.is_cuda and t.is_contiguous() for t in ts)
+        assert fmt not in FMT_NUMPY or out_t.element_size() == np.dtype(FMT_NUMPY[fmt]).itemsize
         n_jobs = jobs_t.numel() * jobs_t.element_size() // FLAC_JOB_DTYPE.itemsize
         n_groups = groups_t.numel() * groups_t.element_size() // FLAC_GROUP_DTYPE.itemsize
         assert group_frames_t.numel() >= n_groups and group_frames_t.element_size() == 8 and status_t.numel() >= n_jobs
-        self._check(self._lib.symgpu_flac_decode_dev(self._ctx, _dev_ptr(data_t), data_t.numel(), _dev_ptr(jobs_t), n_jobs, _dev_ptr(groups_t), n_groups,
-                                                     _dev_ptr(out_t), out_t.numel(), _dev_ptr(group_frames_t), _dev_ptr(status_t)))
+        self._check(self._lib.symgpu_flac_decode_fmt_dev(self._ctx, _dev_ptr(data_t), data_t.numel(), _dev_ptr(jobs_t), n_jobs, _dev_ptr(groups_t),
+                                                         n_groups, int(fmt), _dev_ptr(out_t), out_t.numel(), _dev_ptr(group_frames_t),
+                                                         _dev_ptr(status_t)))
 
     # -- MPEG Layer I / II decoded on the device ----------------------------------------------------------
     def mpa12_decode_host(self, data, jobs, groups, fmt, out_samples, out=None):
