@@ -947,6 +947,42 @@ symgpu_status symgpu_vorbis_decode_dev(symgpu_ctx* ctx, const uint8_t* headers, 
                                        symgpu_vorbis_group_result* results, uint8_t* status);
 
 /* ===================================================================================================
+ * Ogg pages indexed on the device (DESIGN 5b): many files already in device memory, one call.  The page search, the page
+ * checks (CRC-32 included) and the logical-stream rules are those of symgpu_ogg_index, as the same host / device code.
+ * ================================================================================================= */
+#define SYMGPU_OGG_MAX_FILES 65536
+typedef struct symgpu_file_range {      /* 16 bytes: one file's bytes in a buffer                                      */
+    uint64_t offset;
+    uint64_t len;
+} symgpu_file_range;
+typedef struct symgpu_ogg_file_index {  /* 40 bytes: one file's share of the tables                                     */
+    uint64_t first_packet;   /* its packets start here in `packets` (the n_packets of the files before it, summed)       */
+    uint64_t first_piece;    /* likewise in `pieces`                                                                    */
+    uint64_t packet_bytes;   /* the lengths of its packets, summed                                                      */
+    uint32_t n_packets;
+    uint32_t n_pieces;
+    uint32_t max_packet_len; /* its longest packet                                                                      */
+    uint8_t status;          /* bit 0 (SYMGPU_OGG_CAP_HIT): an open packet passed the 16 MiB cap, what symgpu_ogg_index
+                                reports as SYMGPU_ERR_DECODE; bit 1 (SYMGPU_OGG_NOT_WRITTEN): first + n passes a capacity,
+                                so none of the file's records were written                                             */
+    uint8_t reserved[3];
+} symgpu_ogg_file_index;
+enum { SYMGPU_OGG_CAP_HIT = 1, SYMGPU_OGG_NOT_WRITTEN = 2 };
+/* For every file data[files[i].offset ..][.. len), what symgpu_ogg_index returns for those bytes alone: its packets at
+ * packets[index[i].first_packet ..] and its pieces at pieces[index[i].first_piece ..], with piece offsets relative to the
+ * file's first byte and first_piece relative to the file's first piece, so each file's tables equal the host call's.  data,
+ * packets, pieces and index are device memory; files host memory.  SYMGPU_ERR_ARG for a range outside data[0 .. n_bytes) or a
+ * missing pointer, SYMGPU_ERR_LIMIT for more than SYMGPU_OGG_MAX_FILES files or a file of 2^32 bytes or more; both before
+ * anything is launched.  The sizes are found on the device: a caller who does not know them calls with zero capacities,
+ * reads index[] back (every total is first + n of the last file) and calls again.  Five launches whatever the number of files,
+ * no host wait; the call returns with them queued.  Each file is walked by one thread in time linear in its bytes and pages,
+ * however many logical streams it holds.  Scratch from the context's staging buffer: 16 bytes per 4 file bytes and 28 per
+ * file. */
+symgpu_status symgpu_ogg_index_dev(symgpu_ctx* ctx, const uint8_t* data, size_t n_bytes, const symgpu_file_range* files, size_t n_files,
+                                   symgpu_ogg_packet* packets, size_t cap_packets, symgpu_piece* pieces, size_t cap_pieces,
+                                   symgpu_ogg_file_index* index);
+
+/* ===================================================================================================
  * MPEG Layer I / II sample decoders (SURVEY 8f N1 for the Layer I / II path): a packet becomes the sub-band samples
  * symgpu_mpa12_synth_* take.  CPU only, stateless apart from the stream's signal specification.
  *   Layer1::decode up to the synthesis call   symphonia-bundle-mp3/src/layer1/mod.rs:19-176

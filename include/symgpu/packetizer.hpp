@@ -48,8 +48,8 @@ namespace detail {
 SYMGPU_PACKET_HD inline uint32_t be32(const uint8_t* p) { return uint32_t(p[0]) << 24 | uint32_t(p[1]) << 16 | uint32_t(p[2]) << 8 | p[3]; }
 inline uint32_t be24(const uint8_t* p) { return uint32_t(p[0]) << 16 | uint32_t(p[1]) << 8 | p[2]; }
 inline uint32_t be16(const uint8_t* p) { return uint32_t(p[0]) << 8 | p[1]; }
-inline uint32_t le32(const uint8_t* p) { return uint32_t(p[3]) << 24 | uint32_t(p[2]) << 16 | uint32_t(p[1]) << 8 | p[0]; }
-inline uint64_t le64(const uint8_t* p) { return uint64_t(le32(p + 4)) << 32 | le32(p); }
+SYMGPU_PACKET_HD inline uint32_t le32(const uint8_t* p) { return uint32_t(p[3]) << 24 | uint32_t(p[2]) << 16 | uint32_t(p[1]) << 8 | p[0]; }
+SYMGPU_PACKET_HD inline uint64_t le64(const uint8_t* p) { return uint64_t(le32(p + 4)) << 32 | le32(p); }
 
 struct Crc32Table {  // slicing-by-8: t[k][b] = contribution of byte b seen k bytes before the end of an 8-byte block
     uint32_t t[8][256];
@@ -77,15 +77,19 @@ struct Crc16Table {
 
 // CRC-32, polynomial 0x04c11db7, most-significant bit first, no final xor; the caller supplies the initial state
 // (Ogg pages: 0).  symphonia-core/src/checksum/crc32.rs:543-570.
-inline uint32_t crc32_update(uint32_t state, const uint8_t* p, size_t n) {
-    static constexpr detail::Crc32Table tab{};
+// `t` is a slicing-by-8 table (detail::Crc32Table::t): the device keeps its copy in shared memory.
+SYMGPU_PACKET_HD inline uint32_t crc32_update_with(const uint32_t (*t)[256], uint32_t state, const uint8_t* p, size_t n) {
     for (; n >= 8; p += 8, n -= 8) {
         const uint32_t hi = state ^ detail::be32(p), lo = detail::be32(p + 4);
-        state = tab.t[7][hi >> 24] ^ tab.t[6][(hi >> 16) & 0xff] ^ tab.t[5][(hi >> 8) & 0xff] ^ tab.t[4][hi & 0xff] ^
-                tab.t[3][lo >> 24] ^ tab.t[2][(lo >> 16) & 0xff] ^ tab.t[1][(lo >> 8) & 0xff] ^ tab.t[0][lo & 0xff];
+        state = t[7][hi >> 24] ^ t[6][(hi >> 16) & 0xff] ^ t[5][(hi >> 8) & 0xff] ^ t[4][hi & 0xff] ^
+                t[3][lo >> 24] ^ t[2][(lo >> 16) & 0xff] ^ t[1][(lo >> 8) & 0xff] ^ t[0][lo & 0xff];
     }
-    for (size_t i = 0; i < n; ++i) state = (state << 8) ^ tab.t[0][(state >> 24) ^ p[i]];
+    for (size_t i = 0; i < n; ++i) state = (state << 8) ^ t[0][(state >> 24) ^ p[i]];
     return state;
+}
+inline uint32_t crc32_update(uint32_t state, const uint8_t* p, size_t n) {
+    static constexpr detail::Crc32Table tab{};
+    return crc32_update_with(tab.t, state, p, n);
 }
 
 // CRC-16, polynomial 0x8005, least-significant bit first, no final xor (the LAME tag's checksum).
@@ -579,6 +583,7 @@ struct OggPage {
     bool continuation, first, last;
     uint64_t body_offset;  // first body byte
     uint32_t body_len;
+    const uint8_t* lacing; // the n_segments lacing values, in the source buffer
     uint16_t n_packets;    // packets that END on this page
     uint16_t packet_len[255];
     uint32_t partial_len() const {  // body bytes after the last packet end: a packet continued on a later page
@@ -587,6 +592,52 @@ struct OggPage {
         return body_len - used;
     }
 };
+
+// The fields of a page header, read where a capture pattern was found.
+struct OggPageHead {
+    uint64_t offset;       // of the capture pattern
+    uint64_t absgp;        // granule position
+    uint64_t body_offset;  // first body byte
+    uint32_t serial, sequence, crc, body_len;
+    uint8_t n_segments;    // lacing values, at offset + kOggHeaderSize
+    bool continuation, first, last;
+};
+
+// The header fields of the page at q, its lacing values included (the caller knows they lie inside the buffer).
+SYMGPU_PACKET_HD inline void ogg_page_fields(const uint8_t* d, size_t q, OggPageHead& pg) {
+    const uint8_t* h = d + q;
+    pg.offset = q;
+    pg.continuation = h[5] & 1, pg.first = (h[5] & 2) != 0, pg.last = (h[5] & 4) != 0;
+    pg.absgp = detail::le64(h + 6);
+    pg.serial = detail::le32(h + 14), pg.sequence = detail::le32(h + 18), pg.crc = detail::le32(h + 22);
+    pg.n_segments = h[26];
+    uint32_t body = 0;
+    for (unsigned i = 0; i < pg.n_segments; ++i) body += h[kOggHeaderSize + i];
+    pg.body_offset = q + kOggHeaderSize + pg.n_segments, pg.body_len = body;
+}
+
+// One attempt of page.rs:166-271 at a capture pattern: d[0..n) is the file, "OggS" starts at q (q + 4 <= n).  Ok: a page
+// that verifies, *next = its end.  DecodeError: a bad version / flag byte (*next = q + 27, the search resumes after that
+// header) or a checksum mismatch (*next = q + 4, right after the capture pattern).  EndOfStream: the header, the lacing or the
+// body is cut by the end of the file, which ends the search.  Nothing outside d[0..n) is read.  `crc` is a slicing-by-8 table.
+SYMGPU_PACKET_HD inline Status ogg_check_page(const uint8_t* d, size_t n, size_t q, const uint32_t (*crc)[256], OggPageHead& pg, size_t* next) {
+    *next = n;
+    if (q + kOggHeaderSize > n) return Status::EndOfStream;
+    const uint8_t* h = d + q;
+    if (h[4] != 0 || (h[5] & 0xf8)) return *next = q + kOggHeaderSize, Status::DecodeError;
+    if (q + kOggHeaderSize + h[26] > n) return Status::EndOfStream;
+    ogg_page_fields(d, q, pg);
+    const uint32_t body = pg.body_len;
+    if (pg.body_offset + body > n) return Status::EndOfStream;
+    // checksum over the page with its own checksum field read as zero
+    const uint8_t zero[4] = {0, 0, 0, 0};
+    uint32_t c = crc32_update_with(crc, 0, h, 22);
+    c = crc32_update_with(crc, c, zero, 4);
+    c = crc32_update_with(crc, c, h + 26, 1 + size_t(pg.n_segments) + body);
+    if (c != pg.crc) return *next = q + 4, Status::DecodeError;
+    *next = pg.body_offset + body;
+    return Status::Ok;
+}
 
 // page.rs:166-271 over a resident buffer.
 class OggPageReader {
@@ -607,36 +658,20 @@ class OggPageReader {
             }
             if (std::memcmp(d_ + q, "OggS", 4) == 0) break;
         }
-        if (q + kOggHeaderSize > n_) return pos_ = n_, Status::EndOfStream;
-        const uint8_t* h = d_ + q;
-        pos_ = q + kOggHeaderSize;
-        if (h[4] != 0 || (h[5] & 0xf8)) return Status::DecodeError;
-        pg.offset = q;
-        pg.continuation = h[5] & 1, pg.first = (h[5] & 2) != 0, pg.last = (h[5] & 4) != 0;
-        pg.absgp = detail::le64(h + 6);
-        pg.serial = detail::le32(h + 14), pg.sequence = detail::le32(h + 18), pg.crc = detail::le32(h + 22);
-        pg.n_segments = h[26];
-        if (pos_ + pg.n_segments > n_) return pos_ = n_, Status::EndOfStream;
-        const uint8_t* lacing = d_ + pos_;
-        uint32_t body = 0, run = 0;
+        static constexpr detail::Crc32Table tab{};
+        OggPageHead h;
+        const Status s = ogg_check_page(d_, n_, q, tab.t, h, &pos_);
+        if (s != Status::Ok) return s;
+        pg.offset = h.offset, pg.absgp = h.absgp, pg.serial = h.serial, pg.sequence = h.sequence, pg.crc = h.crc;
+        pg.n_segments = h.n_segments, pg.continuation = h.continuation, pg.first = h.first, pg.last = h.last;
+        pg.body_offset = h.body_offset, pg.body_len = h.body_len;
+        pg.lacing = d_ + q + kOggHeaderSize;
+        uint32_t run = 0;
         pg.n_packets = 0;
         for (unsigned i = 0; i < pg.n_segments; ++i) {
-            body += lacing[i], run += lacing[i];
-            if (lacing[i] < 255) pg.packet_len[pg.n_packets++] = uint16_t(run), run = 0;  // a short segment closes a packet
+            run += pg.lacing[i];
+            if (pg.lacing[i] < 255) pg.packet_len[pg.n_packets++] = uint16_t(run), run = 0;  // a short segment closes a packet
         }
-        pos_ += pg.n_segments;
-        if (pos_ + body > n_) return pos_ = n_, Status::EndOfStream;
-        pg.body_offset = pos_, pg.body_len = body;
-        // checksum over the page with its own checksum field read as zero
-        static const uint8_t zero[4] = {0, 0, 0, 0};
-        uint32_t crc = crc32_update(0, h, 22);
-        crc = crc32_update(crc, zero, 4);
-        crc = crc32_update(crc, h + 26, 1 + size_t(pg.n_segments) + body);
-        if (crc != pg.crc) {
-            pos_ = q + 4;
-            return Status::DecodeError;
-        }
-        pos_ += body;
         return Status::Ok;
     }
 
@@ -668,45 +703,82 @@ struct OggPacket {
     bool last_on_page;
 };
 
-// logical.rs:104-205, 577-620 without the codec mapper: reassembles the packets of one serial number.
+// What a logical stream carries from one page to the next.  The stream's pieces are numbered from 0; the open packet owns
+// pieces [part_first, n_pieces).
+struct OggStreamState {
+    uint64_t part_len = 0;  // bytes of the packet still waiting for its continuation
+    uint32_t part_first = 0, n_pieces = 0, prev_seq = 0;
+    bool have_prev = false;
+};
+
+// logical.rs:104-205, 577-620 without the codec mapper: one page of a logical stream.  `lacing` holds the page's
+// n_segments lacing values.  The sink is told sink.piece(index, offset, len) for every piece (an index below an earlier
+// one replaces what was dropped), sink.packet(first_piece, n_pieces, len, page) for every completed packet and
+// sink.last_on_page() after the page's last completed packet.  DecodeError when an open packet would pass the reference's
+// 16 MiB cap; the page's completed packets are kept.
+#if defined(__CUDACC__)
+#pragma nv_exec_check_disable  // a host sink makes a host-only instantiation
+#endif
+template <class Sink>
+SYMGPU_PACKET_HD inline Status ogg_stream_page(OggStreamState& st, const OggPageHead& pg, const uint8_t* lacing, Sink& sink) {
+    if (st.have_prev && (pg.sequence < st.prev_seq || pg.sequence - st.prev_seq > 1)) st.n_pieces = st.part_first, st.part_len = 0;  // lost or re-ordered pages
+    st.have_prev = true, st.prev_seq = pg.sequence;
+    if (!pg.continuation && st.part_len > 0) st.n_pieces = st.part_first, st.part_len = 0;  // the continuation never came
+    unsigned seg = 0;
+    // the next packet that ends on this page (false: none left)
+    auto next_len = [&](uint32_t& len) {
+        uint32_t run = 0;
+        while (seg < pg.n_segments) {
+            const uint8_t v = lacing[seg++];
+            run += v;
+            if (v < 255) return len = run, true;
+        }
+        return false;
+    };
+    uint64_t at = pg.body_offset;
+    uint32_t n;
+    bool more = next_len(n);
+    if (pg.continuation && st.part_len == 0) {
+        // the head of this packet was never seen: drop its tail, or the whole page when nothing else ends here
+        if (!more) return Status::Ok;
+        at += n;
+        more = next_len(n);
+    }
+    bool any = false;
+    for (; more; more = next_len(n)) {
+        sink.piece(st.n_pieces++, at, n);
+        sink.packet(st.part_first, st.n_pieces - st.part_first, st.part_len + n, pg);
+        st.part_first = st.n_pieces, st.part_len = 0;
+        at += n;
+        any = true;
+    }
+    if (any) sink.last_on_page();
+    const uint64_t rest = pg.body_offset + pg.body_len - at;
+    if (rest > 0) {
+        if (st.part_len + rest > kOggMaxPacketLen) return Status::DecodeError;
+        sink.piece(st.n_pieces++, at, uint32_t(rest));
+        st.part_len += rest;
+    }
+    return Status::Ok;
+}
+
 class OggLogicalStream {
   public:
     // DecodeError when an open packet would pass the reference's 16 MiB cap; the page's completed packets are kept.
     Status read_page(const OggPage& pg) {
-        if (have_prev_ && (pg.sequence < prev_seq_ || pg.sequence - prev_seq_ > 1)) drop_partial();  // lost or re-ordered pages
-        have_prev_ = true, prev_seq_ = pg.sequence;
-        if (!pg.continuation && part_len_ > 0) drop_partial();  // the continuation never came
-        unsigned i = 0;
-        uint64_t at = pg.body_offset;
-        if (pg.continuation && part_len_ == 0) {
-            // the head of this packet was never seen: drop its tail, or the whole page when nothing else ends here
-            if (pg.n_packets == 0) return Status::Ok;
-            at += pg.packet_len[i++];
-        }
-        const size_t before = packets_.size();
-        for (; i < pg.n_packets; ++i) {
-            const uint32_t n = pg.packet_len[i];
-            pieces_.push_back(Piece{at, n});
-            OggPacket p;
-            p.first_piece = part_first_, p.n_pieces = uint32_t(pieces_.size()) - part_first_, p.len = part_len_ + n;
-            p.page_sequence = pg.sequence, p.page_absgp = pg.absgp, p.last_on_page = false;
-            packets_.push_back(p);
-            part_first_ = uint32_t(pieces_.size()), part_len_ = 0;
-            at += n;
-        }
-        if (packets_.size() > before) packets_.back().last_on_page = true;
-        const uint64_t rest = pg.body_offset + pg.body_len - at;
-        if (rest > 0) {
-            if (part_len_ + rest > kOggMaxPacketLen) return Status::DecodeError;
-            pieces_.push_back(Piece{at, uint32_t(rest)});
-            part_len_ += rest;
-        }
-        return Status::Ok;
+        OggPageHead h;
+        h.offset = pg.offset, h.absgp = pg.absgp, h.body_offset = pg.body_offset, h.serial = pg.serial, h.sequence = pg.sequence;
+        h.crc = pg.crc, h.body_len = pg.body_len, h.n_segments = pg.n_segments;
+        h.continuation = pg.continuation, h.first = pg.first, h.last = pg.last;
+        Sink sink{this};
+        const Status s = ogg_stream_page(st_, h, pg.lacing, sink);
+        pieces_.resize(st_.n_pieces);
+        return s;
     }
 
     const std::vector<OggPacket>& packets() const { return packets_; }
     const std::vector<Piece>& pieces() const { return pieces_; }
-    uint64_t open_len() const { return part_len_; }  // bytes of a packet still waiting for its continuation
+    uint64_t open_len() const { return st_.part_len; }  // bytes of a packet still waiting for its continuation
 
     // Copy a packet out of the source buffer (tests, host-side header parsing); the device path gathers instead.
     void gather(const uint8_t* src, const OggPacket& p, uint8_t* dst) const {
@@ -718,17 +790,110 @@ class OggLogicalStream {
     }
 
   private:
-    void drop_partial() {
-        pieces_.resize(part_first_);
-        part_len_ = 0;
-    }
+    struct Sink {
+        OggLogicalStream* ls;
+        void piece(uint32_t i, uint64_t offset, uint32_t len) {
+            ls->pieces_.resize(i);
+            ls->pieces_.push_back(Piece{offset, len});
+        }
+        void packet(uint32_t first, uint32_t count, uint64_t len, const OggPageHead& pg) {
+            ls->packets_.push_back(OggPacket{first, count, len, pg.sequence, pg.absgp, false});
+        }
+        void last_on_page() { ls->packets_.back().last_on_page = true; }
+    };
     std::vector<OggPacket> packets_;
     std::vector<Piece> pieces_;
-    uint32_t part_first_ = 0;  // pieces_[part_first_..] belong to the packet still open
-    uint64_t part_len_ = 0;
-    bool have_prev_ = false;
-    uint32_t prev_seq_ = 0;
+    OggStreamState st_;
 };
+
+// ---- the schedule of the device index (symgpu_ogg_index_dev), step by step over one file d[0..n) --------------------------
+// 1. A successor word per 4-byte group, each found on its own: two capture patterns cannot start within 4 bytes of each other, so
+//    a group holds at most one.  0 = none; else bits 0-1 its place in the group, bits 2-3 the kind, bits 5.. the distance from
+//    it to where the reader goes next (< 2^17: at most a page).
+enum : uint32_t { kOggWordPage = 1, kOggWordSkip = 2, kOggWordEnd = 3 };
+
+SYMGPU_PACKET_HD inline uint32_t ogg_successor_word(const uint8_t* d, size_t n, size_t w, const uint32_t (*crc)[256]) {
+    for (uint32_t k = 0; k < 4 && w * 4 + k + 4 <= n; ++k) {
+        const size_t q = w * 4 + k;
+        if (d[q] != 'O' || d[q + 1] != 'g' || d[q + 2] != 'g' || d[q + 3] != 'S') continue;
+        OggPageHead pg;
+        size_t next;
+        const Status s = ogg_check_page(d, n, q, crc, pg, &next);
+        const uint32_t kind = s == Status::Ok ? kOggWordPage : s == Status::DecodeError ? kOggWordSkip : kOggWordEnd;
+        return uint32_t(kind == kOggWordEnd ? 0 : next - q) << 5 | kind << 2 | k;
+    }
+    return 0;
+}
+
+// 2. The chain: the next page that verifies at or after *pos (false: the file ends); *pos moves past it as the reader's does.
+//    Over a whole file, *pos only grows, so the chain costs one look per word at most.
+SYMGPU_PACKET_HD inline bool ogg_next_page(const uint32_t* succ, uint64_t n, uint64_t* pos, uint64_t* page) {
+    const uint64_t n_words = (n + 3) / 4;
+    for (uint64_t w = *pos / 4; w < n_words; ++w) {
+        const uint32_t v = succ[w];
+        if (!v) continue;
+        const uint64_t q = w * 4 + (v & 3);
+        if (q < *pos) continue;
+        const uint32_t kind = (v >> 2) & 3;
+        if (kind == kOggWordEnd) break;
+        *pos = q + (v >> 5);
+        if (kind == kOggWordPage) return *page = q, true;
+        w = *pos / 4 - 1;
+    }
+    *pos = n;
+    return false;
+}
+
+// 3. The chain's pages ordered by serial, chain order kept within a serial: a stable least-significant-digit radix sort, four
+//    passes of 8 bits, so linear in the pages whatever the serials.  keys[i] = the serial of page i, vals[i] = its offset;
+//    tmp_keys / tmp_vals hold n items each; the result is back in keys / vals.
+SYMGPU_PACKET_HD inline void ogg_sort_by_serial(uint32_t* keys, uint32_t* vals, uint32_t* tmp_keys, uint32_t* tmp_vals, size_t n) {
+    uint32_t *ik = keys, *iv = vals, *ok = tmp_keys, *ov = tmp_vals;
+    for (int shift = 0; shift < 32; shift += 8) {
+        uint32_t count[256];
+        for (int b = 0; b < 256; ++b) count[b] = 0;
+        for (size_t i = 0; i < n; ++i) ++count[(ik[i] >> shift) & 0xff];
+        uint32_t at = 0;
+        for (int b = 0; b < 256; ++b) {
+            const uint32_t c = count[b];
+            count[b] = at, at += c;
+        }
+        for (size_t i = 0; i < n; ++i) {
+            const uint32_t j = count[(ik[i] >> shift) & 0xff]++;
+            ok[j] = ik[i], ov[j] = iv[i];
+        }
+        uint32_t* t = ik;
+        ik = ok, ok = t, t = iv, iv = ov, ov = t;
+    }
+}
+
+// 4. The logical streams (OggIndex::build's routing) from the chain sorted by serial: in ascending serial order, a serial's pages
+//    before its first first-page are orphans, the rest go through ogg_stream_page.  sink.begin_stream(serial) / end_stream()
+//    bracket every stream.  Linear in the pages.  Returns true when a page hit the 16 MiB cap.
+#if defined(__CUDACC__)
+#pragma nv_exec_check_disable  // a host sink makes a host-only instantiation
+#endif
+template <class Sink>
+SYMGPU_PACKET_HD inline bool ogg_walk_streams(const uint8_t* d, const uint32_t* serials, const uint32_t* offsets, size_t n_pages, Sink& sink) {
+    bool cap_hit = false;
+    for (size_t k = 0; k < n_pages;) {
+        const uint32_t serial = serials[k];
+        size_t j = k;
+        while (j < n_pages && serials[j] == serial && !(d[offsets[j] + 5] & 2)) ++j;
+        if (j < n_pages && serials[j] == serial) {
+            OggStreamState st;
+            sink.begin_stream(serial);
+            for (; j < n_pages && serials[j] == serial; ++j) {
+                OggPageHead pg;
+                ogg_page_fields(d, offsets[j], pg);
+                if (ogg_stream_page(st, pg, d + offsets[j] + kOggHeaderSize, sink) != Status::Ok) cap_hit = true;
+            }
+            sink.end_stream();
+        }
+        k = j;
+    }
+    return cap_hit;
+}
 
 // A physical stream: every page that verifies, routed by serial number.  A logical stream exists from its
 // beginning-of-stream page on (demuxer.rs:320-345); pages of serials never announced are counted and skipped.
@@ -772,11 +937,11 @@ struct OggIndex {
 // Bits least-significant first, as Vorbis packs them (symphonia-core/src/io/bit.rs:941-1027).
 class BitReaderRtl {
   public:
-    BitReaderRtl(const uint8_t* p, size_t n) : p_(p), n_bits_(uint64_t(n) * 8) {}
-    bool ok() const { return ok_; }
-    uint64_t bits_left() const { return n_bits_ - at_; }
+    SYMGPU_PACKET_HD BitReaderRtl(const uint8_t* p, size_t n) : p_(p), n_bits_(uint64_t(n) * 8) {}
+    SYMGPU_PACKET_HD bool ok() const { return ok_; }
+    SYMGPU_PACKET_HD uint64_t bits_left() const { return n_bits_ - at_; }
     // Past the end: returns 0 and latches !ok() (every caller checks once per structure, not per field).
-    uint32_t read(unsigned width) {
+    SYMGPU_PACKET_HD uint32_t read(unsigned width) {
         if (width > bits_left()) return ok_ = false, at_ = n_bits_, 0u;
         uint64_t v = 0;
         const uint64_t byte = at_ >> 3;
@@ -785,8 +950,8 @@ class BitReaderRtl {
         at_ += width;
         return uint32_t((v >> shift) & ((uint64_t(1) << width) - 1));
     }
-    bool read_bool() { return read(1) != 0; }
-    void ignore(uint64_t width) {
+    SYMGPU_PACKET_HD bool read_bool() { return read(1) != 0; }
+    SYMGPU_PACKET_HD void ignore(uint64_t width) {
         if (width > bits_left()) ok_ = false, at_ = n_bits_;
         else at_ += width;
     }
@@ -797,7 +962,7 @@ class BitReaderRtl {
     bool ok_ = true;
 };
 
-inline uint32_t vorbis_ilog(uint32_t x) {
+SYMGPU_PACKET_HD inline uint32_t vorbis_ilog(uint32_t x) {
     uint32_t n = 0;
     for (; x; x >>= 1) ++n;
     return n;
@@ -1140,17 +1305,17 @@ inline Status vorbis_read_setup(const uint8_t* p, size_t n, const VorbisIdent& i
 class VorbisPacketTimer {
   public:
     VorbisPacketTimer() = default;
-    VorbisPacketTimer(const VorbisIdent& id, uint8_t num_modes, uint64_t long_block_mask)
+    SYMGPU_PACKET_HD VorbisPacketTimer(const VorbisIdent& id, uint8_t num_modes, uint64_t long_block_mask)
         : mask_(long_block_mask), num_modes_(num_modes), bs0_(id.bs0_exp), bs1_(id.bs1_exp) {}
-    void reset() { prev_exp_ = 0; }
+    SYMGPU_PACKET_HD void reset() { prev_exp_ = 0; }
     // New headers, same overlap state (a chained stream restarts its modes but a caller batching one stream in
     // several calls carries the previous block across them).
-    void rebind(const VorbisIdent& id, uint8_t num_modes, uint64_t long_block_mask) {
+    SYMGPU_PACKET_HD void rebind(const VorbisIdent& id, uint8_t num_modes, uint64_t long_block_mask) {
         mask_ = long_block_mask, num_modes_ = num_modes, bs0_ = id.bs0_exp, bs1_ = id.bs1_exp;
     }
-    uint8_t prev_exp() const { return prev_exp_; }  // 0: no previous block
+    SYMGPU_PACKET_HD uint8_t prev_exp() const { return prev_exp_; }  // 0: no previous block
     // A packet that is not audio, names no valid mode or is cut short takes no time and leaves the state alone.
-    void next(const uint8_t* p, size_t n, uint64_t& dur, uint64_t& discard) {
+    SYMGPU_PACKET_HD void next(const uint8_t* p, size_t n, uint64_t& dur, uint64_t& discard) {
         dur = discard = 0;
         BitReaderRtl bs(p, n);
         if (bs.read_bool() || !bs.ok()) return;
@@ -1196,7 +1361,7 @@ inline Status vorbis_unpack_xiph_laced(const uint8_t* p, size_t n, Piece& ident,
 // sequence number is the previous one's + 1), otherwise at end - total duration; a stream whose packets all end on one page
 // starts at -discard when that leaves padding at the end (the reference's single-page rule, applied here to "every stream
 // packet ends on the same page").
-inline void ogg_page_end_trims(const uint32_t* page_sequence, const uint64_t* page_absgp, const uint32_t* dur, const uint32_t* discard,
+SYMGPU_PACKET_HD inline void ogg_page_end_trims(const uint32_t* page_sequence, const uint64_t* page_absgp, const uint32_t* dur, const uint32_t* discard,
                                size_t n, uint32_t* trim_end) {
     bool single_page = true;
     for (size_t i = 1; i < n; ++i) single_page = single_page && page_sequence[i] == page_sequence[0];
@@ -1216,7 +1381,8 @@ inline void ogg_page_end_trims(const uint32_t* page_sequence, const uint64_t* pa
         for (size_t k = i; k < j; ++k) {
             next += dur[k];
             const int64_t left = int64_t(dur[k]) - int64_t(discard[k]);
-            trim_end[k] = next > page_end ? uint32_t(std::min<int64_t>(next - page_end, left < 0 ? 0 : left)) : 0u;
+            const int64_t over = next - page_end, room = left < 0 ? 0 : left;
+            trim_end[k] = next > page_end ? uint32_t(over < room ? over : room) : 0u;
         }
         have_prev = true, prev_seq = page_sequence[i], prev_end = page_end, i = j;
     }

@@ -130,6 +130,14 @@ assert VORBIS_JOB_DTYPE.itemsize == 24 and VORBIS_SETUP_REF_DTYPE.itemsize == 24
 assert VORBIS_GROUP_DTYPE.itemsize == 24 and VORBIS_RESULT_DTYPE.itemsize == 24
 VORBIS_JOB_DECODED, VORBIS_JOB_REFUSED, VORBIS_JOB_INVALID = 0, 1, 2
 VORBIS_MAX_FILES = 65536
+
+# Ogg pages indexed on the device: `symgpu_file_range` (16 bytes), `symgpu_ogg_file_index` (40 bytes)
+FILE_RANGE_DTYPE = np.dtype([("offset", "<u8"), ("len", "<u8")])
+OGG_FILE_INDEX_DTYPE = np.dtype([("first_packet", "<u8"), ("first_piece", "<u8"), ("packet_bytes", "<u8"), ("n_packets", "<u4"), ("n_pieces", "<u4"),
+                                 ("max_packet_len", "<u4"), ("status", "u1"), ("reserved", "u1", (3,))])
+assert FILE_RANGE_DTYPE.itemsize == 16 and OGG_FILE_INDEX_DTYPE.itemsize == 40
+OGG_MAX_FILES = 65536
+OGG_CAP_HIT, OGG_NOT_WRITTEN = 1, 2
 MP3_FILE_DTYPE = np.dtype([("data", "<u8"), ("n", "<u8"), ("packets", "<u8"), ("n_packets", "<u8"), ("stream", "<u4"), ("reserved", "<u4")])
 assert MP3_FILE_DTYPE.itemsize == 40
 VORBIS_SETUP_INFO_DTYPE = np.dtype([("n_codebooks", "<u4"), ("n_floors", "<u4"), ("n_residues", "<u4"), ("n_mappings", "<u4"), ("n_modes", "<u4"),
@@ -317,6 +325,8 @@ def lib():
     L.symgpu_vorbis_fe_config.argtypes = [vp, vp, vp, ctypes.POINTER(u32)]
     L.symgpu_vorbis_fe_decode.restype = ctypes.c_int
     L.symgpu_vorbis_fe_decode.argtypes = [vp, vp, sz, u32, u32, vp, vp, vp]
+    L.symgpu_ogg_index_dev.restype = ctypes.c_int
+    L.symgpu_ogg_index_dev.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, sz, vp]
     L.symgpu_ogg_gather.restype = ctypes.c_int
     L.symgpu_ogg_gather.argtypes = [vp, sz, vp, sz, vp, sz, vp, sz, vp, ctypes.POINTER(sz)]
     L.symgpu_ogg_page_end_trims.restype = ctypes.c_int

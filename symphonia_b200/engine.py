@@ -395,6 +395,37 @@ class Engine:
                                                        _dev_ptr(jobs_t), n_jobs, _host_ptr(groups), len(groups), int(fmt), _dev_ptr(out_t),
                                                        out_t.numel() * out_t.element_size(), _dev_ptr(results_t), _dev_ptr(status_t)))
 
+    # -- Ogg pages indexed on the device --------------------------------------------------------
+    def ogg_index_dev(self, data_t, ranges, cap_packets=None, cap_pieces=None):
+        """(packets_t, pieces_t, index) for the files data_t[offset : offset + len] of `ranges` (FILE_RANGE_DTYPE records, or
+        (offset, len) pairs) in a uint8 CUDA tensor: packets_t / pieces_t the uint8 bytes of OGG_PACKET_DTYPE / PIECE_DTYPE
+        records on the device, index the files' OGG_FILE_INDEX_DTYPE records on the host.  File i's tables, its packets
+        [first_packet, first_packet + n_packets) and pieces likewise, equal packetizer.ogg_index of its bytes.  Without
+        capacities the sizes are found first by a call with none (its index read back), then the tables written by a second."""
+        import torch
+        from ._native import FILE_RANGE_DTYPE, OGG_FILE_INDEX_DTYPE, OGG_PACKET_DTYPE, PIECE_DTYPE
+        assert data_t.is_cuda and data_t.is_contiguous() and data_t.dtype == torch.uint8
+        r = np.ascontiguousarray(np.array(ranges, dtype=np.uint64).reshape(-1, 2).view(FILE_RANGE_DTYPE).reshape(-1)
+                                 if not isinstance(ranges, np.ndarray) or ranges.dtype != FILE_RANGE_DTYPE else ranges)
+        index_t = torch.empty(len(r) * OGG_FILE_INDEX_DTYPE.itemsize, dtype=torch.uint8, device=data_t.device)
+
+        def call(packets_t, pieces_t):
+            torch.cuda.current_stream(data_t.device).synchronize()  # data_t and the outputs are torch's: written / allocated on its stream
+            self._check(self._lib.symgpu_ogg_index_dev(self._ctx, _dev_ptr(data_t), data_t.numel(), _host_ptr(r), len(r), _dev_ptr(packets_t),
+                                                       packets_t.numel() // OGG_PACKET_DTYPE.itemsize, _dev_ptr(pieces_t),
+                                                       pieces_t.numel() // PIECE_DTYPE.itemsize, _dev_ptr(index_t)))
+            self.sync()
+            return index_t.cpu().numpy().view(OGG_FILE_INDEX_DTYPE)
+
+        def totals(ix):
+            return (int(ix["first_packet"][-1]) + int(ix["n_packets"][-1]), int(ix["first_piece"][-1]) + int(ix["n_pieces"][-1])) if len(ix) else (0, 0)
+        none = torch.empty(0, dtype=torch.uint8, device=data_t.device)
+        if cap_packets is None or cap_pieces is None:
+            cap_packets, cap_pieces = totals(call(none, none))
+        packets_t = torch.empty(cap_packets * OGG_PACKET_DTYPE.itemsize, dtype=torch.uint8, device=data_t.device)
+        pieces_t = torch.empty(cap_pieces * PIECE_DTYPE.itemsize, dtype=torch.uint8, device=data_t.device)
+        return packets_t, pieces_t, call(packets_t, pieces_t)
+
     # -- output stage -------------------------------------------------------------------------
     def pcm_pack_host(self, pcm, spans, channels, fmt, out_frames, plane_stride=0, frames=0, n_spans=None, out=None):
         """Trim + interleave + convert planar f32 `pcm` (any shape, flat indexing) into [out_frames, channels]
