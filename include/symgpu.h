@@ -983,6 +983,74 @@ symgpu_status symgpu_ogg_index_dev(symgpu_ctx* ctx, const uint8_t* data, size_t 
                                    symgpu_ogg_file_index* index);
 
 /* ===================================================================================================
+ * Vorbis jobs built on the device from the device Ogg index (DESIGN 5b / 5f): what decode.ogg_vorbis_index chooses and
+ * computes for each file, as records symgpu_vorbis_decode_dev takes.  The three calls below take the tables of
+ * symgpu_ogg_index_dev (data, files, packets, pieces, index as it wrote them) and share its argument rules: data, packets,
+ * pieces and index device memory, files host memory; SYMGPU_ERR_ARG for a range outside data[0 .. n_bytes) or a missing
+ * pointer, SYMGPU_ERR_LIMIT for more than SYMGPU_OGG_MAX_FILES files; both before anything is launched.  Each call queues a
+ * fixed number of launches, whatever the number of files or packets, and returns without a host wait.
+ * ================================================================================================= */
+typedef struct symgpu_vorbis_file_heads {  /* 32 bytes: one file's Vorbis stream                                      */
+    uint64_t audio_bytes;    /* its audio packets' lengths, summed                                                     */
+    uint32_t n_stream;       /* the stream: the file's packets [0, n_stream), those of its first packet's serial       */
+    uint32_t ident_len;      /* the identification header is the file's packet 0                                       */
+    uint32_t setup;          /* the setup header: the first later packet of >= 7 bytes starting 0x05 "vorbis"          */
+    uint32_t setup_len;
+    uint32_t n_audio;        /* audio packets: after the setup, in the stream, not empty, first byte even              */
+    uint8_t status;          /* SYMGPU_VORBIS_NO_PACKETS, SYMGPU_VORBIS_NO_SETUP (setup, setup_len and n_audio 0) or 0 */
+    uint8_t reserved[3];
+} symgpu_vorbis_file_heads;
+enum { SYMGPU_VORBIS_NO_PACKETS = 1, SYMGPU_VORBIS_NO_SETUP = 2 };
+typedef struct symgpu_vorbis_packet_rank { /* 24 bytes: one packet of the table                                        */
+    uint64_t byte_at;        /* audio bytes of the packets before it in the table, every file's                        */
+    uint64_t rank;           /* audio packets before it in the table, every file's                                      */
+    uint8_t audio;           /* 1: an audio packet of its file's Vorbis stream                                          */
+    uint8_t reserved[7];
+} symgpu_vorbis_packet_rank;
+/* heads[i] for every file and ranks[k] for every packet of the table (n_packets: the table's total).  Each file's packets
+ * are walked only to its setup header; the ranks are a scan over the whole table.  Four launches.  Scratch from the context's
+ * staging buffer: 16 bytes per file. */
+symgpu_status symgpu_vorbis_heads_dev(symgpu_ctx* ctx, const uint8_t* data, size_t n_bytes, const symgpu_file_range* files, size_t n_files,
+                                      const symgpu_ogg_packet* packets, size_t n_packets, const symgpu_piece* pieces,
+                                      const symgpu_ogg_file_index* index, symgpu_vorbis_file_heads* heads, symgpu_vorbis_packet_rank* ranks);
+
+typedef struct symgpu_ogg_packet_ref {     /* 16 bytes                                                                  */
+    uint64_t dst;            /* where the packet's bytes go in `out`                                                    */
+    uint32_t file;
+    uint32_t packet;         /* index among the file's packets                                                          */
+} symgpu_ogg_packet_ref;
+/* Copies the packets `refs` (host memory) name, their pieces back to back, to out + dst (device memory, out_cap bytes).  A
+ * ref whose file or packet does not exist, or whose bytes would pass out_cap, copies nothing.  One launch, one warp per ref.
+ * Scratch from the staging buffer: 16 bytes per file and per ref. */
+symgpu_status symgpu_ogg_gather_dev(symgpu_ctx* ctx, const uint8_t* data, size_t n_bytes, const symgpu_file_range* files, size_t n_files,
+                                    const symgpu_ogg_packet* packets, const symgpu_piece* pieces, const symgpu_ogg_file_index* index,
+                                    const symgpu_ogg_packet_ref* refs, size_t n_refs, uint8_t* out, size_t out_cap);
+
+typedef struct symgpu_vorbis_file_jobs {   /* 40 bytes: one file's share of the jobs (host memory)                          */
+    uint64_t long_block_mask;/* from its setup: bit i = mode i uses the long block                                      */
+    uint64_t byte_at;        /* its audio packets go to out[byte_at ..][.. n_bytes) back to back                         */
+    uint64_t n_bytes;        /* = heads[i].audio_bytes                                                                  */
+    uint32_t first_job;      /* its jobs are jobs[first_job ..][.. n_jobs) in stream order                               */
+    uint32_t n_jobs;         /* = heads[i].n_audio                                                                      */
+    uint8_t n_modes;         /* 1 .. 64; 0: the file has no jobs (the other fields are ignored)                          */
+    uint8_t bs0_exp, bs1_exp;/* from its identification header: 6 <= bs0_exp <= bs1_exp <= 13                           */
+    uint8_t reserved[5];
+} symgpu_vorbis_file_jobs;
+/* For every audio packet of every file with n_modes != 0: its bytes gathered to `out`, and its symgpu_vorbis_job with the
+ * offset into `out`, its length, the leading discard and the page end trim of symgpu_vorbis_packet_durations and
+ * symgpu_ogg_page_end_trims over the file's audio packets (mappings/vorbis.rs:45-107, symphonia-format-ogg/src/logical.rs:
+ * 164-302), computed by scans rather than a walk per file.  ranks as symgpu_vorbis_heads_dev wrote them.  SYMGPU_ERR_ARG, on
+ * top of the rules above, for a file record out of range (n_modes over 64, block exponents outside 6..13 or out of order, jobs
+ * past n_jobs, bytes past out_cap); SYMGPU_ERR_LIMIT for n_jobs of 2^32 or more.  A job slot no packet fills is written as
+ * {0, 0, 0, 0}.  Three launches, one warp per packet for the gather.  Scratch from the staging buffer: 40 bytes per file and
+ * about 60 per job. */
+symgpu_status symgpu_vorbis_jobs_dev(symgpu_ctx* ctx, const uint8_t* data, size_t n_bytes, const symgpu_file_range* files, size_t n_files,
+                                     const symgpu_ogg_packet* packets, size_t n_packets, const symgpu_piece* pieces,
+                                     const symgpu_ogg_file_index* index, const symgpu_vorbis_packet_rank* ranks,
+                                     const symgpu_vorbis_file_jobs* file_jobs, uint8_t* out, size_t out_cap, symgpu_vorbis_job* jobs,
+                                     size_t n_jobs);
+
+/* ===================================================================================================
  * MPEG Layer I / II sample decoders (SURVEY 8f N1 for the Layer I / II path): a packet becomes the sub-band samples
  * symgpu_mpa12_synth_* take.  CPU only, stateless apart from the stream's signal specification.
  *   Layer1::decode up to the synthesis call   symphonia-bundle-mp3/src/layer1/mod.rs:19-176

@@ -1301,6 +1301,27 @@ inline Status vorbis_read_setup(const uint8_t* p, size_t n, const VorbisIdent& i
     return Status::Ok;
 }
 
+// mappings/vorbis.rs:62-106 for one packet: the block exponent its mode names, 0 when the packet is not audio (type bit set),
+// is cut short or names no mode.  p / n: its first bytes (two always suffice: 1 type bit + at most 6 mode bits).
+SYMGPU_PACKET_HD inline uint8_t vorbis_packet_exp(const uint8_t* p, size_t n, uint8_t num_modes, uint64_t long_block_mask, uint8_t bs0_exp,
+                                                  uint8_t bs1_exp) {
+    BitReaderRtl bs(p, n);
+    if (bs.read_bool() || !bs.ok()) return 0;
+    const uint32_t mode = bs.read(vorbis_ilog(uint32_t(num_modes) - 1)) & 0xff;
+    if (!bs.ok() || mode >= num_modes) return 0;
+    return (long_block_mask >> mode) & 1 ? bs1_exp : bs0_exp;
+}
+
+// (duration, leading samples to discard) of a packet of block exponent `exp` whose nearest earlier packet with a non-zero
+// exponent had `prev_exp` (0: none): a packet without a block takes no time, and a first block has nothing to overlap with,
+// so its lapped half is thrown away.
+SYMGPU_PACKET_HD inline void vorbis_packet_time(uint8_t prev_exp, uint8_t exp, uint64_t& dur, uint64_t& discard) {
+    const uint64_t cur = exp ? uint64_t(1) << exp : 0;
+    dur = discard = 0;
+    if (exp && prev_exp) dur = ((uint64_t(1) << prev_exp) >> 2) + (cur >> 2);
+    else if (exp) dur = discard = cur >> 1;
+}
+
 // mappings/vorbis.rs:45-107: (duration, leading samples to discard) of each audio packet in turn.
 class VorbisPacketTimer {
   public:
@@ -1316,16 +1337,9 @@ class VorbisPacketTimer {
     SYMGPU_PACKET_HD uint8_t prev_exp() const { return prev_exp_; }  // 0: no previous block
     // A packet that is not audio, names no valid mode or is cut short takes no time and leaves the state alone.
     SYMGPU_PACKET_HD void next(const uint8_t* p, size_t n, uint64_t& dur, uint64_t& discard) {
-        dur = discard = 0;
-        BitReaderRtl bs(p, n);
-        if (bs.read_bool() || !bs.ok()) return;
-        const uint32_t mode = bs.read(vorbis_ilog(uint32_t(num_modes_) - 1)) & 0xff;
-        if (!bs.ok() || mode >= num_modes_) return;
-        const unsigned exp = (mask_ >> mode) & 1 ? bs1_ : bs0_;
-        const uint64_t cur = uint64_t(1) << exp;
-        if (prev_exp_) dur = ((uint64_t(1) << prev_exp_) >> 2) + (cur >> 2);
-        else dur = discard = cur >> 1;  // nothing to overlap with: the lapped half is thrown away
-        prev_exp_ = uint8_t(exp);
+        const uint8_t exp = vorbis_packet_exp(p, n, num_modes_, mask_, bs0_, bs1_);
+        vorbis_packet_time(prev_exp_, exp, dur, discard);
+        if (exp) prev_exp_ = exp;
     }
 
   private:
@@ -1386,6 +1400,68 @@ SYMGPU_PACKET_HD inline void ogg_page_end_trims(const uint32_t* page_sequence, c
         }
         have_prev = true, prev_seq = page_sequence[i], prev_end = page_end, i = j;
     }
+}
+
+// ogg_page_end_trims restated run by run, so that each packet's trim can be computed on its own from prefix sums.  A run is a
+// stretch of consecutive packets with equal page_sequence; `end` is its first packet's page_absgp, tot / disc its packets' dur
+// / discard summed.  The run's start: the previous run's end when that run's sequence number is one less (uint32, so a wrap
+// counts), else -disc when the run is the stream's only run and that leaves padding at the end, else end - tot.
+SYMGPU_PACKET_HD inline int64_t ogg_run_start(bool have_prev, uint32_t prev_seq, int64_t prev_end, uint32_t seq, bool only_run, int64_t tot,
+                                              int64_t disc, int64_t end) {
+    if (have_prev && uint32_t(prev_seq + 1) == seq) return prev_end;
+    if (only_run && tot >= disc + end) return -disc;
+    return end - tot;
+}
+// A packet's trim: `next` is its run's start plus the durations of the run's packets up to and including it.
+SYMGPU_PACKET_HD inline uint32_t ogg_packet_end_trim(int64_t next, int64_t end, uint32_t dur, uint32_t discard) {
+    const int64_t left = int64_t(dur) - int64_t(discard), room = left < 0 ? 0 : left, over = next - end;
+    return next > end ? uint32_t(over < room ? over : room) : 0u;
+}
+
+// Up to n leading bytes of a packet whose pieces are pieces[0 .. n_pieces) (offsets into d) into out; returns how many exist.
+template <class P>
+SYMGPU_PACKET_HD inline uint32_t ogg_packet_head(const uint8_t* d, const P* pieces, uint32_t n_pieces, uint8_t* out, uint32_t n) {
+    uint32_t got = 0;
+    for (uint32_t k = 0; k < n_pieces && got < n; ++k)
+        for (uint32_t b = 0; b < pieces[k].len && got < n; ++b) out[got++] = d[pieces[k].offset + b];
+    return got;
+}
+
+// The Vorbis headers of a file's packet table (packets grouped by serial in ascending order, as symgpu_ogg_index gives them),
+// chosen as decode.ogg_vorbis_index chooses them: the stream is the packets of the first packet's serial, [0, n_stream); its
+// first packet is the identification header; the setup header is the first later packet of 7 bytes or more that starts with
+// 0x05 "vorbis" (n_stream when there is none).  The stream's end is found by bisection and the walk stops at the setup.
+struct VorbisStreamHeads {
+    uint32_t n_stream, setup;
+};
+template <class Pk, class P>
+SYMGPU_PACKET_HD inline VorbisStreamHeads vorbis_stream_heads(const uint8_t* d, const Pk* packets, uint32_t n_packets, const P* pieces) {
+    VorbisStreamHeads h{0, 0};
+    if (n_packets == 0) return h;
+    const uint32_t serial = packets[0].serial;
+    uint32_t lo = 1, hi = n_packets;
+    while (lo < hi) {
+        const uint32_t mid = lo + (hi - lo) / 2;
+        if (packets[mid].serial == serial) lo = mid + 1;
+        else hi = mid;
+    }
+    h.n_stream = h.setup = lo;
+    for (uint32_t k = 1; k < lo; ++k) {
+        uint8_t b[7];
+        if (packets[k].len < 7 || ogg_packet_head(d, pieces + packets[k].first_piece, packets[k].n_pieces, b, 7) < 7) continue;
+        if (b[0] == 5 && b[1] == 'v' && b[2] == 'o' && b[3] == 'r' && b[4] == 'b' && b[5] == 'i' && b[6] == 's') {
+            h.setup = k;
+            break;
+        }
+    }
+    return h;
+}
+// Packet k of the table is an audio packet of the stream: after the setup, inside the stream, not empty, first byte even.
+template <class Pk, class P>
+SYMGPU_PACKET_HD inline bool vorbis_is_audio(const uint8_t* d, const Pk* packets, const P* pieces, VorbisStreamHeads h, uint32_t k) {
+    uint8_t b0 = 1;
+    return k > h.setup && k < h.n_stream && packets[k].len > 0 &&
+           ogg_packet_head(d, pieces + packets[k].first_piece, packets[k].n_pieces, &b0, 1) == 1 && (b0 & 1) == 0;
 }
 
 // mappings/vorbis.rs:109-285: the per-stream state machine.  detect() on the first packet of the first page,

@@ -138,6 +138,17 @@ OGG_FILE_INDEX_DTYPE = np.dtype([("first_packet", "<u8"), ("first_piece", "<u8")
 assert FILE_RANGE_DTYPE.itemsize == 16 and OGG_FILE_INDEX_DTYPE.itemsize == 40
 OGG_MAX_FILES = 65536
 OGG_CAP_HIT, OGG_NOT_WRITTEN = 1, 2
+# Vorbis jobs built on the device: `symgpu_vorbis_file_heads` (32 bytes), `symgpu_vorbis_packet_rank` (24),
+# `symgpu_ogg_packet_ref` (16), `symgpu_vorbis_file_jobs` (40)
+VORBIS_FILE_HEADS_DTYPE = np.dtype([("audio_bytes", "<u8"), ("n_stream", "<u4"), ("ident_len", "<u4"), ("setup", "<u4"), ("setup_len", "<u4"),
+                                    ("n_audio", "<u4"), ("status", "u1"), ("reserved", "u1", (3,))])
+VORBIS_PACKET_RANK_DTYPE = np.dtype([("byte_at", "<u8"), ("rank", "<u8"), ("audio", "u1"), ("reserved", "u1", (7,))])
+OGG_PACKET_REF_DTYPE = np.dtype([("dst", "<u8"), ("file", "<u4"), ("packet", "<u4")])
+VORBIS_FILE_JOBS_DTYPE = np.dtype([("long_block_mask", "<u8"), ("byte_at", "<u8"), ("n_bytes", "<u8"), ("first_job", "<u4"), ("n_jobs", "<u4"),
+                                   ("n_modes", "u1"), ("bs0_exp", "u1"), ("bs1_exp", "u1"), ("reserved", "u1", (5,))])
+assert VORBIS_FILE_HEADS_DTYPE.itemsize == 32 and VORBIS_PACKET_RANK_DTYPE.itemsize == 24
+assert OGG_PACKET_REF_DTYPE.itemsize == 16 and VORBIS_FILE_JOBS_DTYPE.itemsize == 40
+VORBIS_NO_PACKETS, VORBIS_NO_SETUP = 1, 2
 MP3_FILE_DTYPE = np.dtype([("data", "<u8"), ("n", "<u8"), ("packets", "<u8"), ("n_packets", "<u8"), ("stream", "<u4"), ("reserved", "<u4")])
 assert MP3_FILE_DTYPE.itemsize == 40
 VORBIS_SETUP_INFO_DTYPE = np.dtype([("n_codebooks", "<u4"), ("n_floors", "<u4"), ("n_residues", "<u4"), ("n_mappings", "<u4"), ("n_modes", "<u4"),
@@ -327,6 +338,12 @@ def lib():
     L.symgpu_vorbis_fe_decode.argtypes = [vp, vp, sz, u32, u32, vp, vp, vp]
     L.symgpu_ogg_index_dev.restype = ctypes.c_int
     L.symgpu_ogg_index_dev.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, sz, vp]
+    L.symgpu_vorbis_heads_dev.restype = ctypes.c_int
+    L.symgpu_vorbis_heads_dev.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, vp, vp, vp]
+    L.symgpu_ogg_gather_dev.restype = ctypes.c_int
+    L.symgpu_ogg_gather_dev.argtypes = [vp, vp, sz, vp, sz, vp, vp, vp, vp, sz, vp, sz]
+    L.symgpu_vorbis_jobs_dev.restype = ctypes.c_int
+    L.symgpu_vorbis_jobs_dev.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, vp, vp, vp, vp, sz, vp, sz]
     L.symgpu_ogg_gather.restype = ctypes.c_int
     L.symgpu_ogg_gather.argtypes = [vp, sz, vp, sz, vp, sz, vp, sz, vp, ctypes.POINTER(sz)]
     L.symgpu_ogg_page_end_trims.restype = ctypes.c_int

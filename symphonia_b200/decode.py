@@ -62,23 +62,29 @@ def ogg_vorbis_index(data, serial=None):
     padded = np.concatenate([blob, np.zeros(8, dtype=np.uint8)])
     b0, b1 = padded[off], padded[off + 1]                           # (bytes beyond a short packet are masked by `ln` below)
     ident_b = blob[off[0]:off[0] + ln[0]].tobytes()
-    ident = packetizer.vorbis_ident(ident_b)
     is_setup = (ln >= 7) & (b0 == 5)
     for k, c in enumerate(b"vorbis"):
         is_setup &= padded[off + 1 + k] == c
     is_setup[0] = False
-    if not is_setup.any():
-        raise ValueError("no Vorbis setup header")
-    at = int(np.argmax(is_setup))
-    setup_b = blob[off[at]:off[at] + ln[at]].tobytes()
-    n_modes, mask = packetizer.vorbis_setup_modes(setup_b, ident)
+    at = int(np.argmax(is_setup)) if is_setup.any() else None
+    setup_b = blob[off[at]:off[at] + ln[at]].tobytes() if at is not None else None
+    ident, n_modes, mask, fe = vorbis_open_headers(ident_b, setup_b)
     audio = np.nonzero((np.arange(len(mine)) > at) & (ln > 0) & ((b0 & 1) == 0))[0]
     heads = b0[audio].astype(np.uint16) | (np.where(ln[audio] > 1, b1[audio], 0).astype(np.uint16) << 8)
     dur, discard, _ = packetizer.vorbis_packet_durations(ident, n_modes, mask, None, heads=heads, lens=np.minimum(ln[audio], 2))
     dur, discard = dur.astype(np.int64), discard.astype(np.int64)
     trim_end = packetizer.ogg_page_end_trims(mine["page_sequence"][audio], mine["page_absgp"][audio], dur, discard).astype(np.int64)
-    fe = frontend.VorbisFrontend(ident_b, setup_b)
     return dict(blob=blob, table=table[audio], ident=ident, fe=fe, discard=discard, trim_end=trim_end, headers=(ident_b, setup_b))
+
+
+def vorbis_open_headers(ident_b, setup_b):
+    """The checks ogg_vorbis_index makes of a stream's identification and setup packets (setup_b None: the stream has none),
+    in its order and with its exceptions: (ident record, number of modes, long-block mask, VorbisFrontend on the two)."""
+    ident = packetizer.vorbis_ident(ident_b)
+    if setup_b is None:
+        raise ValueError("no Vorbis setup header")
+    n_modes, mask = packetizer.vorbis_setup_modes(setup_b, ident)
+    return ident, n_modes, mask, frontend.VorbisFrontend(ident_b, setup_b)
 
 
 def ogg_vorbis_plan(data, serial=None, index=None, out=None, slot=None, floor_base=0, threads=1):
@@ -839,6 +845,143 @@ def decode_vorbis_files(engine, files, fmt=nat.FMT_S16, threads=None, device=Fal
         stats.update(status=status, n_setups=len(setups))
     return _per_file(out, groups, plan["failed"],
                      lambda g: (int(results[g]["frames"]), int(results[g]["channels"]), int(results[g]["sample_rate"])))
+
+
+def decode_vorbis_files_dev(engine, data_t, ranges, fmt=nat.FMT_S16, errors=None, stats=None):
+    """decode_vorbis_files(engine, files, fmt, device=True) for Ogg Vorbis files already in device memory: file i is
+    data_t[offset : offset + len] of ranges[i] ((offset, len) pairs or FILE_RANGE_DTYPE records) in a uint8 CUDA tensor, and
+    its result, its message in errors[i] and `stats` (`status`, `n_setups`) are what decode_vorbis_files gives for those bytes.
+    The pages are indexed, the headers chosen and every audio packet's job built on the device; only per-file records and the
+    identification and setup packets come back to the host, which builds the setups from them.  stats also receives
+    `read_back_bytes`, every byte the call copies from the device.  A constant number of launches and host waits per call
+    (DESIGN §5f).  At most 65 536 files, mono / stereo, floor 1; replaces the engine's Vorbis stream and floor registration."""
+    return _vorbis_files_dev(engine, data_t, ranges, fmt, errors, stats)
+
+
+def _vorbis_files_dev(engine, data_t, ranges, fmt, errors, stats, mark=None):
+    """decode_vorbis_files_dev; mark(phase, state), when given, is called as each phase has been queued: 'start', 'index',
+    'heads', 'setup' (the host's work on the headers), 'jobs' (state: the gathered audio bytes, the job table and the groups,
+    on the device), 'decode'; state is {} for the others."""
+    import torch
+
+    from .engine import file_ranges
+    r = file_ranges(ranges)
+    n = len(r)
+    if n > nat.VORBIS_MAX_FILES:
+        raise ValueError(f"decode_vorbis_files_dev takes at most {nat.VORBIS_MAX_FILES} files per call, not {n}")
+    if not (data_t.is_cuda and data_t.dtype == torch.uint8 and data_t.is_contiguous()):
+        raise ValueError("decode_vorbis_files_dev takes a contiguous uint8 CUDA tensor")
+    size = data_t.numel()
+    if ((r["offset"] > size) | (r["len"] > size - np.minimum(r["offset"], size))).any():
+        raise ValueError(f"a file range lies outside the {size} bytes of data_t")
+    mark = mark or (lambda phase, state: None)
+    dev = data_t.device
+
+    def u8(count):
+        return torch.empty(int(count), dtype=torch.uint8, device=dev)
+
+    def bytes_of(t, dtype):
+        return t.cpu().numpy().view(dtype)
+    torch.cuda.current_stream(dev).synchronize()   # data_t is torch's: written on its stream
+    mark("start", {})
+    # 1. the page index, as Engine.ogg_index_dev builds it: sizes first, then the tables; the index stays on the device
+    index_t = u8(n * nat.OGG_FILE_INDEX_DTYPE.itemsize)
+    engine.ogg_index_dev_queue(data_t, r, u8(0), u8(0), index_t)
+    engine.sync()
+    ix = bytes_of(index_t, nat.OGG_FILE_INDEX_DTYPE)
+    read = ix.nbytes
+    n_packets = int(ix["first_packet"][-1]) + int(ix["n_packets"][-1]) if n else 0
+    n_pieces = int(ix["first_piece"][-1]) + int(ix["n_pieces"][-1]) if n else 0
+    packets_t, pieces_t = u8(n_packets * nat.OGG_PACKET_DTYPE.itemsize), u8(n_pieces * nat.PIECE_DTYPE.itemsize)
+    engine.ogg_index_dev_queue(data_t, r, packets_t, pieces_t, index_t)
+    mark("index", {})
+    # 2. each file's headers and audio packets
+    heads_t, ranks_t = u8(n * nat.VORBIS_FILE_HEADS_DTYPE.itemsize), u8(n_packets * nat.VORBIS_PACKET_RANK_DTYPE.itemsize)
+    engine.vorbis_heads_dev(data_t, r, packets_t, pieces_t, index_t, heads_t, ranks_t)
+    mark("heads", {})
+    engine.sync()
+    heads = bytes_of(heads_t, nat.VORBIS_FILE_HEADS_DTYPE)
+    read += heads.nbytes
+    # 3. the header packets gathered into one buffer, read back, and checked on the host as ogg_vorbis_index checks them
+    refs, spans, at = [], {}, 0
+    for i in range(n):
+        h = heads[i]
+        if h["status"] == nat.VORBIS_NO_PACKETS:
+            continue
+        refs.append((at, i, 0))
+        spans[i] = [(at, int(h["ident_len"]))]
+        at += int(h["ident_len"])
+        if h["status"] == 0:
+            refs.append((at, i, int(h["setup"])))
+            spans[i].append((at, int(h["setup_len"])))
+            at += int(h["setup_len"])
+    head_t = u8(at)
+    engine.ogg_gather_dev(data_t, r, packets_t, pieces_t, index_t, np.array(refs, dtype=nat.OGG_PACKET_REF_DTYPE), head_t)
+    engine.sync()
+    head_bytes = head_t.cpu().numpy().tobytes()
+    read += len(head_bytes)
+    messages, opened = {}, {}
+
+    def check(ident_b, setup_b):
+        try:
+            ident, n_modes, mask, fe = vorbis_open_headers(ident_b, setup_b)
+            fe.close()   # (it checked the setup; the device call builds its own)
+            return ident, n_modes, mask
+        except Exception as e:  # noqa: BLE001 -- one bad file must not abort the batch; its message is kept
+            return f"{type(e).__name__}: {e}"
+    keys = {}
+    for i in range(n):
+        if i not in spans:
+            messages[i] = "ValueError: no Ogg packets"
+            continue
+        parts = [head_bytes[a:a + ln] for a, ln in spans[i]]
+        key = (parts[0], parts[1] if len(parts) > 1 else None)
+        if key not in opened:    # identical headers are checked once: the checks depend on nothing else
+            opened[key] = check(*key)
+        if isinstance(opened[key], str):
+            messages[i] = opened[key]
+        else:
+            keys[i] = key
+    if errors is not None:
+        errors.update(messages)
+    # setups shared by identical headers, groups and each file's share of the jobs, as vorbis_files_plan lays them out
+    groups = np.zeros(n, dtype=nat.VORBIS_GROUP_DTYPE)
+    file_jobs = np.zeros(n, dtype=nat.VORBIS_FILE_JOBS_DTYPE)
+    setup_of, setup_refs, headers, head_at, job_at, byte_at, out_at = {}, [], [], 0, 0, 0, 0
+    for i, key in keys.items():
+        ident, n_modes, mask = opened[key]
+        if key not in setup_of:
+            setup_of[key] = len(setup_refs)
+            setup_refs.append((head_at, head_at + len(key[0]), len(key[0]), len(key[1])))
+            headers += list(key)
+            head_at += len(key[0]) + len(key[1])
+        n_audio, n_bytes = int(heads[i]["n_audio"]), int(heads[i]["audio_bytes"])
+        groups[i] = (out_at, job_at, n_audio, setup_of[key], 0)
+        file_jobs[i] = (mask, byte_at, n_bytes, job_at, n_audio, n_modes, ident["bs0_exp"], ident["bs1_exp"], 0)
+        job_at, byte_at = job_at + n_audio, byte_at + n_bytes
+        out_at += n_audio * ((1 << int(ident["bs1_exp"])) >> 1) * int(ident["channels"])
+    failed = [i for i in range(n) if i not in keys]
+    groups["out_offset"][failed], groups["first_job"][failed] = out_at, job_at
+    setups = np.array(setup_refs, dtype=nat.VORBIS_SETUP_REF_DTYPE)
+    mark("setup", {})
+    # 4. every audio packet's bytes and job
+    audio_t, jobs_t = u8(byte_at), u8(job_at * nat.VORBIS_JOB_DTYPE.itemsize)
+    engine.vorbis_jobs_dev(data_t, r, packets_t, pieces_t, index_t, ranks_t, file_jobs, audio_t, jobs_t)
+    mark("jobs", dict(audio=audio_t, jobs=jobs_t, groups=groups))
+    # 5. the decode
+    out = torch.empty(out_at, dtype=getattr(torch, _TORCH_DTYPES[fmt]), device=dev)
+    status = np.zeros(0, dtype=np.uint8)
+    results = np.zeros(n, dtype=nat.VORBIS_RESULT_DTYPE)
+    if len(setups):    # (else every file failed: nothing is decoded)
+        results_t, status_t = u8(n * nat.VORBIS_RESULT_DTYPE.itemsize), u8(job_at)
+        engine.vorbis_decode_dev(b"".join(headers), setups, audio_t, jobs_t, groups, fmt, out, results_t, status_t)
+        mark("decode", {})
+        engine.sync()
+        results, status = bytes_of(results_t, nat.VORBIS_RESULT_DTYPE), status_t.cpu().numpy()
+        read += results.nbytes + status.nbytes
+    if stats is not None:
+        stats.update(status=status, n_setups=len(setups), read_back_bytes=read)
+    return _per_file(out, groups, failed, lambda g: (int(results[g]["frames"]), int(results[g]["channels"]), int(results[g]["sample_rate"])))
 
 
 # ---- a mixed list: every file to the device decoder of its kind ----------------------------------------------------------------

@@ -39,6 +39,13 @@ def _dev_ptr(t):
     return ctypes.c_void_p(t.data_ptr()) if t.numel() else None
 
 
+def file_ranges(ranges):
+    """FILE_RANGE_DTYPE records, or (offset, len) pairs, as a contiguous FILE_RANGE_DTYPE array."""
+    from ._native import FILE_RANGE_DTYPE
+    return np.ascontiguousarray(np.array(ranges, dtype=np.uint64).reshape(-1, 2).view(FILE_RANGE_DTYPE).reshape(-1)
+                                if not isinstance(ranges, np.ndarray) or ranges.dtype != FILE_RANGE_DTYPE else ranges)
+
+
 class Engine:
     def __init__(self, device=0):
         self._lib = _native.lib()
@@ -403,17 +410,14 @@ class Engine:
         [first_packet, first_packet + n_packets) and pieces likewise, equal packetizer.ogg_index of its bytes.  Without
         capacities the sizes are found first by a call with none (its index read back), then the tables written by a second."""
         import torch
-        from ._native import FILE_RANGE_DTYPE, OGG_FILE_INDEX_DTYPE, OGG_PACKET_DTYPE, PIECE_DTYPE
+        from ._native import OGG_FILE_INDEX_DTYPE
         assert data_t.is_cuda and data_t.is_contiguous() and data_t.dtype == torch.uint8
-        r = np.ascontiguousarray(np.array(ranges, dtype=np.uint64).reshape(-1, 2).view(FILE_RANGE_DTYPE).reshape(-1)
-                                 if not isinstance(ranges, np.ndarray) or ranges.dtype != FILE_RANGE_DTYPE else ranges)
+        r = file_ranges(ranges)
         index_t = torch.empty(len(r) * OGG_FILE_INDEX_DTYPE.itemsize, dtype=torch.uint8, device=data_t.device)
 
         def call(packets_t, pieces_t):
             torch.cuda.current_stream(data_t.device).synchronize()  # data_t and the outputs are torch's: written / allocated on its stream
-            self._check(self._lib.symgpu_ogg_index_dev(self._ctx, _dev_ptr(data_t), data_t.numel(), _host_ptr(r), len(r), _dev_ptr(packets_t),
-                                                       packets_t.numel() // OGG_PACKET_DTYPE.itemsize, _dev_ptr(pieces_t),
-                                                       pieces_t.numel() // PIECE_DTYPE.itemsize, _dev_ptr(index_t)))
+            self.ogg_index_dev_queue(data_t, r, packets_t, pieces_t, index_t)
             self.sync()
             return index_t.cpu().numpy().view(OGG_FILE_INDEX_DTYPE)
 
@@ -422,9 +426,47 @@ class Engine:
         none = torch.empty(0, dtype=torch.uint8, device=data_t.device)
         if cap_packets is None or cap_pieces is None:
             cap_packets, cap_pieces = totals(call(none, none))
-        packets_t = torch.empty(cap_packets * OGG_PACKET_DTYPE.itemsize, dtype=torch.uint8, device=data_t.device)
-        pieces_t = torch.empty(cap_pieces * PIECE_DTYPE.itemsize, dtype=torch.uint8, device=data_t.device)
+        packets_t = torch.empty(cap_packets * _native.OGG_PACKET_DTYPE.itemsize, dtype=torch.uint8, device=data_t.device)
+        pieces_t = torch.empty(cap_pieces * _native.PIECE_DTYPE.itemsize, dtype=torch.uint8, device=data_t.device)
         return packets_t, pieces_t, call(packets_t, pieces_t)
+
+    def ogg_index_dev_queue(self, data_t, ranges, packets_t, pieces_t, index_t):
+        """symgpu_ogg_index_dev on uint8 CUDA tensors (packets_t / pieces_t / index_t the bytes of their records), left queued on
+        the engine's stream: no wait for torch's stream before it, none for the engine's after it."""
+        from ._native import OGG_PACKET_DTYPE, PIECE_DTYPE
+        r = file_ranges(ranges)
+        self._check(self._lib.symgpu_ogg_index_dev(self._ctx, _dev_ptr(data_t), data_t.numel(), _host_ptr(r), len(r), _dev_ptr(packets_t),
+                                                   packets_t.numel() // OGG_PACKET_DTYPE.itemsize, _dev_ptr(pieces_t),
+                                                   pieces_t.numel() // PIECE_DTYPE.itemsize, _dev_ptr(index_t)))
+
+    # -- Vorbis jobs built on the device from the device Ogg index (uint8 CUDA tensors holding the records; queued, no wait) -----
+    def vorbis_heads_dev(self, data_t, ranges, packets_t, pieces_t, index_t, heads_t, ranks_t):
+        """symgpu_vorbis_heads_dev: per file a VORBIS_FILE_HEADS_DTYPE record in heads_t, per packet of packets_t a
+        VORBIS_PACKET_RANK_DTYPE record in ranks_t, from the tables ogg_index_dev_queue wrote."""
+        from ._native import OGG_PACKET_DTYPE
+        r = file_ranges(ranges)
+        self._check(self._lib.symgpu_vorbis_heads_dev(self._ctx, _dev_ptr(data_t), data_t.numel(), _host_ptr(r), len(r), _dev_ptr(packets_t),
+                                                      packets_t.numel() // OGG_PACKET_DTYPE.itemsize, _dev_ptr(pieces_t), _dev_ptr(index_t),
+                                                      _dev_ptr(heads_t), _dev_ptr(ranks_t)))
+
+    def ogg_gather_dev(self, data_t, ranges, packets_t, pieces_t, index_t, refs, out_t):
+        """symgpu_ogg_gather_dev: the packets `refs` (OGG_PACKET_REF_DTYPE, host) name copied to out_t[dst ..]."""
+        from ._native import OGG_PACKET_REF_DTYPE
+        r = file_ranges(ranges)
+        refs = np.ascontiguousarray(refs, dtype=OGG_PACKET_REF_DTYPE)
+        self._check(self._lib.symgpu_ogg_gather_dev(self._ctx, _dev_ptr(data_t), data_t.numel(), _host_ptr(r), len(r), _dev_ptr(packets_t),
+                                                    _dev_ptr(pieces_t), _dev_ptr(index_t), _host_ptr(refs), len(refs), _dev_ptr(out_t), out_t.numel()))
+
+    def vorbis_jobs_dev(self, data_t, ranges, packets_t, pieces_t, index_t, ranks_t, file_jobs, out_t, jobs_t):
+        """symgpu_vorbis_jobs_dev: every audio packet of the files whose VORBIS_FILE_JOBS_DTYPE record (host) has n_modes gathered
+        to out_t, and its VORBIS_JOB_DTYPE record written to jobs_t."""
+        from ._native import OGG_PACKET_DTYPE, VORBIS_FILE_JOBS_DTYPE, VORBIS_JOB_DTYPE
+        r = file_ranges(ranges)
+        file_jobs = np.ascontiguousarray(file_jobs, dtype=VORBIS_FILE_JOBS_DTYPE)
+        self._check(self._lib.symgpu_vorbis_jobs_dev(self._ctx, _dev_ptr(data_t), data_t.numel(), _host_ptr(r), len(r), _dev_ptr(packets_t),
+                                                     packets_t.numel() // OGG_PACKET_DTYPE.itemsize, _dev_ptr(pieces_t), _dev_ptr(index_t),
+                                                     _dev_ptr(ranks_t), _host_ptr(file_jobs), _dev_ptr(out_t), out_t.numel(), _dev_ptr(jobs_t),
+                                                     jobs_t.numel() // VORBIS_JOB_DTYPE.itemsize))
 
     # -- output stage -------------------------------------------------------------------------
     def pcm_pack_host(self, pcm, spans, channels, fmt, out_frames, plane_stride=0, frames=0, n_spans=None, out=None):
