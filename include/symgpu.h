@@ -1051,6 +1051,38 @@ symgpu_status symgpu_vorbis_jobs_dev(symgpu_ctx* ctx, const uint8_t* data, size_
                                      size_t n_jobs);
 
 /* ===================================================================================================
+ * ADTS frames indexed on the device (DESIGN 5b): many files already in device memory, one call.  The sync search, the header
+ * rules and the stops are those of symgpu_adts_index, as the same host / device code (packetizer.hpp).  Each file's frame chain
+ * is found by pointer doubling over its sync candidates, in rounds logarithmic in the longest file, not by a walk per file.
+ * ================================================================================================= */
+#define SYMGPU_ADTS_MAX_FILES 65536
+typedef struct symgpu_adts_file_index { /* 24 bytes: one file's share of the tables                                     */
+    uint64_t first_packet;   /* its packets start here in `packets` and `jobs` (the n_packets of the files before it, summed) */
+    uint32_t n_packets;
+    uint32_t sample_rate;    /* the first frame's; 0 without frames                                                      */
+    uint8_t channels;        /* the first frame's channel configuration value, as symgpu_adts_packet.channels           */
+    uint8_t profile;         /* the first frame's                                                                       */
+    uint8_t stop;            /* what symgpu_adts_index returns in *stop for these bytes (a symgpu_status)                */
+    uint8_t status;          /* SYMGPU_ADTS_NOT_WRITTEN: first_packet + n_packets passes the capacity, so none of the
+                                file's records were written                                                             */
+    uint8_t reserved[4];
+} symgpu_adts_file_index;
+enum { SYMGPU_ADTS_NOT_WRITTEN = 1 };
+/* For every file data[files[i].offset ..][.. len): what symgpu_adts_index returns for those bytes alone, its packets at
+ * packets[index[i].first_packet ..] with offsets relative to the file's first byte, and the same payloads at jobs[...] as
+ * absolute byte ranges of data (what symgpu_aac_decode_dev takes).  packets and jobs hold cap_packets records each; either may
+ * be NULL.  data, packets, jobs and index are device memory; files host memory.  SYMGPU_ERR_ARG for a range outside data[0 ..
+ * n_bytes) or a missing pointer, SYMGPU_ERR_LIMIT for more than SYMGPU_ADTS_MAX_FILES files or a file of 2^32 bytes or more;
+ * both before anything is launched.  A frame is at least 7 bytes, so a capacity of the files' lengths / 7, summed, always
+ * suffices: one call.  No file: no launch.  Otherwise 7 + K launches, K = bit_length(longest file's length / 2), whatever the
+ * number of files, and one host wait, for the 8-byte number of sync candidates, which sizes the scratch from the context's
+ * staging buffer: 24 bytes per candidate (a candidate is a 0xff byte whose next byte could start an ADTS header), 24 per file
+ * and 8 per 4 KiB of file bytes.  SYMGPU_ERR_LIMIT, after that wait, for 2^32 - 1 candidates or more.  The call returns with the
+ * rest queued. */
+symgpu_status symgpu_adts_index_dev(symgpu_ctx* ctx, const uint8_t* data, size_t n_bytes, const symgpu_file_range* files, size_t n_files,
+                                    symgpu_adts_packet* packets, symgpu_piece* jobs, size_t cap_packets, symgpu_adts_file_index* index);
+
+/* ===================================================================================================
  * MPEG Layer I / II sample decoders (SURVEY 8f N1 for the Layer I / II path): a packet becomes the sub-band samples
  * symgpu_mpa12_synth_* take.  CPU only, stateless apart from the stream's signal specification.
  *   Layer1::decode up to the synthesis call   symphonia-bundle-mp3/src/layer1/mod.rs:19-176

@@ -10,9 +10,9 @@
 // skipped as junk, which frames are tags, how packets continue across pages, where the time stamps and trims come
 // from) are the reference's, cited at each function, and are checked bit for bit against oracle/packetizer_oracle.py.
 //
-// Header-only C++17, no dependencies.  The MPEG frame-header functions are also device functions when the header is compiled by
-// nvcc (SYMGPU_PACKET_HD), so the Layer I / II device decoder parses headers with this very code; C++ compilers see plain inline
-// functions.
+// Header-only C++17, no dependencies.  The MPEG and ADTS frame-header functions are also device functions when the header is
+// compiled by nvcc (SYMGPU_PACKET_HD), so the Layer I / II device decoder and the device ADTS index parse headers with this very
+// code; C++ compilers see plain inline functions.
 #pragma once
 #include <algorithm>
 #include <cstddef>
@@ -47,7 +47,7 @@ struct Piece {
 namespace detail {
 SYMGPU_PACKET_HD inline uint32_t be32(const uint8_t* p) { return uint32_t(p[0]) << 24 | uint32_t(p[1]) << 16 | uint32_t(p[2]) << 8 | p[3]; }
 inline uint32_t be24(const uint8_t* p) { return uint32_t(p[0]) << 16 | uint32_t(p[1]) << 8 | p[2]; }
-inline uint32_t be16(const uint8_t* p) { return uint32_t(p[0]) << 8 | p[1]; }
+SYMGPU_PACKET_HD inline uint32_t be16(const uint8_t* p) { return uint32_t(p[0]) << 8 | p[1]; }
 SYMGPU_PACKET_HD inline uint32_t le32(const uint8_t* p) { return uint32_t(p[3]) << 24 | uint32_t(p[2]) << 16 | uint32_t(p[1]) << 8 | p[0]; }
 SYMGPU_PACKET_HD inline uint64_t le64(const uint8_t* p) { return uint64_t(le32(p + 4)) << 32 | le32(p); }
 
@@ -482,14 +482,14 @@ struct AdtsHeader {
     uint16_t crc;
     uint16_t frame_len;    // sync word, header and payload
     uint32_t sample_rate;
-    uint32_t payload_len() const { return uint32_t(frame_len) - header_len; }
+    SYMGPU_PACKET_HD uint32_t payload_len() const { return uint32_t(frame_len) - header_len; }
 };
 
 // adts.rs:202-204: 0xfff, layer bits zero; the MPEG-2/4 bit and the protection bit are free.
-inline bool adts_is_sync(uint32_t w16) { return (w16 & 0xfff6u) == 0xfff0u; }
+SYMGPU_PACKET_HD inline bool adts_is_sync(uint32_t w16) { return (w16 & 0xfff6u) == 0xfff0u; }
 
 // adts.rs:137-198.  `p` points at the sync word; `n` bytes are readable.  EndOfStream: fewer than header_len bytes.
-inline Status adts_parse_header(const uint8_t* p, size_t n, AdtsHeader& h) {
+SYMGPU_PACKET_HD inline Status adts_parse_header(const uint8_t* p, size_t n, AdtsHeader& h) {
     static constexpr uint32_t rates[13] = {96000, 88200, 64000, 48000, 44100, 32000, 24000, 22050, 16000, 12000, 11025, 8000, 7350};
     static constexpr uint8_t chans[8] = {0, 1, 2, 3, 4, 5, 6, 8};
     if (n < 2) return Status::EndOfStream;
@@ -566,6 +566,87 @@ class AdtsIndexer {
     int64_t ts_ = 0;
     bool truncated_ = false;
 };
+
+// ---- the schedule of the device index (symgpu_adts_index_dev), step by step over the files of a call ----------------------------
+// The files lie back to back, in call order, in one virtual byte space, so the candidates of every file sorted by virtual
+// position are each file's candidates in turn.  A candidate is named by its 32-bit index in that order.
+//
+// 1. A candidate: a place where AdtsIndexer::next ends its search for sync.  Its second byte is never 0xff, so two candidates are
+//    never adjacent and a file of n bytes holds at most n / 2.
+SYMGPU_PACKET_HD inline bool adts_is_candidate(const uint8_t* d, size_t n, size_t q) {
+    return q + 2 <= n && d[q] == 0xff && adts_is_sync(detail::be16(d + q));
+}
+
+// 2. A candidate's node word, what AdtsIndexer::next does there.  Bits 0-2, the kind: a Frame, whose payload lies in the file, or a
+//    Stop, numbered as the stop symgpu_adts_index reports (0 a cut header, a clean end; 1 / 2 a bad header, decode error /
+//    unsupported; 3 a payload past the file's end).  Bit 3 (kAdtsLast): set in step 3 when the node has no successor.  Bits 4-16:
+//    a Frame's frame length.
+enum : uint32_t { kAdtsStopOk = 0, kAdtsStopDecode = 1, kAdtsStopUnsupported = 2, kAdtsStopLimit = 3, kAdtsFrame = 4, kAdtsLast = 8 };
+constexpr uint32_t kAdtsEnd = 0xffffffffu;       // no successor
+constexpr uint32_t kAdtsUnranked = 0xffffffffu;  // not (yet) known to be on its file's chain
+
+SYMGPU_PACKET_HD inline uint32_t adts_node(const uint8_t* d, size_t n, size_t q) {
+    AdtsHeader h;
+    const Status s = adts_parse_header(d + q, n - q, h);
+    if (s == Status::EndOfStream) return kAdtsStopOk;
+    if (s != Status::Ok) return s == Status::DecodeError ? kAdtsStopDecode : kAdtsStopUnsupported;
+    if (q + h.frame_len > n) return kAdtsStopLimit;
+    return uint32_t(h.frame_len) << 4 | kAdtsFrame;
+}
+
+// 3. A node's successor: for candidate c, a Frame, the first candidate at or after the frame's end when it lies before file_end
+//    (the virtual end of c's file); else, and for a Stop, kAdtsEnd.  vpos: the n_cand candidates' virtual positions, ascending.
+SYMGPU_PACKET_HD inline uint32_t adts_successor(const uint64_t* vpos, uint32_t n_cand, uint32_t c, uint32_t node, uint64_t file_end) {
+    if ((node & 7) != kAdtsFrame) return kAdtsEnd;
+    const uint64_t target = vpos[c] + (node >> 4);
+    uint32_t lo = c + 1, hi = n_cand;  // the first index of [lo, hi) at or after target
+    while (lo < hi) {
+        const uint32_t mid = lo + (hi - lo) / 2;
+        if (vpos[mid] < target) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo < n_cand && vpos[lo] < file_end ? lo : kAdtsEnd;
+}
+
+// 4. The chain of a file starts at its first candidate, rank 0: candidate c is one when the one before it lies before file_begin
+//    (the virtual start of c's file).  Every other candidate starts unranked.
+SYMGPU_PACKET_HD inline uint32_t adts_initial_rank(const uint64_t* vpos, uint32_t c, uint64_t file_begin) {
+    return c == 0 || vpos[c - 1] < file_begin ? 0 : kAdtsUnranked;
+}
+
+// 5. Doubling round k at candidate c: jump = J_k (J_0: the successors), next = J_(k+1) = J_k o J_k, and a chain node ranked below
+//    2^k ranks the node J_k leads to as its rank + 2^k.  After round k exactly the chain nodes of rank below 2^(k+1) are ranked.
+//    The candidates may run in any order: J_k is injective on the chain, so no two writes meet, and a node ranked in round k had no
+//    rank before it and gets one of at least 2^k, so its own test fails whether it reads the old rank or the new one.
+SYMGPU_PACKET_HD inline void adts_double(uint32_t* rank, const uint32_t* jump, uint32_t* next, uint32_t c, uint32_t k) {
+    const uint32_t j = jump[c], r = rank[c];
+    next[c] = j == kAdtsEnd ? kAdtsEnd : jump[j];
+    if (j != kAdtsEnd && r < (1u << k)) rank[j] = r + (1u << k);
+}
+
+// The rounds that rank every chain of files of at most max_len bytes: a chain has at most max_len / 2 nodes.
+SYMGPU_PACKET_HD inline uint32_t adts_rounds(uint64_t max_len) {
+    uint32_t k = 0;
+    for (uint64_t m = max_len / 2; m; m >>= 1) ++k;
+    return k;
+}
+
+// 6. The file's record from its chain's last node (ranked, kAdtsLast): its packets are the chain's Frames, and the stop is the
+//    last node's kind, or a clean end after a Frame.
+SYMGPU_PACKET_HD inline void adts_file_end(uint32_t node, uint32_t rank, uint32_t* n_packets, uint32_t* stop) {
+    const bool frame = (node & 7) == kAdtsFrame;
+    *n_packets = rank + (frame ? 1u : 0u), *stop = frame ? kAdtsStopOk : node & 7;
+}
+
+// 7. The packet of the chain's Frame of rank `rank` at q of a file of n bytes, as AdtsIndexer::next gives it.
+SYMGPU_PACKET_HD inline AdtsPacket adts_frame_packet(const uint8_t* d, size_t n, size_t q, uint32_t rank) {
+    AdtsHeader h{};
+    adts_parse_header(d + q, n - q, h);
+    AdtsPacket p{};
+    p.offset = q + h.header_len, p.size = h.payload_len(), p.pts = int64_t(rank) * 1024;
+    p.sample_rate = h.sample_rate, p.channels = h.channels, p.profile = h.profile;
+    return p;
+}
 
 // =====================================================================================================================
 // Ogg

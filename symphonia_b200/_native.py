@@ -138,6 +138,12 @@ OGG_FILE_INDEX_DTYPE = np.dtype([("first_packet", "<u8"), ("first_piece", "<u8")
 assert FILE_RANGE_DTYPE.itemsize == 16 and OGG_FILE_INDEX_DTYPE.itemsize == 40
 OGG_MAX_FILES = 65536
 OGG_CAP_HIT, OGG_NOT_WRITTEN = 1, 2
+# ADTS frames indexed on the device: `symgpu_adts_file_index` (24 bytes)
+ADTS_FILE_INDEX_DTYPE = np.dtype([("first_packet", "<u8"), ("n_packets", "<u4"), ("sample_rate", "<u4"), ("channels", "u1"), ("profile", "u1"),
+                                  ("stop", "u1"), ("status", "u1"), ("reserved", "u1", (4,))])
+assert ADTS_FILE_INDEX_DTYPE.itemsize == 24
+ADTS_MAX_FILES = 65536
+ADTS_NOT_WRITTEN = 1
 # Vorbis jobs built on the device: `symgpu_vorbis_file_heads` (32 bytes), `symgpu_vorbis_packet_rank` (24),
 # `symgpu_ogg_packet_ref` (16), `symgpu_vorbis_file_jobs` (40)
 VORBIS_FILE_HEADS_DTYPE = np.dtype([("audio_bytes", "<u8"), ("n_stream", "<u4"), ("ident_len", "<u4"), ("setup", "<u4"), ("setup_len", "<u4"),
@@ -336,6 +342,8 @@ def lib():
     L.symgpu_vorbis_fe_config.argtypes = [vp, vp, vp, ctypes.POINTER(u32)]
     L.symgpu_vorbis_fe_decode.restype = ctypes.c_int
     L.symgpu_vorbis_fe_decode.argtypes = [vp, vp, sz, u32, u32, vp, vp, vp]
+    L.symgpu_adts_index_dev.restype = ctypes.c_int
+    L.symgpu_adts_index_dev.argtypes = [vp, vp, sz, vp, sz, vp, vp, sz, vp]
     L.symgpu_ogg_index_dev.restype = ctypes.c_int
     L.symgpu_ogg_index_dev.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, sz, vp]
     L.symgpu_vorbis_heads_dev.restype = ctypes.c_int

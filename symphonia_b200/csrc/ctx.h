@@ -149,4 +149,23 @@ inline symgpu_status ensure_stage(symgpu_ctx* ctx, size_t need) {
     return SYMGPU_OK;
 }
 
+// ensure_stage for a call that has already written the first `keep` bytes of the buffer: a larger buffer starts with a copy of them.
+inline symgpu_status ensure_stage_keep(symgpu_ctx* ctx, size_t need, size_t keep) {
+    if (need <= ctx->stage_cap) return SYMGPU_OK;
+    cudaError_t e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) return cuda_fail(ctx, e, "cudaStreamSynchronize");
+    void* grown = nullptr;
+    e = cudaMalloc(&grown, need);
+    if (e != cudaSuccess) return cuda_fail(ctx, e, "cudaMalloc(stage)");
+    if (keep) e = cudaMemcpy(grown, ctx->d_stage, keep, cudaMemcpyDeviceToDevice);
+    if (e != cudaSuccess) {
+        cudaFree(grown);
+        return cuda_fail(ctx, e, "cudaMemcpy(stage)");
+    }
+    cudaFree(ctx->d_stage);
+    ctx->d_stage = grown;
+    ctx->stage_cap = need;
+    return SYMGPU_OK;
+}
+
 } // namespace symgpu_detail

@@ -5,13 +5,14 @@
 //   2. ogg_chain_kernel, one thread per file: the chain of pages that verify (ogg_next_page), then those pages ordered by serial
 //      (ogg_sort_by_serial);
 //   3. ogg_walk_kernel<false>, one thread per file: the logical streams (ogg_walk_streams), packets and pieces counted;
-//   4. ogg_file_scan_kernel, one block: each file's first packet and first piece;
+//   4. exclusive_scan_kernel (block_scan.cuh), one block: each file's first packet and first piece;
 //   5. ogg_walk_kernel<true>: the same walk, writing the tables of every file that fits the capacities.
 // Each per-file step is linear in the file's words and pages.
 #include <cuda_runtime.h>
 
 #include "../../include/symgpu/packetizer.hpp"
 #include "batch_call.h"
+#include "block_scan.cuh"
 
 namespace {
 
@@ -120,41 +121,12 @@ __global__ void ogg_walk_kernel(const uint8_t* __restrict__ data, const FileDev*
     }
 }
 
-// Inclusive sum over a warp.
-__device__ inline uint64_t warp_sum(uint64_t v) {
-    const uint32_t lane = threadIdx.x & 31;
-    for (int o = 1; o < 32; o *= 2) {
-        const uint64_t u = __shfl_up_sync(0xffffffffu, v, o);
-        if (lane >= uint32_t(o)) v += u;
-    }
-    return v;
-}
-
-// Exclusive sums of n_packets and n_pieces over the files, in one block of 1024 threads.
-__global__ void __launch_bounds__(1024) ogg_file_scan_kernel(symgpu_ogg_file_index* index, uint32_t n_files) {
-    __shared__ uint64_t warp_tot[2][32];
-    __shared__ uint64_t carry[2];
-    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) carry[0] = carry[1] = 0;
-    __syncthreads();
-    for (uint32_t base = 0; base < n_files; base += 1024) {
-        const uint32_t i = base + threadIdx.x;
-        const uint64_t a = i < n_files ? index[i].n_packets : 0, b = i < n_files ? index[i].n_pieces : 0;
-        const uint64_t sa = warp_sum(a), sb = warp_sum(b);
-        if (lane == 31) warp_tot[0][warp] = sa, warp_tot[1][warp] = sb;
-        __syncthreads();
-        if (warp == 0) {
-            const uint64_t ta = warp_sum(warp_tot[0][lane]), tb = warp_sum(warp_tot[1][lane]);
-            warp_tot[0][lane] = ta, warp_tot[1][lane] = tb;  // inclusive over the warps
-        }
-        __syncthreads();
-        const uint64_t before_a = carry[0] + (warp ? warp_tot[0][warp - 1] : 0), before_b = carry[1] + (warp ? warp_tot[1][warp - 1] : 0);
-        if (i < n_files) index[i].first_packet = before_a + sa - a, index[i].first_piece = before_b + sb - b;
-        __syncthreads();
-        if (threadIdx.x == 0) carry[0] += warp_tot[0][31], carry[1] += warp_tot[1][31];
-        __syncthreads();
-    }
-}
+// Each file's first packet and first piece: exclusive sums of n_packets and n_pieces (exclusive_scan_kernel).
+struct FileFirsts {
+    static constexpr int kN = 2;
+    __device__ uint64_t get(const symgpu_ogg_file_index& r, int k) const { return k ? r.n_pieces : r.n_packets; }
+    __device__ void put(symgpu_ogg_file_index& r, int k, uint64_t before) const { (k ? r.first_piece : r.first_packet) = before; }
+};
 
 }  // namespace
 
@@ -200,7 +172,7 @@ extern "C" symgpu_status symgpu_ogg_index_dev(symgpu_ctx* ctx, const uint8_t* da
     CU(ctx, cudaGetLastError());
     ogg_walk_kernel<false><<<file_blocks, 128, 0, st>>>(data, d_files, nf, chain, packets, cap_packets, pieces, cap_pieces, index);
     CU(ctx, cudaGetLastError());
-    ogg_file_scan_kernel<<<1, 1024, 0, st>>>(index, nf);
+    exclusive_scan_kernel<<<1, 1024, 0, st>>>(index, nf, FileFirsts{});
     CU(ctx, cudaGetLastError());
     ogg_walk_kernel<true><<<file_blocks, 128, 0, st>>>(data, d_files, nf, chain, packets, cap_packets, pieces, cap_pieces, index);
     CU(ctx, cudaGetLastError());

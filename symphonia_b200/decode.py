@@ -753,6 +753,76 @@ def decode_aac_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False,
                      lambda g: (int(results[g]["frames"]), int(groups[g]["channels"]), int(groups[g]["sample_rate"])))
 
 
+def decode_aac_files_dev(engine, data_t, ranges, fmt=nat.FMT_S16, errors=None, stats=None):
+    """decode_aac_files(engine, files, fmt, device=True) for ADTS AAC-LC files already in device memory: file i is
+    data_t[offset : offset + len] of ranges[i] ((offset, len) pairs or FILE_RANGE_DTYPE records) in a uint8 CUDA tensor, and its
+    result, its message in errors[i] and `stats` (`status`, `n_redecoded`) are what decode_aac_files gives for those bytes.
+    The frames are indexed on the device (symgpu_adts_index_dev) into a job table the decode reads in place; only the per-file
+    index records, the decode's results and its per-packet status come back to the host.  stats also receives
+    `read_back_bytes`, every byte the call copies from the device.  A failed file's packets stay in the job table, named by no
+    group.  At most 65 536 files; (re)allocates the engine's AAC state slots, one per file, as decode_aac_files does."""
+    import torch
+
+    from .engine import file_ranges
+    r = file_ranges(ranges)
+    n = len(r)
+    if n > nat.ADTS_MAX_FILES:
+        raise ValueError(f"decode_aac_files_dev takes at most {nat.ADTS_MAX_FILES} files per call, not {n}")
+    if not (data_t.is_cuda and data_t.dtype == torch.uint8 and data_t.is_contiguous()):
+        raise ValueError("decode_aac_files_dev takes a contiguous uint8 CUDA tensor")
+    size = data_t.numel()
+    if ((r["offset"] > size) | (r["len"] > size - np.minimum(r["offset"], size))).any():
+        raise ValueError(f"a file range lies outside the {size} bytes of data_t")
+    if n == 0:
+        return []
+    dev = data_t.device
+
+    def u8(count):
+        return torch.empty(int(count), dtype=torch.uint8, device=dev)
+    # 1. every file's frames as jobs, the table sized by the bound (a frame is at least 7 bytes)
+    cap = int((r["len"] // 7).sum())
+    jobs_t, index_t = u8(cap * nat.PIECE_DTYPE.itemsize), u8(n * nat.ADTS_FILE_INDEX_DTYPE.itemsize)
+    torch.cuda.current_stream(dev).synchronize()   # data_t is torch's: written on its stream
+    engine.adts_index_dev_queue(data_t, r, cap, None, jobs_t, index_t)
+    engine.sync()
+    ix = index_t.cpu().numpy().view(nat.ADTS_FILE_INDEX_DTYPE)
+    read = ix.nbytes
+    # 2. the groups, as aac_files_plan lays them out, with the messages adts_aac_index raises
+    messages = {}
+    groups = np.zeros(n, dtype=nat.AAC_GROUP_DTYPE)
+    groups["slot"] = np.arange(n)
+    groups["channels"], groups["sample_rate"] = 1, 44100
+    groups["first_job"] = ix["first_packet"]
+    out_at = 0
+    for i in range(n):
+        if ix["n_packets"][i] == 0:
+            messages[i] = "ValueError: no ADTS frames"
+        elif ix["channels"][i] not in (1, 2):
+            messages[i] = "ValueError: channel configuration outside AAC-LC mono / stereo"
+        else:
+            ch, n_jobs = int(ix["channels"][i]), int(ix["n_packets"][i])
+            groups[i]["n_jobs"], groups[i]["channels"], groups[i]["sample_rate"] = n_jobs, ch, int(ix["sample_rate"][i])
+            groups[i]["out_offset"] = out_at
+            out_at += n_jobs * 1024 * ch
+    failed = sorted(messages)
+    groups["out_offset"][failed] = out_at
+    if errors is not None:
+        errors.update(messages)
+    # 3. the decode, on the job table in place
+    n_jobs = int(ix["first_packet"][-1]) + int(ix["n_packets"][-1])
+    engine.aac_streams_alloc(n)
+    out = torch.empty(out_at, dtype=getattr(torch, _TORCH_DTYPES[fmt]), device=dev)
+    results_t, status_t = u8(n * nat.AAC_RESULT_DTYPE.itemsize), u8(n_jobs)
+    redone = engine.aac_decode_dev(data_t, jobs_t[:n_jobs * nat.PIECE_DTYPE.itemsize], groups, fmt, out, results_t, status_t)
+    engine.sync()
+    results, status = results_t.cpu().numpy().view(nat.AAC_RESULT_DTYPE), status_t.cpu().numpy()
+    read += results.nbytes + status.nbytes
+    if stats is not None:
+        good = [status[int(g["first_job"]):int(g["first_job"]) + int(g["n_jobs"])] for g in groups[[i for i in range(n) if i not in messages]]]
+        stats.update(status=np.concatenate(good) if good else np.zeros(0, dtype=np.uint8), n_redecoded=redone, read_back_bytes=read)
+    return _per_file(out, groups, failed, lambda g: (int(results[g]["frames"]), int(groups[g]["channels"]), int(groups[g]["sample_rate"])))
+
+
 def decode_mpeg_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False, errors=None, stats=None):
     """[(samples [frames, channels] of `fmt`, sample_rate)] for a list of MPEG audio files of any layer, each what
     decode_mpeg_audio(engine, file, fmt) returns: every file is indexed once, Layer III files go to decode_mp3_files and Layer I / II

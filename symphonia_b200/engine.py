@@ -439,6 +439,39 @@ class Engine:
                                                    packets_t.numel() // OGG_PACKET_DTYPE.itemsize, _dev_ptr(pieces_t),
                                                    pieces_t.numel() // PIECE_DTYPE.itemsize, _dev_ptr(index_t)))
 
+    # -- ADTS frames indexed on the device ---------------------------------------------------------
+    def adts_index_dev(self, data_t, ranges, cap=None):
+        """(packets_t, jobs_t, index) for the files data_t[offset : offset + len] of `ranges` (FILE_RANGE_DTYPE records, or
+        (offset, len) pairs) in a uint8 CUDA tensor: packets_t / jobs_t the uint8 bytes of `cap` ADTS_PACKET_DTYPE / PIECE_DTYPE
+        records on the device, index the files' ADTS_FILE_INDEX_DTYPE records on the host.  File i's packets, [first_packet,
+        first_packet + n_packets), equal packetizer.adts_index of its bytes, with its stop; its jobs are the same payloads as
+        byte ranges of data_t.  cap=None: the lengths // 7, summed, which every file fits (a frame is at least 7 bytes)."""
+        import torch
+        from ._native import ADTS_FILE_INDEX_DTYPE, ADTS_PACKET_DTYPE, PIECE_DTYPE
+        assert data_t.is_cuda and data_t.is_contiguous() and data_t.dtype == torch.uint8
+        r = file_ranges(ranges)
+        if cap is None:
+            cap = int((r["len"] // 7).sum())
+        d = data_t.device
+        packets_t = torch.empty(cap * ADTS_PACKET_DTYPE.itemsize, dtype=torch.uint8, device=d)
+        jobs_t = torch.empty(cap * PIECE_DTYPE.itemsize, dtype=torch.uint8, device=d)
+        index_t = torch.empty(len(r) * ADTS_FILE_INDEX_DTYPE.itemsize, dtype=torch.uint8, device=d)
+        torch.cuda.current_stream(d).synchronize()  # data_t and the outputs are torch's: written / allocated on its stream
+        self.adts_index_dev_queue(data_t, r, cap, packets_t, jobs_t, index_t)
+        self.sync()
+        return packets_t, jobs_t, index_t.cpu().numpy().view(ADTS_FILE_INDEX_DTYPE)
+
+    def adts_index_dev_queue(self, data_t, ranges, cap, packets_t, jobs_t, index_t):
+        """symgpu_adts_index_dev on uint8 CUDA tensors (packets_t / jobs_t, either None, holding `cap` records; index_t one record
+        per file), left queued on the engine's stream after the call's one wait: no wait for torch's stream before it."""
+        from ._native import ADTS_PACKET_DTYPE, PIECE_DTYPE
+        r = file_ranges(ranges)
+        assert packets_t is None or packets_t.numel() >= cap * ADTS_PACKET_DTYPE.itemsize
+        assert jobs_t is None or jobs_t.numel() >= cap * PIECE_DTYPE.itemsize
+        self._check(self._lib.symgpu_adts_index_dev(self._ctx, _dev_ptr(data_t), data_t.numel(), _host_ptr(r), len(r),
+                                                    None if packets_t is None else _dev_ptr(packets_t),
+                                                    None if jobs_t is None else _dev_ptr(jobs_t), cap, _dev_ptr(index_t)))
+
     # -- Vorbis jobs built on the device from the device Ogg index (uint8 CUDA tensors holding the records; queued, no wait) -----
     def vorbis_heads_dev(self, data_t, ranges, packets_t, pieces_t, index_t, heads_t, ranks_t):
         """symgpu_vorbis_heads_dev: per file a VORBIS_FILE_HEADS_DTYPE record in heads_t, per packet of packets_t a
