@@ -1083,6 +1083,40 @@ symgpu_status symgpu_adts_index_dev(symgpu_ctx* ctx, const uint8_t* data, size_t
                                     symgpu_adts_packet* packets, symgpu_piece* jobs, size_t cap_packets, symgpu_adts_file_index* index);
 
 /* ===================================================================================================
+ * MPEG audio frames indexed on the device (DESIGN 5b): many files already in device memory, one call.  The frame search, the
+ * first-frame check, the Xing / Info / LAME / VBRI tags and the trims are those of symgpu_mpa_index, as the same host / device
+ * code (packetizer.hpp).  No file is walked by one thread: each file's first-frame hunt is resolved by pointer jumping and its
+ * frame chain ranked by pointer doubling, in rounds logarithmic in the longest file; the packets' indexes and time stamps are
+ * scans over the candidates.  Only the first frame's tag read and the duration estimate (at most 17 frame headers) run one
+ * thread per file.
+ * ================================================================================================= */
+#define SYMGPU_MPA_MAX_FILES 65536
+typedef struct symgpu_mpa_file_index {  /* 16 bytes: one file's share of the tables                                     */
+    uint64_t first_packet;   /* its packets start here in `packets` and `jobs` (the n_packets of the files before it, summed) */
+    uint32_t n_packets;
+    uint8_t status;          /* SYMGPU_MPA_NO_FRAME: the bytes hold no frame, what symgpu_mpa_index reports as
+                                SYMGPU_ERR_DECODE (its track is written as zeros); SYMGPU_MPA_NOT_WRITTEN: first_packet +
+                                n_packets passes the capacity, so none of the file's packets and jobs were written           */
+    uint8_t reserved[3];
+} symgpu_mpa_file_index;
+enum { SYMGPU_MPA_NO_FRAME = 1, SYMGPU_MPA_NOT_WRITTEN = 2 };
+/* For every file data[files[i].offset ..][.. len): what symgpu_mpa_index(..., seekable, ...) returns for those bytes alone --
+ * tracks[i] byte for byte, its packets at packets[index[i].first_packet ..] with offsets relative to the file's first byte, and the
+ * same frames at jobs[...] as absolute byte ranges of data with the trims saturated to 32 bits (what symgpu_mp3_decode_dev and
+ * symgpu_mpa12_decode_dev take: the two job records have one layout).  packets and jobs hold cap_packets records each; either may
+ * be NULL.  data, packets, jobs, index and tracks are device memory; files host memory.  SYMGPU_ERR_ARG for a range outside
+ * data[0 .. n_bytes) or a missing pointer, SYMGPU_ERR_LIMIT for more than SYMGPU_MPA_MAX_FILES files or a file of 2^32 bytes or
+ * more; both before anything is launched.  A frame is at least 24 bytes (MPEG-2 Layer III, 8 kbit/s, 24 kHz), so a capacity of
+ * the files' lengths / 24, summed, always suffices: one call.  No file: no launch.  Otherwise 10 + H + K launches, H =
+ * bit_length(L) and K = bit_length(L / 4) for the longest file's length L, whatever the number of files, and one host wait, for
+ * the 8-byte number of sync candidates, which sizes the scratch from the context's staging buffer: about 48 bytes per candidate
+ * (a candidate is a 0xff byte that starts a plausible header word), about 100 per file and 8 per 4 KiB of file
+ * bytes.  SYMGPU_ERR_LIMIT, after that wait, for 2^32 - 1 candidates or more.  The call returns with the rest queued. */
+symgpu_status symgpu_mpa_index_dev(symgpu_ctx* ctx, const uint8_t* data, size_t n_bytes, const symgpu_file_range* files, size_t n_files,
+                                   int seekable, symgpu_mpa_packet* packets, symgpu_mp3_job* jobs, size_t cap_packets,
+                                   symgpu_mpa_file_index* index, symgpu_mpa_track* tracks);
+
+/* ===================================================================================================
  * MPEG Layer I / II sample decoders (SURVEY 8f N1 for the Layer I / II path): a packet becomes the sub-band samples
  * symgpu_mpa12_synth_* take.  CPU only, stateless apart from the stream's signal specification.
  *   Layer1::decode up to the synthesis call   symphonia-bundle-mp3/src/layer1/mod.rs:19-176

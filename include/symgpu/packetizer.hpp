@@ -10,9 +10,9 @@
 // skipped as junk, which frames are tags, how packets continue across pages, where the time stamps and trims come
 // from) are the reference's, cited at each function, and are checked bit for bit against oracle/packetizer_oracle.py.
 //
-// Header-only C++17, no dependencies.  The MPEG and ADTS frame-header functions are also device functions when the header is
-// compiled by nvcc (SYMGPU_PACKET_HD), so the Layer I / II device decoder and the device ADTS index parse headers with this very
-// code; C++ compilers see plain inline functions.
+// Header-only C++17, no dependencies.  The MPEG and ADTS rules are also device functions when the header is compiled by nvcc
+// (SYMGPU_PACKET_HD), so the Layer I / II device decoder and the device MPEG and ADTS indexes parse headers and tags with this
+// very code; C++ compilers see plain inline functions.
 #pragma once
 #include <algorithm>
 #include <cstddef>
@@ -46,7 +46,7 @@ struct Piece {
 
 namespace detail {
 SYMGPU_PACKET_HD inline uint32_t be32(const uint8_t* p) { return uint32_t(p[0]) << 24 | uint32_t(p[1]) << 16 | uint32_t(p[2]) << 8 | p[3]; }
-inline uint32_t be24(const uint8_t* p) { return uint32_t(p[0]) << 16 | uint32_t(p[1]) << 8 | p[2]; }
+SYMGPU_PACKET_HD inline uint32_t be24(const uint8_t* p) { return uint32_t(p[0]) << 16 | uint32_t(p[1]) << 8 | p[2]; }
 SYMGPU_PACKET_HD inline uint32_t be16(const uint8_t* p) { return uint32_t(p[0]) << 8 | p[1]; }
 SYMGPU_PACKET_HD inline uint32_t le32(const uint8_t* p) { return uint32_t(p[3]) << 24 | uint32_t(p[2]) << 16 | uint32_t(p[1]) << 8 | p[0]; }
 SYMGPU_PACKET_HD inline uint64_t le64(const uint8_t* p) { return uint64_t(le32(p + 4)) << 32 | le32(p); }
@@ -73,6 +73,19 @@ struct Crc16Table {
         }
     }
 };
+// Four-character codes as the big-endian words be32 reads.
+constexpr uint32_t tag4(const char (&s)[5]) { return uint32_t(uint8_t(s[0])) << 24 | uint32_t(uint8_t(s[1])) << 16 | uint32_t(uint8_t(s[2])) << 8 | uint8_t(s[3]); }
+constexpr uint32_t kXing = tag4("Xing"), kInfo = tag4("Info"), kVbri = tag4("VBRI"), kLame = tag4("LAME"), kLavf = tag4("Lavf"), kLavc = tag4("Lavc");
+// The first candidate of vpos[lo .. n) (ascending) at or after target; n when there is none.
+SYMGPU_PACKET_HD inline uint32_t first_at_or_after(const uint64_t* vpos, uint32_t lo, uint32_t n, uint64_t target) {
+    uint32_t hi = n;
+    while (lo < hi) {
+        const uint32_t mid = lo + (hi - lo) / 2;
+        if (vpos[mid] < target) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo;
+}
 }  // namespace detail
 
 // CRC-32, polynomial 0x04c11db7, most-significant bit first, no final xor; the caller supplies the initial state
@@ -93,12 +106,16 @@ inline uint32_t crc32_update(uint32_t state, const uint8_t* p, size_t n) {
 }
 
 // CRC-16, polynomial 0x8005, least-significant bit first, no final xor (the LAME tag's checksum).
-// symphonia-core/src/checksum/crc16.rs:377-404.
-inline uint16_t crc16_ansi_le_update(uint16_t state, const uint8_t* p, size_t n) {
-    static constexpr detail::Crc16Table tab{};
-    for (size_t i = 0; i < n; ++i) state = uint16_t((state >> 8) ^ tab.t[(state ^ p[i]) & 0xff]);
+// symphonia-core/src/checksum/crc16.rs:377-404.  `t` is detail::Crc16Table::t: the device keeps its copy in constant memory.
+SYMGPU_PACKET_HD inline uint16_t crc16_ansi_le_update_with(const uint16_t* t, uint16_t state, const uint8_t* p, size_t n) {
+    for (size_t i = 0; i < n; ++i) state = uint16_t((state >> 8) ^ t[(state ^ p[i]) & 0xff]);
     return state;
 }
+inline const uint16_t* crc16_ansi_le_table() {
+    static constexpr detail::Crc16Table tab{};
+    return tab.t;
+}
+inline uint16_t crc16_ansi_le_update(uint16_t state, const uint8_t* p, size_t n) { return crc16_ansi_le_update_with(crc16_ansi_le_table(), state, p, n); }
 
 // =====================================================================================================================
 // MPEG audio (Layers I-III)
@@ -209,51 +226,52 @@ struct MpaVbriTag {
 };
 
 // demuxer.rs:942-968.  `f` = the whole frame, header word first.
-inline bool mpa_is_maybe_info_tag(const uint8_t* f, size_t n, const MpaHeader& h) {
+SYMGPU_PACKET_HD inline bool mpa_is_maybe_info_tag(const uint8_t* f, size_t n, const MpaHeader& h) {
     if (h.layer != 3) return false;
     const size_t at = 4 + h.side_info_len();
     if (n < at + 8) return false;
-    if (std::memcmp(f + at, "Xing", 4) != 0 && std::memcmp(f + at, "Info", 4) != 0) return false;
+    const uint32_t id = detail::be32(f + at);
+    if (id != detail::kXing && id != detail::kInfo) return false;
     for (size_t i = h.header_size(); i < at; ++i)
         if (f[i]) return false;
     return true;
 }
 
 // True when the frame is a tag the reference would act on; false for everything else, INCLUDING a tag whose
-// flagged fields do not fit the frame (the reference flattens that read error to "no tag").
-inline bool mpa_read_info_tag(const uint8_t* f, size_t n, const MpaHeader& h, MpaInfoTag& t) {
+// flagged fields do not fit the frame (the reference flattens that read error to "no tag").  crc16: crc16_ansi_le_table().
+SYMGPU_PACKET_HD inline bool mpa_read_info_tag_with(const uint16_t* crc16, const uint8_t* f, size_t n, const MpaHeader& h, MpaInfoTag& t) {
     if (!mpa_is_maybe_info_tag(f, n, h)) return false;
     const size_t base = 4 + h.side_info_len();
     size_t at = base;
-    auto need = [&](size_t k) { return at + k <= n; };
     t = MpaInfoTag{};
-    t.is_cbr = std::memcmp(f + at, "Info", 4) == 0;
+    t.is_cbr = detail::be32(f + at) == detail::kInfo;
     const uint32_t flags = detail::be32(f + at + 4);
     at += 8;
     if (flags & 1) {
-        if (!need(4)) return false;
+        if (at + 4 > n) return false;
         t.has_num_frames = true, t.num_frames = detail::be32(f + at), at += 4;
     }
     if (flags & 2) {
-        if (!need(4)) return false;
+        if (at + 4 > n) return false;
         t.has_num_bytes = true, t.num_bytes = detail::be32(f + at), at += 4;
     }
     if (flags & 4) {
-        if (!need(100)) return false;
+        if (at + 100 > n) return false;
         t.has_toc = true, at += 100;
     }
     if (flags & 8) {
-        if (!need(4)) return false;
+        if (at + 4 > n) return false;
         t.has_quality = true, t.quality = detail::be32(f + at), at += 4;
     }
     // LAME extension: 24 bytes up to the delay / padding field, 12 more up to its CRC-16 (over everything before it).
     if (n - at >= 24) {
         const uint8_t* e = f + at;
         MpaLameInfo li{};
-        std::memcpy(li.encoder, e, 9);
+        for (int i = 0; i < 9; ++i) li.encoder[i] = char(e[i]);
         li.peak = detail::be32(e + 11);
         const uint32_t trim = detail::be24(e + 21);
-        const bool known = !std::memcmp(e, "LAME", 4) || !std::memcmp(e, "Lavf", 4) || !std::memcmp(e, "Lavc", 4);
+        const uint32_t id = detail::be32(e);
+        const bool lame = id == detail::kLame, known = lame || id == detail::kLavf || id == detail::kLavc;
         if (known) {
             li.delay = 528 + 1 + (trim >> 12);
             const uint32_t pad = trim & 0xfff;
@@ -263,24 +281,27 @@ inline bool mpa_read_info_tag(const uint8_t* f, size_t n, const MpaHeader& h, Mp
         bool ok = true;
         if (n - at >= 12) {
             at += 10;
-            if (h.crc || !std::memcmp(e, "LAME", 4)) {
+            if (h.crc || lame) {
                 const uint32_t written = detail::be16(f + at);
-                ok = written == 0 || written == crc16_ansi_le_update(0, f, at);
+                ok = written == 0 || written == crc16_ansi_le_update_with(crc16, 0, f, at);
             }
         }
         if (ok) t.has_lame = true, t.lame = li;
     }
     return true;
 }
+inline bool mpa_read_info_tag(const uint8_t* f, size_t n, const MpaHeader& h, MpaInfoTag& t) {
+    return mpa_read_info_tag_with(crc16_ansi_le_table(), f, n, h, t);
+}
 
 // demuxer.rs:1023-1047, 980-1019.
-inline bool mpa_is_maybe_vbri_tag(const uint8_t* f, size_t n, const MpaHeader& h) {
-    if (h.layer != 3 || n < 36 + 26 || std::memcmp(f + 36, "VBRI", 4) != 0) return false;
+SYMGPU_PACKET_HD inline bool mpa_is_maybe_vbri_tag(const uint8_t* f, size_t n, const MpaHeader& h) {
+    if (h.layer != 3 || n < 36 + 26 || detail::be32(f + 36) != detail::kVbri) return false;
     for (size_t i = h.header_size(); i < 36; ++i)
         if (f[i]) return false;
     return true;
 }
-inline bool mpa_read_vbri_tag(const uint8_t* f, size_t n, const MpaHeader& h, MpaVbriTag& t) {
+SYMGPU_PACKET_HD inline bool mpa_read_vbri_tag(const uint8_t* f, size_t n, const MpaHeader& h, MpaVbriTag& t) {
     if (!mpa_is_maybe_vbri_tag(f, n, h) || detail::be16(f + 40) != 1) return false;
     t.num_bytes = detail::be32(f + 46);
     t.num_mpeg_frames = detail::be32(f + 50);
@@ -289,10 +310,74 @@ inline bool mpa_read_vbri_tag(const uint8_t* f, size_t n, const MpaHeader& h, Mp
 
 // main_data_begin of a Layer III frame: how many bytes of THIS frame's main data live in earlier frames
 // (demuxer.rs:664-680).  The bit-reservoir front end needs it per frame; -1 when the frame is too short.
-inline int mpa_main_data_begin(const uint8_t* f, size_t n, const MpaHeader& h) {
+SYMGPU_PACKET_HD inline int mpa_main_data_begin(const uint8_t* f, size_t n, const MpaHeader& h) {
     const size_t at = h.header_size();
     if (h.version == MpaVersion::Mpeg1) return at + 2 <= n ? int(detail::be16(f + at) >> 7) : -1;
     return at + 1 <= n ? int(f[at]) : -1;
+}
+
+// demuxer.rs:186-200: a frame next() drops wherever it turns up -- a Xing / Info tag when it looks like one and reads as one,
+// else a VBRI tag that reads as one.
+SYMGPU_PACKET_HD inline bool mpa_drops_tag(const uint16_t* crc16, const uint8_t* f, size_t n, const MpaHeader& h) {
+    MpaInfoTag info;
+    MpaVbriTag vbri;
+    return mpa_is_maybe_info_tag(f, n, h) ? mpa_read_info_tag_with(crc16, f, n, h, info) : mpa_read_vbri_tag(f, n, h, vbri);
+}
+
+// demuxer.rs:620-627: the word behind a first-frame candidate h looks like the same kind of stream.
+SYMGPU_PACKET_HD inline bool mpa_similar(uint32_t next, const MpaHeader& h) {
+    MpaHeader c;
+    return mpa_is_synced(next) && mpa_parse_header(next, c) == Status::Ok && c.version == h.version && c.layer == h.layer &&
+           c.sample_rate == h.sample_rate && c.n_channels() == h.n_channels();
+}
+
+namespace detail {
+// m x 2^e = n / d rounded to nearest, ties to even, with 2^52 <= m < 2^53: an IEEE double division of positive values, in integers.
+SYMGPU_PACKET_HD inline uint64_t div_rn53(unsigned __int128 n, unsigned __int128 d, int& e) {
+    auto bits = [](unsigned __int128 v) {
+        int b = 0;
+        for (; v; v >>= 1) ++b;
+        return b;
+    };
+    for (int sh = 52 - (bits(n) - bits(d));; ++sh) {
+        const unsigned __int128 num = sh >= 0 ? n << sh : n, den = sh >= 0 ? d : d << -sh;
+        uint64_t m = uint64_t(num / den);
+        if (m < (uint64_t(1) << 52)) continue;
+        const unsigned __int128 r2 = (num % den) * 2;
+        if (r2 > den || (r2 == den && (m & 1))) ++m;
+        e = -sh;
+        if (m == uint64_t(1) << 53) m >>= 1, ++e;
+        return m;
+    }
+}
+}  // namespace detail
+
+// uint64_t(double(total) / (double(len) / double(count))) for 0 < count <= len < 2^32 and total < 2^33, computed in integers: both
+// divisions correctly rounded as IEEE doubles, the quotient truncated.  The device gets the same bits without double arithmetic.
+SYMGPU_PACKET_HD inline uint64_t mpa_extrapolate(uint64_t total, uint64_t len, uint64_t count) {
+    if (total == 0) return 0;
+    int ex, ey;
+    const uint64_t mx = detail::div_rn53(len, count, ex);                                   // len / count = mx x 2^ex
+    const uint64_t my = ex <= 0 ? detail::div_rn53((unsigned __int128)(total) << -ex, mx, ey)  // total / (mx x 2^ex)
+                                : detail::div_rn53(total, (unsigned __int128)(mx) << ex, ey);
+    return ey >= 0 ? my << ey : ey <= -64 ? 0 : my >> -ey;
+}
+
+// demuxer.rs:683-733: average the first frames of d[from ..][.. n) (more than 16 of them or more than 16 KiB) and extrapolate.
+// At most 17 frames are read.
+SYMGPU_PACKET_HD inline bool mpa_estimate_frames(const uint8_t* d, size_t n, size_t from, uint64_t& frames) {
+    size_t q = from, len = 0;
+    unsigned count = 0;
+    for (;;) {
+        MpaHeader h;
+        if (q + 4 > n || mpa_parse_header(detail::be32(d + q), h) != Status::Ok) return false;
+        len += 4 + h.frame_size, ++count;
+        if (q + 4 + h.frame_size > n) return false;
+        q += 4 + h.frame_size;
+        if (count > 16 || len > 16 * 1024) break;
+    }
+    frames = mpa_extrapolate(n - from, len, count);
+    return true;
 }
 
 // One packet = one frame, a byte range of the source.
@@ -316,6 +401,139 @@ struct MpaTrack {
     uint64_t first_packet_pos;
 };
 
+// demuxer.rs:445-487: what open() learns from the accepted first frame at d[at ..] of a buffer of n bytes.  A frame that reads
+// as a Xing / Info or VBRI tag is no packet (first_packet_pos lies behind it); for any other, a seekable stream gets the estimate.
+SYMGPU_PACKET_HD inline void mpa_open_track(const uint16_t* crc16, const uint8_t* d, size_t n, size_t at, bool seekable, MpaTrack& t) {
+    const uint32_t w = detail::be32(d + at);
+    MpaHeader h{};
+    mpa_parse_header(w, h);
+    const size_t size = 4 + size_t(h.frame_size);
+    t = MpaTrack{};
+    t.first = h;
+    t.first_word = w;
+    t.tag = MpaTrack::None;
+    t.first_packet_pos = at + size;
+    MpaInfoTag info;
+    MpaVbriTag vbri;
+    if (mpa_read_info_tag_with(crc16, d + at, size, h, info)) {
+        t.tag = info.is_cbr ? MpaTrack::Info : MpaTrack::Xing;
+        if (info.has_lame) t.has_delay = true, t.delay = info.lame.delay, t.padding = info.lame.padding;
+        if (info.has_num_frames) {
+            const uint64_t total = uint64_t(info.num_frames) * h.samples_per_frame();
+            const uint64_t cut = uint64_t(t.delay) + t.padding;
+            t.has_num_frames = true, t.num_frames = total > cut ? total - cut : 0;
+        }
+    } else if (mpa_read_vbri_tag(d + at, size, h, vbri)) {
+        t.tag = MpaTrack::Vbri;
+        t.has_num_frames = true, t.num_frames = uint64_t(vbri.num_mpeg_frames) * h.samples_per_frame();
+    } else {
+        t.first_packet_pos = at;  // an ordinary frame: it is the first packet
+        uint64_t frames;
+        if (seekable && mpa_estimate_frames(d, n, at, frames)) t.has_num_frames = true, t.num_frames = frames * h.samples_per_frame();
+    }
+}
+
+// demuxer.rs:201-218: the packet of a kept frame with header word w at `at`, ts = the samples of the packets before it - delay.
+SYMGPU_PACKET_HD inline MpaPacket mpa_frame_packet(uint32_t w, uint64_t at, int64_t ts, const MpaTrack& t) {
+    MpaHeader h{};
+    mpa_parse_header(w, h);
+    const uint32_t dur = h.samples_per_frame();
+    MpaPacket p;
+    p.offset = at, p.size = 4 + h.frame_size, p.header = w, p.pts = ts, p.dur = dur;
+    p.trim_start = ts < 0 ? uint32_t(-ts < int64_t(dur) ? -ts : int64_t(dur)) : 0u;
+    p.trim_end = 0;
+    if (t.has_num_frames) {
+        const int64_t over = ts + int64_t(dur) - int64_t(t.num_frames);
+        if (over > 0) p.trim_end = uint64_t(over);
+    }
+    return p;
+}
+
+// ---- the frame search, step by step: shared by MpaIndexer and the device index (symgpu_mpa_index_dev) ------------------------
+// 1. A candidate: where the frame search stops to look at a word -- the sync bits and the plausibility test (header.rs:77-103).
+//    Candidates may be adjacent (FF FF E...), so a buffer of n bytes holds at most n - 3.
+SYMGPU_PACKET_HD inline bool mpa_is_candidate(const uint8_t* d, size_t n, size_t q) {
+    if (q + 4 > n || d[q] != 0xff) return false;
+    const uint32_t w = detail::be32(d + q);
+    return mpa_is_synced(w) && mpa_check_header(w);
+}
+
+// 2. A candidate's node word, what the search does there.  Bits 0-1, the kind: a Skip (the full parse fails: the search goes on
+//    4 bytes later), a Stop (the frame runs past the buffer: the search ends) or a Frame.  Bits 3 on: a Frame's size, header
+//    word included.
+enum : uint32_t { kMpaSkip = 0, kMpaStop = 1, kMpaFrame = 2 };
+constexpr uint32_t kMpaEnd = 0xffffffffu;  // no such candidate
+SYMGPU_PACKET_HD inline uint32_t mpa_node(const uint8_t* d, size_t n, size_t q) {
+    MpaHeader h;
+    if (mpa_parse_header(detail::be32(d + q), h) != Status::Ok) return kMpaSkip;
+    const size_t size = 4 + size_t(h.frame_size);
+    return q + size > n ? kMpaStop : uint32_t(size) << 3 | kMpaFrame;
+}
+SYMGPU_PACKET_HD inline uint32_t mpa_node_kind(uint32_t node) { return node & 3; }
+SYMGPU_PACKET_HD inline uint32_t mpa_node_size(uint32_t node) { return node >> 3; }
+
+// The smallest frame a header can express, header word included (MPEG-2 Layer III, 8 kbit/s, 24 kHz: 72 x 8000 / 24000).  A
+// file's frames do not overlap, so a buffer of n bytes holds at most n / kMpaMinFrameSize packets.
+constexpr uint32_t kMpaMinFrameSize = 24;
+
+// 3. open() rejects a Frame as the first frame when the word behind it exists but does not look like the same stream
+//    (demuxer.rs:610-640); the hunt then restarts one byte on.
+SYMGPU_PACKET_HD inline bool mpa_first_rejected(const uint8_t* d, size_t n, size_t q, uint32_t node) {
+    if (mpa_node_kind(node) != kMpaFrame) return false;
+    const size_t size = mpa_node_size(node);
+    MpaHeader h;
+    mpa_parse_header(detail::be32(d + q), h);
+    return q + size + 4 <= n && !mpa_similar(detail::be32(d + q + size), h);
+}
+
+// The candidates of the files of a device call lie in one virtual byte space, named by their index in ascending virtual position
+// (vpos); file_end is the virtual end of candidate c's file.
+// 4. S(c), the packet successor: the candidate the search visits after c -- for a Frame the first at or after its end, for a
+//    Skip the first at or after c + 4; none (kMpaEnd) for a Stop or when that lies past the file.
+SYMGPU_PACKET_HD inline uint32_t mpa_successor(const uint64_t* vpos, uint32_t n_cand, uint32_t c, uint32_t node, uint64_t file_end) {
+    const uint32_t kind = mpa_node_kind(node);
+    if (kind == kMpaStop) return kMpaEnd;
+    const uint32_t s = detail::first_at_or_after(vpos, c + 1, n_cand, vpos[c] + (kind == kMpaFrame ? mpa_node_size(node) : 4));
+    return s < n_cand && vpos[s] < file_end ? s : kMpaEnd;
+}
+
+// 5. G(c), the first-frame hunt: S(c) for a Skip, c + 1 (when in the file) for a rejected Frame, and c itself for a root -- a
+//    Stop or an accepted Frame.  The file's first frame is the root G leads to from its first candidate, when that is a Frame.
+SYMGPU_PACKET_HD inline uint32_t mpa_hunt(const uint64_t* vpos, uint32_t n_cand, uint32_t c, uint32_t node, bool rejected, uint32_t succ,
+                                          uint64_t file_end) {
+    if (mpa_node_kind(node) == kMpaSkip) return succ;
+    if (!rejected) return c;
+    return c + 1 < n_cand && vpos[c + 1] < file_end ? c + 1 : kMpaEnd;
+}
+
+// 6. Jumping round at c: next = G o G.  After k rounds hunt[c] = G^(2^k)(c); roots are fixed points, kMpaEnd absorbs.
+SYMGPU_PACKET_HD inline void mpa_hunt_jump(const uint32_t* hunt, uint32_t* next, uint32_t c) {
+    const uint32_t g = hunt[c];
+    next[c] = g == kMpaEnd ? kMpaEnd : hunt[g];
+}
+
+// The jumping rounds that bring every hunt of files of at most max_len bytes to its end: G rises by at least one candidate a step.
+SYMGPU_PACKET_HD inline uint32_t mpa_hunt_rounds(uint64_t max_len) {
+    uint32_t k = 0;
+    for (uint64_t m = max_len; m; m >>= 1) ++k;
+    return k;
+}
+
+// 7. The packets are the Frames on the S-chain from the first frame, ranked from it by adts_double over S; S moves at least 4
+//    bytes, so a chain has at most max_len / 4 nodes and these rounds rank them all.
+SYMGPU_PACKET_HD inline uint32_t mpa_chain_rounds(uint64_t max_len) { return mpa_hunt_rounds(max_len / 4); }
+
+// 8. The samples of the packet candidate c at d[q ..] of a file of n bytes gives, 0 when it gives none: c must be a chain Frame
+//    (rank: its rank on the chain, kAdtsUnranked off it) that next() keeps; the first frame (rank 0) is left out when open() read
+//    it as a tag (first_tag).
+SYMGPU_PACKET_HD inline uint32_t mpa_packet_dur(const uint16_t* crc16, const uint8_t* d, size_t q, uint32_t node, uint32_t rank, uint8_t first_tag) {
+    if (rank == 0xffffffffu /* kAdtsUnranked */ || mpa_node_kind(node) != kMpaFrame) return 0;
+    MpaHeader h;
+    mpa_parse_header(detail::be32(d + q), h);
+    if (rank == 0 ? first_tag != MpaTrack::None : mpa_drops_tag(crc16, d + q, mpa_node_size(node), h)) return 0;
+    return h.samples_per_frame();
+}
+
 // The reference's MpaReader over a resident buffer: open() = try_new, next() = next_packet.
 class MpaIndexer {
   public:
@@ -324,50 +542,17 @@ class MpaIndexer {
     // demuxer.rs:414-487.  EndOfStream: the buffer holds no frame.  `seekable` = the reference's is_seekable():
     // without it no duration is estimated for an untagged stream and nothing is trimmed from its end.
     Status open(bool seekable = true) {
-        size_t at = 0, size = 0;
-        MpaHeader h;
-        uint32_t w;
+        size_t at = 0;
+        uint32_t node;
         // demuxer.rs:610-640: accept a first frame only when the next word looks like the same kind of stream;
         // rejected candidates restart the hunt one byte further.
         for (size_t from = 0;;) {
-            if (!find_frame(from, at, w, h)) return Status::EndOfStream;
-            size = 4 + size_t(h.frame_size);
-            if (at + size + 4 <= n_) {
-                const uint32_t nxt = detail::be32(d_ + at + size);
-                MpaHeader c;
-                const bool similar = mpa_is_synced(nxt) && mpa_parse_header(nxt, c) == Status::Ok && c.version == h.version &&
-                                     c.layer == h.layer && c.sample_rate == h.sample_rate && c.n_channels() == h.n_channels();
-                if (!similar) {
-                    from = at + 1;
-                    continue;
-                }
-            }
-            break;
+            if (!find_frame(from, at, node)) return Status::EndOfStream;
+            if (!mpa_first_rejected(d_, n_, at, node)) break;
+            from = at + 1;
         }
-        track_ = MpaTrack{};
-        track_.first = h;
-        track_.first_word = w;
-        track_.tag = MpaTrack::None;
-        pos_ = at + size;
-        MpaInfoTag info;
-        MpaVbriTag vbri;
-        if (mpa_read_info_tag(d_ + at, size, h, info)) {
-            track_.tag = info.is_cbr ? MpaTrack::Info : MpaTrack::Xing;
-            if (info.has_lame) track_.has_delay = true, track_.delay = info.lame.delay, track_.padding = info.lame.padding;
-            if (info.has_num_frames) {
-                const uint64_t total = uint64_t(info.num_frames) * h.samples_per_frame();
-                const uint64_t cut = uint64_t(track_.delay) + track_.padding;
-                track_.has_num_frames = true, track_.num_frames = total > cut ? total - cut : 0;
-            }
-        } else if (mpa_read_vbri_tag(d_ + at, size, h, vbri)) {
-            track_.tag = MpaTrack::Vbri;
-            track_.has_num_frames = true, track_.num_frames = uint64_t(vbri.num_mpeg_frames) * h.samples_per_frame();
-        } else {
-            pos_ = at;  // an ordinary frame: it is the first packet
-            uint64_t frames;
-            if (seekable && estimate_frames(at, frames)) track_.has_num_frames = true, track_.num_frames = frames * h.samples_per_frame();
-        }
-        track_.first_packet_pos = pos_;
+        mpa_open_track(crc16_ansi_le_table(), d_, n_, at, seekable, track_);
+        pos_ = track_.first_packet_pos;
         ts_ = -int64_t(track_.delay);
         open_ = true;
         return Status::Ok;
@@ -380,27 +565,16 @@ class MpaIndexer {
         if (!open_) return Status::DecodeError;
         for (;;) {
             size_t at;
-            MpaHeader h;
-            uint32_t w;
-            if (!find_frame(pos_, at, w, h)) return Status::EndOfStream;
-            const size_t size = 4 + size_t(h.frame_size);
+            uint32_t node;
+            if (!find_frame(pos_, at, node)) return Status::EndOfStream;
+            const size_t size = mpa_node_size(node);
             pos_ = at + size;
-            MpaInfoTag info;
-            MpaVbriTag vbri;
-            if (mpa_is_maybe_info_tag(d_ + at, size, h)) {
-                if (mpa_read_info_tag(d_ + at, size, h, info)) continue;
-            } else if (mpa_read_vbri_tag(d_ + at, size, h, vbri)) {
-                continue;
-            }
-            const uint32_t dur = h.samples_per_frame();
-            p.offset = at, p.size = uint32_t(size), p.header = w, p.pts = ts_, p.dur = dur;
-            p.trim_start = ts_ < 0 ? uint32_t(-ts_ < int64_t(dur) ? -ts_ : int64_t(dur)) : 0u;
-            p.trim_end = 0;
-            if (track_.has_num_frames) {
-                const int64_t over = ts_ + int64_t(dur) - int64_t(track_.num_frames);
-                if (over > 0) p.trim_end = uint64_t(over);
-            }
-            ts_ += dur;
+            const uint32_t w = detail::be32(d_ + at);
+            MpaHeader h;
+            mpa_parse_header(w, h);
+            if (mpa_drops_tag(crc16_ansi_le_table(), d_ + at, size, h)) continue;
+            p = mpa_frame_packet(w, at, ts_, track_);
+            ts_ += p.dur;
             return Status::Ok;
         }
     }
@@ -417,10 +591,9 @@ class MpaIndexer {
     }
 
   private:
-    // header.rs:77-103 + demuxer.rs:585-607 as a window search: the first offset >= from whose word has the sync
-    // bits and passes the plausibility test; a word that then fails the full parse (free format, a forbidden Layer II
-    // combination) costs its 4 bytes, and a frame whose body runs past the buffer ends the stream.
-    bool find_frame(size_t from, size_t& at, uint32_t& w, MpaHeader& h) const {
+    // header.rs:77-103 + demuxer.rs:585-607 as a window search: the first candidate at or after `from`; a Skip costs its 4
+    // bytes, a Stop ends the stream, a Frame is returned with its node word.
+    bool find_frame(size_t from, size_t& at, uint32_t& node) const {
         for (size_t q = from; q + 4 <= n_;) {
             // cheap reject on the first byte keeps the scan at memchr speed through payload bytes
             if (d_[q] != 0xff) {
@@ -429,37 +602,20 @@ class MpaIndexer {
                 q = size_t(static_cast<const uint8_t*>(hit) - d_);
                 if (q + 4 > n_) return false;
             }
-            const uint32_t word = detail::be32(d_ + q);
-            if (!mpa_is_synced(word) || !mpa_check_header(word)) {
+            if (!mpa_is_candidate(d_, n_, q)) {
                 ++q;
                 continue;
             }
-            if (mpa_parse_header(word, h) != Status::Ok) {
+            node = mpa_node(d_, n_, q);
+            if (mpa_node_kind(node) == kMpaSkip) {
                 q += 4;
                 continue;
             }
-            if (q + 4 + size_t(h.frame_size) > n_) return false;
-            at = q, w = word;
+            if (mpa_node_kind(node) == kMpaStop) return false;
+            at = q;
             return true;
         }
         return false;
-    }
-
-    // demuxer.rs:683-733: average the first frames (more than 16 of them or more than 16 KiB) and extrapolate.
-    bool estimate_frames(size_t from, uint64_t& frames) const {
-        const double total_len = double(n_ - from);
-        size_t q = from, len = 0;
-        unsigned count = 0;
-        for (;;) {
-            MpaHeader h;
-            if (q + 4 > n_ || mpa_parse_header(detail::be32(d_ + q), h) != Status::Ok) return false;
-            len += 4 + h.frame_size, ++count;
-            if (q + 4 + h.frame_size > n_) return false;
-            q += 4 + h.frame_size;
-            if (count > 16 || len > 16 * 1024) break;
-        }
-        frames = uint64_t(total_len / (double(len) / double(count)));
-        return true;
     }
 
     const uint8_t* d_;
@@ -598,13 +754,7 @@ SYMGPU_PACKET_HD inline uint32_t adts_node(const uint8_t* d, size_t n, size_t q)
 //    (the virtual end of c's file); else, and for a Stop, kAdtsEnd.  vpos: the n_cand candidates' virtual positions, ascending.
 SYMGPU_PACKET_HD inline uint32_t adts_successor(const uint64_t* vpos, uint32_t n_cand, uint32_t c, uint32_t node, uint64_t file_end) {
     if ((node & 7) != kAdtsFrame) return kAdtsEnd;
-    const uint64_t target = vpos[c] + (node >> 4);
-    uint32_t lo = c + 1, hi = n_cand;  // the first index of [lo, hi) at or after target
-    while (lo < hi) {
-        const uint32_t mid = lo + (hi - lo) / 2;
-        if (vpos[mid] < target) lo = mid + 1;
-        else hi = mid;
-    }
+    const uint32_t lo = detail::first_at_or_after(vpos, c + 1, n_cand, vpos[c] + (node >> 4));
     return lo < n_cand && vpos[lo] < file_end ? lo : kAdtsEnd;
 }
 

@@ -144,6 +144,12 @@ ADTS_FILE_INDEX_DTYPE = np.dtype([("first_packet", "<u8"), ("n_packets", "<u4"),
 assert ADTS_FILE_INDEX_DTYPE.itemsize == 24
 ADTS_MAX_FILES = 65536
 ADTS_NOT_WRITTEN = 1
+# MPEG audio frames indexed on the device: `symgpu_mpa_file_index` (16 bytes); jobs are MP3_JOB_DTYPE (= MPA12_JOB_DTYPE)
+MPA_FILE_INDEX_DTYPE = np.dtype([("first_packet", "<u8"), ("n_packets", "<u4"), ("status", "u1"), ("reserved", "u1", (3,))])
+assert MPA_FILE_INDEX_DTYPE.itemsize == 16 and MP3_JOB_DTYPE == MPA12_JOB_DTYPE
+MPA_MAX_FILES = 65536
+MPA_NO_FRAME, MPA_NOT_WRITTEN = 1, 2
+MPA_MIN_FRAME = 24   # the smallest frame a header can express: the files' lengths / 24, summed, hold every packet
 # Vorbis jobs built on the device: `symgpu_vorbis_file_heads` (32 bytes), `symgpu_vorbis_packet_rank` (24),
 # `symgpu_ogg_packet_ref` (16), `symgpu_vorbis_file_jobs` (40)
 VORBIS_FILE_HEADS_DTYPE = np.dtype([("audio_bytes", "<u8"), ("n_stream", "<u4"), ("ident_len", "<u4"), ("setup", "<u4"), ("setup_len", "<u4"),
@@ -344,6 +350,8 @@ def lib():
     L.symgpu_vorbis_fe_decode.argtypes = [vp, vp, sz, u32, u32, vp, vp, vp]
     L.symgpu_adts_index_dev.restype = ctypes.c_int
     L.symgpu_adts_index_dev.argtypes = [vp, vp, sz, vp, sz, vp, vp, sz, vp]
+    L.symgpu_mpa_index_dev.restype = ctypes.c_int
+    L.symgpu_mpa_index_dev.argtypes = [vp, vp, sz, vp, sz, ctypes.c_int, vp, vp, sz, vp, vp]
     L.symgpu_ogg_index_dev.restype = ctypes.c_int
     L.symgpu_ogg_index_dev.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, sz, vp]
     L.symgpu_vorbis_heads_dev.restype = ctypes.c_int

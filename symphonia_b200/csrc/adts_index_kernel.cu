@@ -2,97 +2,34 @@
 // per-candidate step is a function of include/symgpu/packetizer.hpp that tests/cpp/adts_index_driver.cpp also runs on the CPU;
 // the header rules are the code symgpu_adts_index runs on the host.  The files' bytes form one virtual byte space, cut into
 // tiles of 4096 bytes, one block each:
-//   1. adts_count_kernel: the sync candidates of each tile;
+//   1. candidate_count_kernel (candidate_tiles.cuh): the sync candidates of each tile;
 //   2. exclusive_scan_kernel (block_scan.cuh): each tile's first candidate, and the total, which is read back (the one host wait)
 //      to size the per-candidate scratch;
-//   3. adts_candidates_kernel: each candidate's virtual position and node word (adts_node), in order;
+//   3. candidates_kernel: each candidate's virtual position and node word (adts_node), in order;
 //   4. adts_successor_kernel: successors (adts_successor) and the chain heads (adts_initial_rank);
-//   5. K x adts_double_kernel, K = adts_rounds(longest file): every chain node's rank by pointer doubling;
+//   5. K x chain_double_kernel (candidate_tiles.cuh), K = adts_rounds(longest file): every chain node's rank by pointer doubling;
 //   6. adts_record_kernel: each file's packet count and stop from its last node, its stream parameters from its first frame;
 //   7. exclusive_scan_kernel: each file's first packet, and whether its packets fit the capacity;
 //   8. adts_packet_kernel: the packets and jobs, one thread per chain Frame.
 #include <cuda_runtime.h>
 
 #include "../../include/symgpu/packetizer.hpp"
-#include "batch_call.h"
-#include "block_scan.cuh"
+#include "candidate_tiles.cuh"
 
 namespace {
 
 using namespace symgpu::packet;
-using symgpu_detail::block_exclusive_sums;
+using namespace symgpu_detail;
 
 static_assert(kAdtsStopOk == uint32_t(SYMGPU_OK) && kAdtsStopDecode == uint32_t(SYMGPU_ERR_DECODE) &&
                   kAdtsStopUnsupported == uint32_t(SYMGPU_ERR_UNSUPPORTED) && kAdtsStopLimit == uint32_t(SYMGPU_ERR_LIMIT),
               "a Stop's kind is the stop symgpu_adts_index reports");
 static_assert(sizeof(symgpu_adts_file_index) == 24, "record sizes are ABI");
 
-struct FileDev {
-    uint64_t offset, len;
-    uint64_t vbase;  // the file's first virtual byte: the lengths of the files before it
+struct AdtsRule {
+    __device__ static bool is_candidate(const uint8_t* d, size_t n, size_t q) { return adts_is_candidate(d, n, q); }
+    __device__ static uint32_t node(const uint8_t* d, size_t n, size_t q) { return adts_node(d, n, q); }
 };
-
-constexpr uint32_t kThreads = 256, kBytesPerThread = 16, kTile = kThreads * kBytesPerThread;
-constexpr unsigned kMaxBlocks = 65535 * 8;
-
-// The file that owns virtual byte v < the files' total: the last whose vbase <= v (an empty file owns no byte).
-__device__ inline uint32_t file_of(const FileDev* files, uint32_t n_files, uint64_t v) {
-    uint32_t lo = 0, hi = n_files;
-    while (hi - lo > 1) {
-        const uint32_t mid = (lo + hi) / 2;
-        if (files[mid].vbase <= v) lo = mid;
-        else hi = mid;
-    }
-    return lo;
-}
-
-// The candidates among this thread's 16 virtual bytes of the tile, in order: on(v, file, q) for each; returns their number.
-template <class On>
-__device__ inline uint32_t thread_candidates(const uint8_t* data, const FileDev* files, uint32_t n_files, uint64_t total, uint64_t tile, On&& on) {
-    const uint64_t v0 = tile * kTile + uint64_t(threadIdx.x) * kBytesPerThread;
-    if (v0 >= total) return 0;
-    const uint64_t v1 = v0 + kBytesPerThread < total ? v0 + kBytesPerThread : total;
-    uint32_t f = file_of(files, n_files, v0), count = 0;
-    for (uint64_t v = v0; v < v1; ++v) {
-        while (v >= files[f].vbase + files[f].len) ++f;
-        const FileDev& fd = files[f];
-        const uint64_t q = v - fd.vbase;
-        if (adts_is_candidate(data + fd.offset, size_t(fd.len), size_t(q))) on(v, f, q), ++count;
-    }
-    return count;
-}
-
-__global__ void __launch_bounds__(kThreads) adts_count_kernel(const uint8_t* __restrict__ data, const FileDev* __restrict__ files, uint32_t n_files,
-                                                              uint64_t total, uint64_t n_tiles, uint64_t* __restrict__ tile_count) {
-    if (blockIdx.x == 0 && threadIdx.x == 0) tile_count[n_tiles] = 0;  // scanned into the total
-    for (uint64_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
-        const uint64_t v[1] = {thread_candidates(data, files, n_files, total, t, [](uint64_t, uint32_t, uint64_t) {})};
-        uint64_t before[1], sum[1];
-        block_exclusive_sums<1>(v, before, sum);
-        if (threadIdx.x == 0) tile_count[t] = sum[0];
-    }
-}
-
-struct TileFirsts {
-    static constexpr int kN = 1;
-    __device__ uint64_t get(const uint64_t& r, int) const { return r; }
-    __device__ void put(uint64_t& r, int, uint64_t before) const { r = before; }
-};
-
-__global__ void __launch_bounds__(kThreads) adts_candidates_kernel(const uint8_t* __restrict__ data, const FileDev* __restrict__ files, uint32_t n_files,
-                                                                   uint64_t total, uint64_t n_tiles, const uint64_t* __restrict__ tile_first,
-                                                                   uint64_t* __restrict__ vpos, uint32_t* __restrict__ node) {
-    for (uint64_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
-        const uint64_t v[1] = {thread_candidates(data, files, n_files, total, t, [](uint64_t, uint32_t, uint64_t) {})};
-        uint64_t before[1], sum[1];
-        block_exclusive_sums<1>(v, before, sum);
-        uint64_t at = tile_first[t] + before[0];
-        thread_candidates(data, files, n_files, total, t, [&](uint64_t pos, uint32_t f, uint64_t q) {
-            vpos[at] = pos;
-            node[at++] = adts_node(data + files[f].offset, size_t(files[f].len), size_t(q));
-        });
-    }
-}
 
 __global__ void adts_successor_kernel(const FileDev* __restrict__ files, uint32_t n_files, const uint64_t* __restrict__ vpos, uint32_t n_cand,
                                       uint32_t* __restrict__ node, uint32_t* __restrict__ jump, uint32_t* __restrict__ rank) {
@@ -103,10 +40,6 @@ __global__ void adts_successor_kernel(const FileDev* __restrict__ files, uint32_
         if (s == kAdtsEnd) node[c] = nd | kAdtsLast;
         rank[c] = adts_initial_rank(vpos, c, f.vbase);
     }
-}
-
-__global__ void adts_double_kernel(uint32_t* rank, const uint32_t* __restrict__ jump, uint32_t* __restrict__ next, uint32_t n_cand, uint32_t k) {
-    for (uint32_t c = blockIdx.x * blockDim.x + threadIdx.x; c < n_cand; c += gridDim.x * blockDim.x) adts_double(rank, jump, next, c, k);
 }
 
 __global__ void adts_record_kernel(const uint8_t* __restrict__ data, const FileDev* __restrict__ files, uint32_t n_files, const uint64_t* __restrict__ vpos,
@@ -161,11 +94,6 @@ __global__ void adts_packet_kernel(const uint8_t* __restrict__ data, const FileD
     }
 }
 
-unsigned blocks_for(uint64_t n, uint32_t per_block) {
-    const uint64_t b = (n + per_block - 1) / per_block;
-    return unsigned(b == 0 ? 1 : b < kMaxBlocks ? b : kMaxBlocks);
-}
-
 }  // namespace
 
 using namespace symgpu_detail;
@@ -174,56 +102,38 @@ extern "C" symgpu_status symgpu_adts_index_dev(symgpu_ctx* ctx, const uint8_t* d
                                                symgpu_adts_packet* packets, symgpu_piece* jobs, size_t cap_packets, symgpu_adts_file_index* index) {
     if (!ctx || (n_bytes && !data) || (n_files && (!files || !index))) return SYMGPU_ERR_ARG;
     if (n_files > SYMGPU_ADTS_MAX_FILES) return SYMGPU_ERR_LIMIT;
-    std::vector<FileDev> dev(n_files);
-    uint64_t total = 0, longest = 0;
-    for (size_t i = 0; i < n_files; ++i) {
-        const symgpu_file_range& r = files[i];
-        if (r.offset > n_bytes || r.len > n_bytes - r.offset) return SYMGPU_ERR_ARG;
-        if (r.len >> 32) return SYMGPU_ERR_LIMIT;
-        dev[i] = FileDev{r.offset, r.len, total};
-        total += r.len;
-        longest = r.len > longest ? r.len : longest;
-    }
+    std::vector<FileDev> dev;
+    uint64_t total, longest;
+    symgpu_status e = file_layout(files, n_files, n_bytes, dev, total, longest);
+    if (e != SYMGPU_OK) return e;
     if (n_files == 0) return SYMGPU_OK;
     DeviceGuard guard(ctx->device);
     const uint32_t nf = uint32_t(n_files), rounds = adts_rounds(longest);
     const uint64_t n_tiles = (total + kTile - 1) / kTile;
     Carver c;
-    const size_t at_files = c.take(n_files * sizeof(FileDev)), at_tiles = c.take((n_tiles + 1) * sizeof(uint64_t));
+    size_t at_files, at_tiles;
+    uint64_t n_cand;
+    if ((e = count_candidates<AdtsRule>(ctx, data, dev, total, c, at_files, at_tiles, n_cand)) != SYMGPU_OK) return e;
     const size_t keep = c.at;
-    symgpu_status e = ensure_stage(ctx, keep);
-    if (e != SYMGPU_OK) return e;
     cudaStream_t st = ctx->stream;
-    FileDev* d_files = reinterpret_cast<FileDev*>(static_cast<char*>(ctx->d_stage) + at_files);
-    uint64_t* d_tiles = reinterpret_cast<uint64_t*>(static_cast<char*>(ctx->d_stage) + at_tiles);
-    // (a copy from pageable memory returns once the source is staged, so `dev` may go out of scope without a wait)
-    CU(ctx, cudaMemcpyAsync(d_files, dev.data(), n_files * sizeof(FileDev), cudaMemcpyHostToDevice, st));
-    adts_count_kernel<<<blocks_for(n_tiles, 1), kThreads, 0, st>>>(data, d_files, nf, total, n_tiles, d_tiles);
-    CU(ctx, cudaGetLastError());
-    exclusive_scan_kernel<<<1, 1024, 0, st>>>(d_tiles, n_tiles + 1, TileFirsts{});
-    CU(ctx, cudaGetLastError());
-    ctx->launches += 2;
-    uint64_t n_cand = 0;
-    CU(ctx, cudaMemcpyAsync(&n_cand, d_tiles + n_tiles, sizeof n_cand, cudaMemcpyDeviceToHost, st));
-    CU(ctx, cudaStreamSynchronize(st));
     if (n_cand >= kAdtsEnd) return SYMGPU_ERR_LIMIT;
     const size_t at_vpos = c.take(n_cand * sizeof(uint64_t)), at_node = c.take(n_cand * 4), at_rank = c.take(n_cand * 4);
     const size_t at_jump[2] = {c.take(n_cand * 4), c.take(n_cand * 4)};
     if ((e = ensure_stage_keep(ctx, c.at, keep)) != SYMGPU_OK) return e;
     char* stage = static_cast<char*>(ctx->d_stage);
-    d_files = reinterpret_cast<FileDev*>(stage + at_files);
-    d_tiles = reinterpret_cast<uint64_t*>(stage + at_tiles);
     uint64_t* vpos = reinterpret_cast<uint64_t*>(stage + at_vpos);
     uint32_t *node = reinterpret_cast<uint32_t*>(stage + at_node), *rank = reinterpret_cast<uint32_t*>(stage + at_rank);
     uint32_t* jump[2] = {reinterpret_cast<uint32_t*>(stage + at_jump[0]), reinterpret_cast<uint32_t*>(stage + at_jump[1])};
     const uint32_t nc = uint32_t(n_cand);
     const unsigned cand_blocks = blocks_for(nc, 256);
-    adts_candidates_kernel<<<blocks_for(n_tiles, 1), kThreads, 0, st>>>(data, d_files, nf, total, n_tiles, d_tiles, vpos, node);
+    FileDev* d_files = reinterpret_cast<FileDev*>(stage + at_files);
+    const uint64_t* d_tiles = reinterpret_cast<const uint64_t*>(stage + at_tiles);
+    candidates_kernel<AdtsRule><<<blocks_for(n_tiles, 1), kTileThreads, 0, st>>>(data, d_files, nf, total, n_tiles, d_tiles, vpos, node);
     CU(ctx, cudaGetLastError());
     adts_successor_kernel<<<cand_blocks, 256, 0, st>>>(d_files, nf, vpos, nc, node, jump[0], rank);
     CU(ctx, cudaGetLastError());
     for (uint32_t k = 0; k < rounds; ++k) {
-        adts_double_kernel<<<cand_blocks, 256, 0, st>>>(rank, jump[k & 1], jump[(k + 1) & 1], nc, k);
+        chain_double_kernel<<<cand_blocks, 256, 0, st>>>(rank, jump[k & 1], jump[(k + 1) & 1], nc, k);
         CU(ctx, cudaGetLastError());
     }
     CU(ctx, cudaMemsetAsync(index, 0, n_files * sizeof(symgpu_adts_file_index), st));

@@ -5,6 +5,7 @@
 
 #include "../../include/symgpu.h"
 #include "../../include/symgpu/packetizer.hpp"
+#include "mpa_records.h"
 
 using namespace symgpu::packet;
 
@@ -21,23 +22,11 @@ extern "C" symgpu_status symgpu_mpa_index(const uint8_t* data, size_t n, int see
     if ((!data && n) || !track || !n_out || (cap && !packets)) return SYMGPU_ERR_ARG;
     MpaIndexer ix(data, n);
     if (ix.open(seekable != 0) != Status::Ok) return *n_out = 0, SYMGPU_ERR_DECODE;
-    const MpaTrack& t = ix.track();
-    *track = symgpu_mpa_track{};
-    track->first_header = t.first_word, track->sample_rate = t.first.sample_rate;
-    track->version = uint8_t(t.first.version), track->layer = t.first.layer, track->channels = uint8_t(t.first.n_channels());
-    track->tag = uint8_t(t.tag), track->has_delay = t.has_delay, track->has_num_frames = t.has_num_frames;
-    track->delay = t.delay, track->padding = t.padding, track->num_frames = t.num_frames, track->first_packet_pos = t.first_packet_pos;
+    *track = symgpu_detail::mpa_track_record(ix.track());
     size_t count = 0;
     MpaPacket p;
     while (ix.next(p) == Status::Ok) {
-        if (count < cap) {
-            symgpu_mpa_packet& o = packets[count];
-            o = symgpu_mpa_packet{};
-            o.offset = p.offset, o.size = p.size, o.header = p.header, o.pts = p.pts, o.dur = p.dur, o.trim_start = p.trim_start, o.trim_end = p.trim_end;
-            MpaHeader h{};
-            mpa_parse_header(p.header, h);
-            o.main_data_begin = h.layer == 3 ? mpa_main_data_begin(data + p.offset, p.size, h) : -1;
-        }
+        if (count < cap) packets[count] = symgpu_detail::mpa_packet_record(p, data + p.offset);
         ++count;
     }
     *n_out = count;

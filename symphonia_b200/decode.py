@@ -848,6 +848,86 @@ def decode_mpeg_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False
     return result
 
 
+def decode_mpeg_files_dev(engine, data_t, ranges, fmt=nat.FMT_S16, errors=None, stats=None):
+    """decode_mpeg_files(engine, files, fmt, device=True) for MPEG audio files already in device memory: file i is
+    data_t[offset : offset + len] of ranges[i] ((offset, len) pairs or FILE_RANGE_DTYPE records) in a uint8 CUDA tensor, and its
+    result, its message in errors[i] and `stats` (`rounds` and the Layer III per-packet `status`, when there is a Layer III file)
+    are what decode_mpeg_files gives for those bytes.  The frames, tags and trims are found on the device (symgpu_mpa_index_dev)
+    into one job table that the Layer III and the Layer I / II decoders read in place, each over the span of the table between its
+    first and last file; only the per-file index records and tracks, the decodes' results and the Layer III per-packet status come
+    back to the host.  stats also receives `read_back_bytes`, every byte the call copies from the device.  At most 65 536 files;
+    (re)allocates the engine's MP3 state slots, one per file."""
+    import torch
+
+    from .engine import SymgpuError, file_ranges
+    r = file_ranges(ranges)
+    n = len(r)
+    if n > nat.MPA_MAX_FILES:
+        raise ValueError(f"decode_mpeg_files_dev takes at most {nat.MPA_MAX_FILES} files per call, not {n}")
+    if not (data_t.is_cuda and data_t.dtype == torch.uint8 and data_t.is_contiguous()):
+        raise ValueError("decode_mpeg_files_dev takes a contiguous uint8 CUDA tensor")
+    size = data_t.numel()
+    if ((r["offset"] > size) | (r["len"] > size - np.minimum(r["offset"], size))).any():
+        raise ValueError(f"a file range lies outside the {size} bytes of data_t")
+    if n == 0:
+        return []
+    dev = data_t.device
+    out_dtype = getattr(torch, _TORCH_DTYPES[fmt])
+
+    def u8(count):
+        return torch.empty(int(count), dtype=torch.uint8, device=dev)
+    # 1. every file's frames as jobs, the table sized by the bound (a frame is at least MPA_MIN_FRAME bytes)
+    cap = int((r["len"] // nat.MPA_MIN_FRAME).sum())
+    jobs_t, index_t, tracks_t = u8(cap * nat.MP3_JOB_DTYPE.itemsize), u8(n * nat.MPA_FILE_INDEX_DTYPE.itemsize), u8(n * nat.MPA_TRACK_DTYPE.itemsize)
+    torch.cuda.current_stream(dev).synchronize()   # data_t is torch's: written on its stream
+    engine.mpa_index_dev_queue(data_t, r, cap, None, jobs_t, index_t, tracks_t)
+    engine.sync()
+    ix, tracks = index_t.cpu().numpy().view(nat.MPA_FILE_INDEX_DTYPE), tracks_t.cpu().numpy().view(nat.MPA_TRACK_DTYPE)
+    read = ix.nbytes + tracks.nbytes
+    messages = {i: f"SymgpuError: {SymgpuError(1, 'symgpu_mpa_index')}" for i in range(n) if ix["status"][i] & nat.MPA_NO_FRAME}
+    if errors is not None:
+        errors.update(messages)
+    # 2. one decode per layer family, on the job table in place, with the groups decode_mp3_files / decode_mpa12_files make
+    engine.mp3_streams_alloc(n)
+    result = [(torch.empty((0, 0), dtype=out_dtype, device=dev), 0)] * n
+    families = (((3,), nat.MP3_GROUP_DTYPE, nat.MP3_RESULT_DTYPE, engine.mp3_decode_dev),
+                ((1, 2), nat.MPA12_GROUP_DTYPE, nat.MPA12_RESULT_DTYPE, engine.mpa12_decode_dev))
+    for layers, group_dtype, result_dtype, decode in families:
+        mine = [i for i in range(n) if i not in messages and int(tracks["layer"][i]) in layers]
+        if not mine:
+            continue
+        lo = int(ix["first_packet"][mine[0]])
+        hi = int(ix["first_packet"][mine[-1]]) + int(ix["n_packets"][mine[-1]])
+        groups = np.zeros(len(mine), dtype=group_dtype)
+        out_at = 0
+        for g, i in enumerate(mine):
+            t, n_jobs = tracks[i], int(ix["n_packets"][i])
+            groups[g]["slot"], groups[g]["first_job"], groups[g]["n_jobs"], groups[g]["out_offset"] = i, int(ix["first_packet"][i]) - lo, n_jobs, out_at
+            if layers == (3,):
+                granules, channels = 2 if int(t["version"]) == 0 else 1, int(t["channels"])
+                groups[g]["granules"], groups[g]["channels"] = granules, channels
+                out_at += n_jobs * granules * 576 * channels
+            else:
+                groups[g]["layer"] = int(t["layer"])
+                out_at += 2 * n_jobs * (384 if int(t["layer"]) == 1 else 1152)
+        out = torch.empty(out_at, dtype=out_dtype, device=dev)
+        results_t, status_t = u8(len(mine) * result_dtype.itemsize), u8(hi - lo)
+        rounds = decode(data_t, jobs_t[lo * nat.MP3_JOB_DTYPE.itemsize:hi * nat.MP3_JOB_DTYPE.itemsize], groups, fmt, out, results_t, status_t)
+        engine.sync()
+        results = results_t.cpu().numpy().view(result_dtype)
+        read += results.nbytes
+        if layers == (3,):
+            status = status_t.cpu().numpy()
+            read += status.nbytes
+            if stats is not None:
+                stats.update(rounds=rounds, status=np.concatenate([status[int(g["first_job"]):int(g["first_job"]) + int(g["n_jobs"])] for g in groups]))
+        for i, got in zip(mine, _per_file(out, groups, [], lambda g: _mpa_shape(results[g], tracks[mine[g]]))):
+            result[i] = got
+    if stats is not None:
+        stats["read_back_bytes"] = read
+    return result
+
+
 # ---- Ogg Vorbis, many files decoded on the device (codebooks, floors, residues in device code) --------------------------------
 
 def vorbis_files_plan(files, threads=None, errors=None):

@@ -472,6 +472,41 @@ class Engine:
                                                     None if packets_t is None else _dev_ptr(packets_t),
                                                     None if jobs_t is None else _dev_ptr(jobs_t), cap, _dev_ptr(index_t)))
 
+    # -- MPEG audio frames indexed on the device ---------------------------------------------------------
+    def mpa_index_dev(self, data_t, ranges, cap=None, seekable=True):
+        """(packets_t, jobs_t, index, tracks) for the files data_t[offset : offset + len] of `ranges` (FILE_RANGE_DTYPE records, or
+        (offset, len) pairs) in a uint8 CUDA tensor: packets_t / jobs_t the uint8 bytes of `cap` MPA_PACKET_DTYPE / MP3_JOB_DTYPE
+        records on the device, index the files' MPA_FILE_INDEX_DTYPE records and tracks their MPA_TRACK_DTYPE records on the host.
+        File i's track and packets, [first_packet, first_packet + n_packets), equal packetizer.mpa_index(bytes, seekable) (status
+        MPA_NO_FRAME where that raises); its jobs are the same frames as byte ranges of data_t.  cap=None: the lengths // 24, summed,
+        which every file fits (a frame is at least 24 bytes)."""
+        import torch
+        from ._native import MP3_JOB_DTYPE, MPA_FILE_INDEX_DTYPE, MPA_MIN_FRAME, MPA_PACKET_DTYPE, MPA_TRACK_DTYPE
+        assert data_t.is_cuda and data_t.is_contiguous() and data_t.dtype == torch.uint8
+        r = file_ranges(ranges)
+        if cap is None:
+            cap = int((r["len"] // MPA_MIN_FRAME).sum())
+        d = data_t.device
+        packets_t = torch.empty(cap * MPA_PACKET_DTYPE.itemsize, dtype=torch.uint8, device=d)
+        jobs_t = torch.empty(cap * MP3_JOB_DTYPE.itemsize, dtype=torch.uint8, device=d)
+        index_t = torch.empty(len(r) * MPA_FILE_INDEX_DTYPE.itemsize, dtype=torch.uint8, device=d)
+        tracks_t = torch.empty(len(r) * MPA_TRACK_DTYPE.itemsize, dtype=torch.uint8, device=d)
+        torch.cuda.current_stream(d).synchronize()  # data_t and the outputs are torch's: written / allocated on its stream
+        self.mpa_index_dev_queue(data_t, r, cap, packets_t, jobs_t, index_t, tracks_t, seekable)
+        self.sync()
+        return packets_t, jobs_t, index_t.cpu().numpy().view(MPA_FILE_INDEX_DTYPE), tracks_t.cpu().numpy().view(MPA_TRACK_DTYPE)
+
+    def mpa_index_dev_queue(self, data_t, ranges, cap, packets_t, jobs_t, index_t, tracks_t, seekable=True):
+        """symgpu_mpa_index_dev on uint8 CUDA tensors (packets_t / jobs_t, either None, holding `cap` records; index_t and tracks_t
+        one record per file), left queued on the engine's stream after the call's one wait: no wait for torch's stream before it."""
+        from ._native import MP3_JOB_DTYPE, MPA_PACKET_DTYPE
+        r = file_ranges(ranges)
+        assert packets_t is None or packets_t.numel() >= cap * MPA_PACKET_DTYPE.itemsize
+        assert jobs_t is None or jobs_t.numel() >= cap * MP3_JOB_DTYPE.itemsize
+        self._check(self._lib.symgpu_mpa_index_dev(self._ctx, _dev_ptr(data_t), data_t.numel(), _host_ptr(r), len(r), int(bool(seekable)),
+                                                   None if packets_t is None else _dev_ptr(packets_t),
+                                                   None if jobs_t is None else _dev_ptr(jobs_t), cap, _dev_ptr(index_t), _dev_ptr(tracks_t)))
+
     # -- Vorbis jobs built on the device from the device Ogg index (uint8 CUDA tensors holding the records; queued, no wait) -----
     def vorbis_heads_dev(self, data_t, ranges, packets_t, pieces_t, index_t, heads_t, ranks_t):
         """symgpu_vorbis_heads_dev: per file a VORBIS_FILE_HEADS_DTYPE record in heads_t, per packet of packets_t a
