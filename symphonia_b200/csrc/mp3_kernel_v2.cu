@@ -212,9 +212,10 @@ __device__ __forceinline__ void imdct12x3(const Ops& o, const f2 (&x)[18], f2 (&
     }
 }
 
-// A sub-band in which one channel is long and the other short (independent block types outside joint stereo;
-// rare): both transforms, component-wise choice.  Kept out of line with its operands in local memory so that
-// its register needs do not shape the granule loop.
+// A sub-band in which one channel is long and the other short: both transforms, component-wise choice.  Only
+// frames without mid-side or intensity stereo reach it (stereo, dual-channel, joint stereo with mode_ext 0), where
+// each channel switches windows on its own; in such streams it is common wherever one channel is on short blocks.
+// Kept out of line with its operands in local memory so that its register needs do not shape the granule loop.
 __device__ __noinline__ void hybrid_mixed(const f2* xin, int wsel0, int wsel1, int cat0, int cat1, f2* fout, f2* sout) {
     const Ops o{};
     f2 x[18], fa[18], sa[18], fb[18], sb[18];
