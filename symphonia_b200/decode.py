@@ -134,14 +134,21 @@ def decode_ogg_vorbis(engine, data, fmt=nat.FMT_S16, serial=None, threads=1):
     return engine.pcm_pack_host(pcm, plan["spans"], plan["channels"], fmt, plan["total_frames"]), plan["sample_rate"]
 
 
+def _aac_refusal(n_frames, channels):
+    """Why an ADTS stream of n_frames frames whose first frame has `channels` cannot be decoded, or None when it can."""
+    if n_frames == 0:
+        return "no ADTS frames"
+    if channels not in (1, 2):
+        return "channel configuration outside AAC-LC mono / stereo"
+
+
 def adts_aac_index(data):
     """(packets, sample_rate, channels): the ADTS frame index and the stream's parameters (the first frame's, AdtsReader::try_new)."""
     packets, _ = packetizer.adts_index(data)
-    if len(packets) == 0:
-        raise ValueError("no ADTS frames")
-    rate, channels = int(packets[0]["sample_rate"]), int(packets[0]["channels"])
-    if channels not in (1, 2):
-        raise ValueError("channel configuration outside AAC-LC mono / stereo")
+    rate, channels = (int(packets[0]["sample_rate"]), int(packets[0]["channels"])) if len(packets) else (0, 0)
+    refusal = _aac_refusal(len(packets), channels)
+    if refusal:
+        raise ValueError(refusal)
     return packets, rate, channels
 
 
@@ -476,54 +483,140 @@ def _index_files(files, index_fn, threads):
     return ix, messages
 
 
+def _packed(n_groups, good, sizes):
+    """Every group's start when the good groups' sizes lie back to back in their order and a failed group starts at their end."""
+    sizes = np.array(sizes, dtype=np.int64)
+    starts = np.full(n_groups, sizes.sum(), dtype=np.int64)
+    starts[good] = np.cumsum(sizes) - sizes
+    return starts
+
+
+def _place(groups, parts, first_job):
+    """Lays out one call's groups.  parts: (i, n_jobs, fields, out samples) of every good file in order, which gets `fields`;
+    out_offset is _packed (a failed file's group, in no part, gets the end of the output).  Where the record has them, a good
+    group gets n_jobs and every group first_job[i], its start in the job table.  Returns (output total, failed files)."""
+    good = [p[0] for p in parts]
+    groups["out_offset"] = _packed(len(groups), good, [p[3] for p in parts])
+    for k in parts[0][2] if parts else ():
+        groups[k][good] = [p[2][k] for p in parts]
+    if "first_job" in groups.dtype.names:
+        groups["first_job"], groups["n_jobs"][good] = first_job, [p[1] for p in parts]
+    placed = set(good)
+    return sum(p[3] for p in parts), [i for i in range(len(groups)) if i not in placed]
+
+
 def _batch(groups, parts, job_dtype):
     """One call's bytes, jobs and groups.  groups: one record per file, already holding what a failed file's group keeps;
-    parts: (i, bytes, jobs, fields, out samples) of every good file in order, its jobs' offsets relative to its bytes.  Each
-    good group gets `fields`, its out_offset and, when the group record has them, first_job / n_jobs; a failed file's group
-    gets no jobs, at the end of the output.  Returns (data, jobs, output total, failed files)."""
-    ranged = "first_job" in groups.dtype.names
-    srcs, jobs, byte_at, job_at, out_at = [], [], 0, 0, 0
-    for i, src, j, fields, n_out in parts:
+    parts: (i, bytes, jobs, fields, out samples) of every good file in order, its jobs' offsets relative to its bytes; their
+    bytes and jobs go back to back.  Returns (data, jobs, output total, failed files)."""
+    srcs, byte_at = [], 0
+    for _, src, j, _, _ in parts:
         src = np.frombuffer(src, dtype=np.uint8) if not isinstance(src, np.ndarray) else np.ascontiguousarray(src, dtype=np.uint8)
-        g = groups[i]
-        for k, v in fields.items():
-            g[k] = v
-        g["out_offset"] = out_at
-        if ranged:
-            g["first_job"], g["n_jobs"] = job_at, len(j)
         j["offset"] += np.uint64(byte_at)
         srcs.append(src)
-        jobs.append(j)
         byte_at += src.size
-        job_at += len(j)
-        out_at += n_out
-    good = {p[0] for p in parts}
-    failed = [i for i in range(len(groups)) if i not in good]
-    groups["out_offset"][failed] = out_at
-    if ranged:
-        groups["first_job"][failed] = job_at
+    out_at, failed = _place(groups, [(i, len(j), fields, n_out) for i, _, j, fields, n_out in parts],
+                            _packed(len(groups), [p[0] for p in parts], [len(p[2]) for p in parts]))
     data = np.concatenate(srcs) if srcs else np.zeros(0, dtype=np.uint8)
-    jobs = np.concatenate(jobs) if jobs else np.zeros(0, dtype=job_dtype)
+    jobs = np.concatenate([p[2] for p in parts]) if parts else np.zeros(0, dtype=job_dtype)
     return data, jobs, out_at, failed
 
 
-def _decode_batch(engine, device, inputs, cap, out_dtype, n_groups, result_dtype, host, dev):
+def _u8(device, count):
+    import torch
+    return torch.empty(int(count), dtype=torch.uint8, device=device)
+
+
+def _decode_dev(engine, device, fmt, cap, n_groups, result_dtype, n_jobs, decode, read_status=True):
+    """decode(out_t, results_t, status_t) -> extra queued on new tensors (`cap` samples of `fmt`, n_groups result_dtype records,
+    n_jobs status bytes), a wait for the engine's stream, and the results (and with read_status the status) read back.  Returns
+    (out_t, results, status or None, extra, bytes read back)."""
+    import torch
+    out = torch.empty(cap, dtype=getattr(torch, _TORCH_DTYPES[fmt]), device=device)
+    results_t, status_t = _u8(device, n_groups * result_dtype.itemsize), _u8(device, n_jobs)
+    extra = decode(out, results_t, status_t)
+    engine.sync()
+    results = results_t.cpu().numpy().view(result_dtype)
+    status = status_t.cpu().numpy() if read_status else None
+    return out, results, status, extra, results.nbytes + (status.nbytes if read_status else 0)
+
+
+def _decode_batch(engine, device, inputs, cap, fmt, n_groups, result_dtype, host, dev):
     """One device call: host() -> (out, results, status, extra) on numpy arrays, or with device=True the `inputs` copied to the
-    device and dev(*inputs_t, out_t, results_t, status_t) -> extra on torch CUDA tensors (out_t: `cap` elements of torch's
-    `out_dtype`; results_t: the bytes of n_groups result_dtype records), read back after the engine's stream is done.  Returns
-    (out, results, status, extra)."""
+    device and _decode_dev of dev(*inputs_t, out_t, results_t, status_t) -> extra, with a status byte per job of inputs[1].
+    Returns (out, results, status, extra)."""
     if not device:
         return host()
     import torch
     d = torch.device("cuda", engine.device)
-    out = torch.empty(cap, dtype=getattr(torch, out_dtype), device=d)
-    results_t = torch.empty(n_groups * result_dtype.itemsize, dtype=torch.uint8, device=d)
-    status_t = torch.empty(len(inputs[1]), dtype=torch.uint8, device=d)
     staged = [torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(-1)).to(d) for a in inputs]
     torch.cuda.current_stream(d).synchronize()  # the copies above are on torch's stream, the decode on the engine's
-    extra = dev(*staged, out, results_t, status_t)
-    engine.sync()
-    return out, results_t.cpu().numpy().view(result_dtype), status_t.cpu().numpy(), extra
+    return _decode_dev(engine, d, fmt, cap, n_groups, result_dtype, len(inputs[1]), lambda *outputs: dev(*staged, *outputs))[:4]
+
+
+def _resident_files(data_t, ranges, name, limit):
+    """The FILE_RANGE_DTYPE records of `ranges`, after the checks a call on device-resident files makes before any launch: at
+    most `limit` files, data_t a contiguous uint8 CUDA tensor, every range inside it.  name: the call, for the messages."""
+    import torch
+
+    from .engine import file_ranges
+    r = file_ranges(ranges)
+    if len(r) > limit:
+        raise ValueError(f"{name} takes at most {limit} files per call, not {len(r)}")
+    if not (data_t.is_cuda and data_t.dtype == torch.uint8 and data_t.is_contiguous()):
+        raise ValueError(f"{name} takes a contiguous uint8 CUDA tensor")
+    size = data_t.numel()
+    if ((r["offset"] > size) | (r["len"] > size - np.minimum(r["offset"], size))).any():
+        raise ValueError(f"a file range lies outside the {size} bytes of data_t")
+    return r
+
+
+def _good_status(status, groups, failed):
+    """The per-packet status of every group not in `failed`, in group order: what the host-indexed path's status holds."""
+    failed = set(failed)
+    runs = [status[int(g["first_job"]):int(g["first_job"]) + int(g["n_jobs"])] for k, g in enumerate(groups) if k not in failed]
+    return np.concatenate(runs) if runs else np.zeros(0, dtype=np.uint8)
+
+
+# each codec's group rule: from what the index says about one good file, (its group fields, its output samples)
+
+def _aac_group(sample_rate, channels, n_packets):
+    return dict(sample_rate=sample_rate, channels=channels), n_packets * 1024 * channels
+
+
+def _mp3_group(track, n_packets):
+    granules, channels = 2 if int(track["version"]) == 0 else 1, int(track["channels"])
+    return dict(granules=granules, channels=channels), n_packets * granules * 576 * channels
+
+
+def _mpa12_group(track, n_packets):
+    layer = int(track["layer"])
+    return dict(layer=layer), 2 * n_packets * (384 if layer == 1 else 1152)
+
+
+def _vorbis_group(ident, n_packets, setup):
+    return dict(setup=setup), n_packets * ((1 << int(ident["bs1_exp"])) >> 1) * int(ident["channels"])
+
+
+def _aac_groups(n):
+    """n AAC groups, group i on state slot i, each holding what a failed file's group keeps (mono, 44.1 kHz)."""
+    groups = np.zeros(n, dtype=nat.AAC_GROUP_DTYPE)
+    groups["slot"] = np.arange(n)
+    groups["channels"], groups["sample_rate"] = 1, 44100
+    return groups
+
+
+def _vorbis_setups(pairs):
+    """One setup per distinct (identification, setup) header pair of `pairs`: ([each pair's setup index],
+    VORBIS_SETUP_REF_DTYPE records, the header bytes they point into)."""
+    index, refs, headers, at = {}, [], [], 0
+    for ident_b, setup_b in pairs:
+        if (ident_b, setup_b) not in index:
+            index[(ident_b, setup_b)] = len(refs)
+            refs.append((at, at + len(ident_b), len(ident_b), len(setup_b)))
+            headers += [ident_b, setup_b]
+            at += len(ident_b) + len(setup_b)
+    return [index[p] for p in pairs], np.array(refs, dtype=nat.VORBIS_SETUP_REF_DTYPE), b"".join(headers)
 
 
 def _per_file(out, groups, failed, shape):
@@ -579,7 +672,7 @@ def decode_flac_files(engine, files, threads=None, device=False, errors=None, fm
     def dev(data_t, jobs_t, groups_t, out_t, frames_t, status_t):
         import torch
         engine.flac_decode_dev(data_t, jobs_t, groups_t, out_t, frames_t.view(torch.int64), status_t, fmt)
-    out, group_frames, _, _ = _decode_batch(engine, device, (plan["data"], plan["jobs"], groups), cap, _TORCH_DTYPES[fmt], len(groups), np.dtype(np.int64),
+    out, group_frames, _, _ = _decode_batch(engine, device, (plan["data"], plan["jobs"], groups), cap, fmt, len(groups), np.dtype(np.int64),
                                             lambda: (*engine.flac_decode_host(plan["data"], plan["jobs"], groups, cap, fmt=fmt), None), dev)
     return _per_file(out, groups, plan["failed"], lambda g: (int(group_frames[g]), int(groups[g]["channels"]), int(rates[g])))
 
@@ -618,27 +711,34 @@ def _mpa_shape(r, track):
     return int(r["frames"]), int(r["channels"]), int(r["sample_rate"])
 
 
+def _mpa_files_plan(files, threads, errors, index, layers, what, group_dtype, job_dtype, group_rule, **failed_fields):
+    """mpa12_files_plan / mp3_files_plan: the files of `layers` (the others refused with `what`) get their group from
+    group_rule, group i uses state slot i, and a failed file's group holds failed_fields."""
+    ix, messages = mpa_index_files(files, threads) if index is None else (index[0], dict(index[1]))
+    ix = _keep_layers(ix, messages, layers, what)
+    if errors is not None:
+        errors.update(messages)
+    groups = np.zeros(len(files), dtype=group_dtype)
+    groups["slot"] = np.arange(len(files))
+    for k, v in failed_fields.items():
+        groups[k] = v
+    parts = []
+    for i, x in enumerate(ix):
+        if x is not None:
+            track, packets = x
+            parts.append((i, files[i], _mpa_jobs(packets, job_dtype), *group_rule(track, len(packets))))
+    data, jobs, cap, failed = _batch(groups, parts, job_dtype)
+    tracks = [None if t is None else t[0] for t in ix]
+    return dict(data=data, jobs=jobs, groups=groups, tracks=tracks, out_samples=cap, failed=failed)
+
+
 def mpa12_files_plan(files, threads=None, errors=None, index=None):
     """Host half of decode_mpa12_files: every file indexed (symgpu_mpa_index, on `threads` host threads), their bytes concatenated
     once, one job per packet and one group per file (group i uses state slot i).  Returns dict(data, jobs, groups, tracks, out_samples,
     failed).  A file that cannot be indexed or is not Layer I / II (listed in `failed`) gets a group without jobs; its message goes to
     errors[i] when `errors` is a dict.  index: the result of mpa_index_files (else computed here)."""
-    ix, messages = mpa_index_files(files, threads) if index is None else (index[0], dict(index[1]))
-    ix = _keep_layers(ix, messages, (1, 2), "decode_mpa12_files takes Layer I / II files")
-    if errors is not None:
-        errors.update(messages)
-    groups = np.zeros(len(files), dtype=nat.MPA12_GROUP_DTYPE)
-    groups["slot"] = np.arange(len(files))
-    groups["layer"] = 1
-    parts = []
-    for i, x in enumerate(ix):
-        if x is not None:
-            track, packets = x
-            layer = int(track["layer"])
-            parts.append((i, files[i], _mpa_jobs(packets, nat.MPA12_JOB_DTYPE), dict(layer=layer), 2 * len(packets) * (384 if layer == 1 else 1152)))
-    data, jobs, cap, failed = _batch(groups, parts, nat.MPA12_JOB_DTYPE)
-    tracks = [None if t is None else t[0] for t in ix]
-    return dict(data=data, jobs=jobs, groups=groups, tracks=tracks, out_samples=cap, failed=failed)
+    return _mpa_files_plan(files, threads, errors, index, (1, 2), "decode_mpa12_files takes Layer I / II files", nat.MPA12_GROUP_DTYPE,
+                           nat.MPA12_JOB_DTYPE, _mpa12_group, layer=1)
 
 
 def decode_mpa12_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False, errors=None, index=None):
@@ -652,7 +752,7 @@ def decode_mpa12_files(engine, files, fmt=nat.FMT_S16, threads=None, device=Fals
     groups, cap = plan["groups"], plan["out_samples"]
     engine.mp3_streams_alloc(max(len(files), 1))
     out, results, _, _ = _decode_batch(
-        engine, device, (plan["data"], plan["jobs"]), cap, _TORCH_DTYPES[fmt], len(groups), nat.MPA12_RESULT_DTYPE,
+        engine, device, (plan["data"], plan["jobs"]), cap, fmt, len(groups), nat.MPA12_RESULT_DTYPE,
         lambda: (*engine.mpa12_decode_host(plan["data"], plan["jobs"], groups, fmt, cap), None),
         lambda data_t, jobs_t, out_t, results_t, status_t: engine.mpa12_decode_dev(data_t, jobs_t, groups, fmt, out_t, results_t, status_t))
     return _per_file(out, groups, plan["failed"], lambda g: _mpa_shape(results[g], plan["tracks"][g]))
@@ -665,23 +765,8 @@ def mp3_files_plan(files, threads=None, errors=None, index=None):
     one job per packet and one group per file (group i uses state slot i; granules and channels from the file's track).  Returns
     dict(data, jobs, groups, tracks, out_samples, failed).  A file that cannot be indexed or is not Layer III (listed in `failed`) gets
     a group without jobs; its message goes to errors[i] when `errors` is a dict.  index: the result of mpa_index_files."""
-    ix, messages = mpa_index_files(files, threads) if index is None else (index[0], dict(index[1]))
-    ix = _keep_layers(ix, messages, (3,), "decode_mp3_files takes Layer III files")
-    if errors is not None:
-        errors.update(messages)
-    groups = np.zeros(len(files), dtype=nat.MP3_GROUP_DTYPE)
-    groups["slot"] = np.arange(len(files))
-    groups["granules"], groups["channels"] = 2, 2
-    parts = []
-    for i, x in enumerate(ix):
-        if x is not None:
-            track, packets = x
-            granules, channels = 2 if int(track["version"]) == 0 else 1, int(track["channels"])
-            parts.append((i, files[i], _mpa_jobs(packets, nat.MP3_JOB_DTYPE), dict(granules=granules, channels=channels),
-                          len(packets) * granules * 576 * channels))
-    data, jobs, cap, failed = _batch(groups, parts, nat.MP3_JOB_DTYPE)
-    tracks = [None if t is None else t[0] for t in ix]
-    return dict(data=data, jobs=jobs, groups=groups, tracks=tracks, out_samples=cap, failed=failed)
+    return _mpa_files_plan(files, threads, errors, index, (3,), "decode_mp3_files takes Layer III files", nat.MP3_GROUP_DTYPE,
+                           nat.MP3_JOB_DTYPE, _mp3_group, granules=2, channels=2)
 
 
 def decode_mp3_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False, errors=None, index=None, stats=None):
@@ -697,7 +782,7 @@ def decode_mp3_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False,
     groups, cap = plan["groups"], plan["out_samples"]
     engine.mp3_streams_alloc(max(len(files), 1))
     out, results, status, rounds = _decode_batch(
-        engine, device, (plan["data"], plan["jobs"]), cap, _TORCH_DTYPES[fmt], len(groups), nat.MP3_RESULT_DTYPE,
+        engine, device, (plan["data"], plan["jobs"]), cap, fmt, len(groups), nat.MP3_RESULT_DTYPE,
         lambda: engine.mp3_decode_host(plan["data"], plan["jobs"], groups, fmt, cap),
         lambda data_t, jobs_t, out_t, results_t, status_t: engine.mp3_decode_dev(data_t, jobs_t, groups, fmt, out_t, results_t, status_t))
     if stats is not None:
@@ -715,16 +800,14 @@ def aac_files_plan(files, threads=None, errors=None):
     ix, messages = _index_files(files, adts_aac_index, threads)
     if errors is not None:
         errors.update(messages)
-    groups = np.zeros(len(files), dtype=nat.AAC_GROUP_DTYPE)
-    groups["slot"] = np.arange(len(files))
-    groups["channels"], groups["sample_rate"] = 1, 44100
+    groups = _aac_groups(len(files))
     parts = []
     for i, x in enumerate(ix):
         if x is not None:
             packets, rate, channels = x
             j = np.zeros(len(packets), dtype=nat.PIECE_DTYPE)
             j["offset"], j["len"] = packets["offset"], packets["size"]
-            parts.append((i, files[i], j, dict(sample_rate=rate, channels=channels), len(packets) * 1024 * channels))
+            parts.append((i, files[i], j, *_aac_group(rate, channels, len(packets))))
     data, jobs, cap, failed = _batch(groups, parts, nat.PIECE_DTYPE)
     return dict(data=data, jobs=jobs, groups=groups, out_samples=cap, failed=failed)
 
@@ -744,7 +827,7 @@ def decode_aac_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False,
     groups, cap = plan["groups"], plan["out_samples"]
     engine.aac_streams_alloc(max(len(files), 1))
     out, results, status, redone = _decode_batch(
-        engine, device, (plan["data"], plan["jobs"]), cap, _TORCH_DTYPES[fmt], len(groups), nat.AAC_RESULT_DTYPE,
+        engine, device, (plan["data"], plan["jobs"]), cap, fmt, len(groups), nat.AAC_RESULT_DTYPE,
         lambda: engine.aac_decode_host(plan["data"], plan["jobs"], groups, fmt, cap),
         lambda data_t, jobs_t, out_t, results_t, status_t: engine.aac_decode_dev(data_t, jobs_t, groups, fmt, out_t, results_t, status_t))
     if stats is not None:
@@ -761,65 +844,34 @@ def decode_aac_files_dev(engine, data_t, ranges, fmt=nat.FMT_S16, errors=None, s
     index records, the decode's results and its per-packet status come back to the host.  stats also receives
     `read_back_bytes`, every byte the call copies from the device.  A failed file's packets stay in the job table, named by no
     group.  At most 65 536 files; (re)allocates the engine's AAC state slots, one per file, as decode_aac_files does."""
-    import torch
-
-    from .engine import file_ranges
-    r = file_ranges(ranges)
+    r = _resident_files(data_t, ranges, "decode_aac_files_dev", nat.ADTS_MAX_FILES)
     n = len(r)
-    if n > nat.ADTS_MAX_FILES:
-        raise ValueError(f"decode_aac_files_dev takes at most {nat.ADTS_MAX_FILES} files per call, not {n}")
-    if not (data_t.is_cuda and data_t.dtype == torch.uint8 and data_t.is_contiguous()):
-        raise ValueError("decode_aac_files_dev takes a contiguous uint8 CUDA tensor")
-    size = data_t.numel()
-    if ((r["offset"] > size) | (r["len"] > size - np.minimum(r["offset"], size))).any():
-        raise ValueError(f"a file range lies outside the {size} bytes of data_t")
     if n == 0:
         return []
-    dev = data_t.device
-
-    def u8(count):
-        return torch.empty(int(count), dtype=torch.uint8, device=dev)
     # 1. every file's frames as jobs, the table sized by the bound (a frame is at least 7 bytes)
-    cap = int((r["len"] // 7).sum())
-    jobs_t, index_t = u8(cap * nat.PIECE_DTYPE.itemsize), u8(n * nat.ADTS_FILE_INDEX_DTYPE.itemsize)
-    torch.cuda.current_stream(dev).synchronize()   # data_t is torch's: written on its stream
-    engine.adts_index_dev_queue(data_t, r, cap, None, jobs_t, index_t)
-    engine.sync()
-    ix = index_t.cpu().numpy().view(nat.ADTS_FILE_INDEX_DTYPE)
-    read = ix.nbytes
-    # 2. the groups, as aac_files_plan lays them out, with the messages adts_aac_index raises
-    messages = {}
-    groups = np.zeros(n, dtype=nat.AAC_GROUP_DTYPE)
-    groups["slot"] = np.arange(n)
-    groups["channels"], groups["sample_rate"] = 1, 44100
-    groups["first_job"] = ix["first_packet"]
-    out_at = 0
+    _, jobs_t, ix = engine._index_dev(engine.adts_index_dev_queue, data_t, r, None, 7, (None, nat.PIECE_DTYPE), (nat.ADTS_FILE_INDEX_DTYPE,))
+    # 2. the groups, as aac_files_plan lays them out (a failed file's group starts at its own packets), with adts_aac_index's messages
+    messages, parts = {}, []
     for i in range(n):
-        if ix["n_packets"][i] == 0:
-            messages[i] = "ValueError: no ADTS frames"
-        elif ix["channels"][i] not in (1, 2):
-            messages[i] = "ValueError: channel configuration outside AAC-LC mono / stereo"
+        n_jobs, channels = int(ix["n_packets"][i]), int(ix["channels"][i])
+        refusal = _aac_refusal(n_jobs, channels)
+        if refusal:
+            messages[i] = f"ValueError: {refusal}"
         else:
-            ch, n_jobs = int(ix["channels"][i]), int(ix["n_packets"][i])
-            groups[i]["n_jobs"], groups[i]["channels"], groups[i]["sample_rate"] = n_jobs, ch, int(ix["sample_rate"][i])
-            groups[i]["out_offset"] = out_at
-            out_at += n_jobs * 1024 * ch
-    failed = sorted(messages)
-    groups["out_offset"][failed] = out_at
+            parts.append((i, n_jobs, *_aac_group(int(ix["sample_rate"][i]), channels, n_jobs)))
+    groups = _aac_groups(n)
+    out_at, failed = _place(groups, parts, ix["first_packet"])
     if errors is not None:
         errors.update(messages)
     # 3. the decode, on the job table in place
     n_jobs = int(ix["first_packet"][-1]) + int(ix["n_packets"][-1])
     engine.aac_streams_alloc(n)
-    out = torch.empty(out_at, dtype=getattr(torch, _TORCH_DTYPES[fmt]), device=dev)
-    results_t, status_t = u8(n * nat.AAC_RESULT_DTYPE.itemsize), u8(n_jobs)
-    redone = engine.aac_decode_dev(data_t, jobs_t[:n_jobs * nat.PIECE_DTYPE.itemsize], groups, fmt, out, results_t, status_t)
-    engine.sync()
-    results, status = results_t.cpu().numpy().view(nat.AAC_RESULT_DTYPE), status_t.cpu().numpy()
-    read += results.nbytes + status.nbytes
+    out, results, status, redone, read = _decode_dev(
+        engine, data_t.device, fmt, out_at, n, nat.AAC_RESULT_DTYPE, n_jobs,
+        lambda out_t, results_t, status_t: engine.aac_decode_dev(data_t, jobs_t[:n_jobs * nat.PIECE_DTYPE.itemsize], groups, fmt, out_t,
+                                                                 results_t, status_t))
     if stats is not None:
-        good = [status[int(g["first_job"]):int(g["first_job"]) + int(g["n_jobs"])] for g in groups[[i for i in range(n) if i not in messages]]]
-        stats.update(status=np.concatenate(good) if good else np.zeros(0, dtype=np.uint8), n_redecoded=redone, read_back_bytes=read)
+        stats.update(status=_good_status(status, groups, failed), n_redecoded=redone, read_back_bytes=ix.nbytes + read)
     return _per_file(out, groups, failed, lambda g: (int(results[g]["frames"]), int(groups[g]["channels"]), int(groups[g]["sample_rate"])))
 
 
@@ -859,68 +911,42 @@ def decode_mpeg_files_dev(engine, data_t, ranges, fmt=nat.FMT_S16, errors=None, 
     (re)allocates the engine's MP3 state slots, one per file."""
     import torch
 
-    from .engine import SymgpuError, file_ranges
-    r = file_ranges(ranges)
+    from .engine import SymgpuError
+    r = _resident_files(data_t, ranges, "decode_mpeg_files_dev", nat.MPA_MAX_FILES)
     n = len(r)
-    if n > nat.MPA_MAX_FILES:
-        raise ValueError(f"decode_mpeg_files_dev takes at most {nat.MPA_MAX_FILES} files per call, not {n}")
-    if not (data_t.is_cuda and data_t.dtype == torch.uint8 and data_t.is_contiguous()):
-        raise ValueError("decode_mpeg_files_dev takes a contiguous uint8 CUDA tensor")
-    size = data_t.numel()
-    if ((r["offset"] > size) | (r["len"] > size - np.minimum(r["offset"], size))).any():
-        raise ValueError(f"a file range lies outside the {size} bytes of data_t")
     if n == 0:
         return []
     dev = data_t.device
-    out_dtype = getattr(torch, _TORCH_DTYPES[fmt])
-
-    def u8(count):
-        return torch.empty(int(count), dtype=torch.uint8, device=dev)
     # 1. every file's frames as jobs, the table sized by the bound (a frame is at least MPA_MIN_FRAME bytes)
-    cap = int((r["len"] // nat.MPA_MIN_FRAME).sum())
-    jobs_t, index_t, tracks_t = u8(cap * nat.MP3_JOB_DTYPE.itemsize), u8(n * nat.MPA_FILE_INDEX_DTYPE.itemsize), u8(n * nat.MPA_TRACK_DTYPE.itemsize)
-    torch.cuda.current_stream(dev).synchronize()   # data_t is torch's: written on its stream
-    engine.mpa_index_dev_queue(data_t, r, cap, None, jobs_t, index_t, tracks_t)
-    engine.sync()
-    ix, tracks = index_t.cpu().numpy().view(nat.MPA_FILE_INDEX_DTYPE), tracks_t.cpu().numpy().view(nat.MPA_TRACK_DTYPE)
+    _, jobs_t, ix, tracks = engine._index_dev(engine.mpa_index_dev_queue, data_t, r, None, nat.MPA_MIN_FRAME, (None, nat.MP3_JOB_DTYPE),
+                                              (nat.MPA_FILE_INDEX_DTYPE, nat.MPA_TRACK_DTYPE))
     read = ix.nbytes + tracks.nbytes
     messages = {i: f"SymgpuError: {SymgpuError(1, 'symgpu_mpa_index')}" for i in range(n) if ix["status"][i] & nat.MPA_NO_FRAME}
     if errors is not None:
         errors.update(messages)
     # 2. one decode per layer family, on the job table in place, with the groups decode_mp3_files / decode_mpa12_files make
     engine.mp3_streams_alloc(n)
-    result = [(torch.empty((0, 0), dtype=out_dtype, device=dev), 0)] * n
-    families = (((3,), nat.MP3_GROUP_DTYPE, nat.MP3_RESULT_DTYPE, engine.mp3_decode_dev),
-                ((1, 2), nat.MPA12_GROUP_DTYPE, nat.MPA12_RESULT_DTYPE, engine.mpa12_decode_dev))
-    for layers, group_dtype, result_dtype, decode in families:
+    result = [(torch.empty((0, 0), dtype=getattr(torch, _TORCH_DTYPES[fmt]), device=dev), 0)] * n
+    families = (((3,), nat.MP3_GROUP_DTYPE, nat.MP3_RESULT_DTYPE, engine.mp3_decode_dev, _mp3_group),
+                ((1, 2), nat.MPA12_GROUP_DTYPE, nat.MPA12_RESULT_DTYPE, engine.mpa12_decode_dev, _mpa12_group))
+    for layers, group_dtype, result_dtype, decode, group_rule in families:
         mine = [i for i in range(n) if i not in messages and int(tracks["layer"][i]) in layers]
         if not mine:
             continue
         lo = int(ix["first_packet"][mine[0]])
         hi = int(ix["first_packet"][mine[-1]]) + int(ix["n_packets"][mine[-1]])
         groups = np.zeros(len(mine), dtype=group_dtype)
-        out_at = 0
-        for g, i in enumerate(mine):
-            t, n_jobs = tracks[i], int(ix["n_packets"][i])
-            groups[g]["slot"], groups[g]["first_job"], groups[g]["n_jobs"], groups[g]["out_offset"] = i, int(ix["first_packet"][i]) - lo, n_jobs, out_at
-            if layers == (3,):
-                granules, channels = 2 if int(t["version"]) == 0 else 1, int(t["channels"])
-                groups[g]["granules"], groups[g]["channels"] = granules, channels
-                out_at += n_jobs * granules * 576 * channels
-            else:
-                groups[g]["layer"] = int(t["layer"])
-                out_at += 2 * n_jobs * (384 if int(t["layer"]) == 1 else 1152)
-        out = torch.empty(out_at, dtype=out_dtype, device=dev)
-        results_t, status_t = u8(len(mine) * result_dtype.itemsize), u8(hi - lo)
-        rounds = decode(data_t, jobs_t[lo * nat.MP3_JOB_DTYPE.itemsize:hi * nat.MP3_JOB_DTYPE.itemsize], groups, fmt, out, results_t, status_t)
-        engine.sync()
-        results = results_t.cpu().numpy().view(result_dtype)
-        read += results.nbytes
-        if layers == (3,):
-            status = status_t.cpu().numpy()
-            read += status.nbytes
-            if stats is not None:
-                stats.update(rounds=rounds, status=np.concatenate([status[int(g["first_job"]):int(g["first_job"]) + int(g["n_jobs"])] for g in groups]))
+        groups["slot"] = mine
+        parts = [(g, int(ix["n_packets"][i]), *group_rule(tracks[i], int(ix["n_packets"][i]))) for g, i in enumerate(mine)]
+        out_at, _ = _place(groups, parts, ix["first_packet"][mine] - lo)
+        out, results, status, rounds, nread = _decode_dev(
+            engine, dev, fmt, out_at, len(mine), result_dtype, hi - lo,
+            lambda out_t, results_t, status_t: decode(data_t, jobs_t[lo * nat.MP3_JOB_DTYPE.itemsize:hi * nat.MP3_JOB_DTYPE.itemsize], groups,
+                                                      fmt, out_t, results_t, status_t),
+            read_status=layers == (3,))
+        read += nread
+        if status is not None and stats is not None:
+            stats.update(rounds=rounds, status=_good_status(status, groups, []))
         for i, got in zip(mine, _per_file(out, groups, [], lambda g: _mpa_shape(results[g], tracks[mine[g]]))):
             result[i] = got
     if stats is not None:
@@ -944,28 +970,18 @@ def vorbis_files_plan(files, threads=None, errors=None):
     if errors is not None:
         errors.update(messages)
     groups = np.zeros(len(files), dtype=nat.VORBIS_GROUP_DTYPE)
-    setup_of, headers, refs, parts, head_at = {}, [], [], [], 0
-    for i, x in enumerate(ix):
-        if x is None:
-            continue
-        ident_b, setup_b = x["headers"]
-        key = (ident_b, setup_b)
-        if key not in setup_of:
-            setup_of[key] = len(refs)
-            refs.append((head_at, head_at + len(ident_b), len(ident_b), len(setup_b)))
-            headers += [ident_b, setup_b]
-            head_at += len(ident_b) + len(setup_b)
-        n, channels = len(x["table"]), int(x["ident"]["channels"])
-        j = np.zeros(n, dtype=nat.VORBIS_JOB_DTYPE)
+    good = [i for i, x in enumerate(ix) if x is not None]
+    setup_of, setups, headers = _vorbis_setups([ix[i]["headers"] for i in good])
+    parts = []
+    for i, setup in zip(good, setup_of):
+        x = ix[i]
+        j = np.zeros(len(x["table"]), dtype=nat.VORBIS_JOB_DTYPE)
         j["offset"], j["len"] = x["table"]["offset"], x["table"]["len"]
         j["discard"] = np.clip(x["discard"], 0, 0xffffffff)
         j["trim_end"] = np.clip(x["trim_end"], 0, 0xffffffff)
-        parts.append((i, x["blob"], j, dict(setup=setup_of[key]), n * ((1 << int(x["ident"]["bs1_exp"])) >> 1) * channels))
+        parts.append((i, x["blob"], j, *_vorbis_group(x["ident"], len(j), setup)))
     data, jobs, cap, failed = _batch(groups, parts, nat.VORBIS_JOB_DTYPE)
-    setups = np.zeros(len(refs), dtype=nat.VORBIS_SETUP_REF_DTYPE)
-    for k, r in enumerate(refs):
-        setups[k] = r
-    return dict(data=data, headers=b"".join(headers), setups=setups, jobs=jobs, groups=groups, out_samples=cap, failed=failed)
+    return dict(data=data, headers=headers, setups=setups, jobs=jobs, groups=groups, out_samples=cap, failed=failed)
 
 
 def decode_vorbis_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False, errors=None, stats=None):
@@ -989,7 +1005,7 @@ def decode_vorbis_files(engine, files, fmt=nat.FMT_S16, threads=None, device=Fal
     def dev(data_t, jobs_t, out_t, results_t, status_t):
         if len(setups):       # (else every file failed: no result is read)
             engine.vorbis_decode_dev(plan["headers"], setups, data_t, jobs_t, groups, fmt, out_t, results_t, status_t)
-    out, results, status, _ = _decode_batch(engine, device, (plan["data"], plan["jobs"]), cap, _TORCH_DTYPES[fmt], len(groups),
+    out, results, status, _ = _decode_batch(engine, device, (plan["data"], plan["jobs"]), cap, fmt, len(groups),
                                             nat.VORBIS_RESULT_DTYPE, host, dev)
     if stats is not None:
         stats.update(status=status, n_setups=len(setups))
@@ -1013,44 +1029,29 @@ def _vorbis_files_dev(engine, data_t, ranges, fmt, errors, stats, mark=None):
     'heads', 'setup' (the host's work on the headers), 'jobs' (state: the gathered audio bytes, the job table and the groups,
     on the device), 'decode'; state is {} for the others."""
     import torch
-
-    from .engine import file_ranges
-    r = file_ranges(ranges)
+    r = _resident_files(data_t, ranges, "decode_vorbis_files_dev", nat.VORBIS_MAX_FILES)
     n = len(r)
-    if n > nat.VORBIS_MAX_FILES:
-        raise ValueError(f"decode_vorbis_files_dev takes at most {nat.VORBIS_MAX_FILES} files per call, not {n}")
-    if not (data_t.is_cuda and data_t.dtype == torch.uint8 and data_t.is_contiguous()):
-        raise ValueError("decode_vorbis_files_dev takes a contiguous uint8 CUDA tensor")
-    size = data_t.numel()
-    if ((r["offset"] > size) | (r["len"] > size - np.minimum(r["offset"], size))).any():
-        raise ValueError(f"a file range lies outside the {size} bytes of data_t")
     mark = mark or (lambda phase, state: None)
     dev = data_t.device
-
-    def u8(count):
-        return torch.empty(int(count), dtype=torch.uint8, device=dev)
-
-    def bytes_of(t, dtype):
-        return t.cpu().numpy().view(dtype)
     torch.cuda.current_stream(dev).synchronize()   # data_t is torch's: written on its stream
     mark("start", {})
     # 1. the page index, as Engine.ogg_index_dev builds it: sizes first, then the tables; the index stays on the device
-    index_t = u8(n * nat.OGG_FILE_INDEX_DTYPE.itemsize)
-    engine.ogg_index_dev_queue(data_t, r, u8(0), u8(0), index_t)
+    index_t = _u8(dev, n * nat.OGG_FILE_INDEX_DTYPE.itemsize)
+    engine.ogg_index_dev_queue(data_t, r, _u8(dev, 0), _u8(dev, 0), index_t)
     engine.sync()
-    ix = bytes_of(index_t, nat.OGG_FILE_INDEX_DTYPE)
+    ix = index_t.cpu().numpy().view(nat.OGG_FILE_INDEX_DTYPE)
     read = ix.nbytes
     n_packets = int(ix["first_packet"][-1]) + int(ix["n_packets"][-1]) if n else 0
     n_pieces = int(ix["first_piece"][-1]) + int(ix["n_pieces"][-1]) if n else 0
-    packets_t, pieces_t = u8(n_packets * nat.OGG_PACKET_DTYPE.itemsize), u8(n_pieces * nat.PIECE_DTYPE.itemsize)
+    packets_t, pieces_t = _u8(dev, n_packets * nat.OGG_PACKET_DTYPE.itemsize), _u8(dev, n_pieces * nat.PIECE_DTYPE.itemsize)
     engine.ogg_index_dev_queue(data_t, r, packets_t, pieces_t, index_t)
     mark("index", {})
     # 2. each file's headers and audio packets
-    heads_t, ranks_t = u8(n * nat.VORBIS_FILE_HEADS_DTYPE.itemsize), u8(n_packets * nat.VORBIS_PACKET_RANK_DTYPE.itemsize)
+    heads_t, ranks_t = _u8(dev, n * nat.VORBIS_FILE_HEADS_DTYPE.itemsize), _u8(dev, n_packets * nat.VORBIS_PACKET_RANK_DTYPE.itemsize)
     engine.vorbis_heads_dev(data_t, r, packets_t, pieces_t, index_t, heads_t, ranks_t)
     mark("heads", {})
     engine.sync()
-    heads = bytes_of(heads_t, nat.VORBIS_FILE_HEADS_DTYPE)
+    heads = heads_t.cpu().numpy().view(nat.VORBIS_FILE_HEADS_DTYPE)
     read += heads.nbytes
     # 3. the header packets gathered into one buffer, read back, and checked on the host as ogg_vorbis_index checks them
     refs, spans, at = [], {}, 0
@@ -1065,7 +1066,7 @@ def _vorbis_files_dev(engine, data_t, ranges, fmt, errors, stats, mark=None):
             refs.append((at, i, int(h["setup"])))
             spans[i].append((at, int(h["setup_len"])))
             at += int(h["setup_len"])
-    head_t = u8(at)
+    head_t = _u8(dev, at)
     engine.ogg_gather_dev(data_t, r, packets_t, pieces_t, index_t, np.array(refs, dtype=nat.OGG_PACKET_REF_DTYPE), head_t)
     engine.sync()
     head_bytes = head_t.cpu().numpy().tobytes()
@@ -1095,40 +1096,30 @@ def _vorbis_files_dev(engine, data_t, ranges, fmt, errors, stats, mark=None):
     if errors is not None:
         errors.update(messages)
     # setups shared by identical headers, groups and each file's share of the jobs, as vorbis_files_plan lays them out
-    groups = np.zeros(n, dtype=nat.VORBIS_GROUP_DTYPE)
+    setup_of, setups, headers = _vorbis_setups(list(keys.values()))
     file_jobs = np.zeros(n, dtype=nat.VORBIS_FILE_JOBS_DTYPE)
-    setup_of, setup_refs, headers, head_at, job_at, byte_at, out_at = {}, [], [], 0, 0, 0, 0
-    for i, key in keys.items():
+    placed, job_at, byte_at = [], 0, 0
+    for (i, key), setup in zip(keys.items(), setup_of):
         ident, n_modes, mask = opened[key]
-        if key not in setup_of:
-            setup_of[key] = len(setup_refs)
-            setup_refs.append((head_at, head_at + len(key[0]), len(key[0]), len(key[1])))
-            headers += list(key)
-            head_at += len(key[0]) + len(key[1])
         n_audio, n_bytes = int(heads[i]["n_audio"]), int(heads[i]["audio_bytes"])
-        groups[i] = (out_at, job_at, n_audio, setup_of[key], 0)
+        placed.append((i, n_audio, *_vorbis_group(ident, n_audio, setup)))
         file_jobs[i] = (mask, byte_at, n_bytes, job_at, n_audio, n_modes, ident["bs0_exp"], ident["bs1_exp"], 0)
         job_at, byte_at = job_at + n_audio, byte_at + n_bytes
-        out_at += n_audio * ((1 << int(ident["bs1_exp"])) >> 1) * int(ident["channels"])
-    failed = [i for i in range(n) if i not in keys]
-    groups["out_offset"][failed], groups["first_job"][failed] = out_at, job_at
-    setups = np.array(setup_refs, dtype=nat.VORBIS_SETUP_REF_DTYPE)
+    groups = np.zeros(n, dtype=nat.VORBIS_GROUP_DTYPE)
+    out_at, failed = _place(groups, placed, _packed(n, list(keys), [p[1] for p in placed]))
     mark("setup", {})
     # 4. every audio packet's bytes and job
-    audio_t, jobs_t = u8(byte_at), u8(job_at * nat.VORBIS_JOB_DTYPE.itemsize)
+    audio_t, jobs_t = _u8(dev, byte_at), _u8(dev, job_at * nat.VORBIS_JOB_DTYPE.itemsize)
     engine.vorbis_jobs_dev(data_t, r, packets_t, pieces_t, index_t, ranks_t, file_jobs, audio_t, jobs_t)
     mark("jobs", dict(audio=audio_t, jobs=jobs_t, groups=groups))
-    # 5. the decode
-    out = torch.empty(out_at, dtype=getattr(torch, _TORCH_DTYPES[fmt]), device=dev)
-    status = np.zeros(0, dtype=np.uint8)
-    results = np.zeros(n, dtype=nat.VORBIS_RESULT_DTYPE)
-    if len(setups):    # (else every file failed: nothing is decoded)
-        results_t, status_t = u8(n * nat.VORBIS_RESULT_DTYPE.itemsize), u8(job_at)
-        engine.vorbis_decode_dev(b"".join(headers), setups, audio_t, jobs_t, groups, fmt, out, results_t, status_t)
-        mark("decode", {})
-        engine.sync()
-        results, status = bytes_of(results_t, nat.VORBIS_RESULT_DTYPE), status_t.cpu().numpy()
-        read += results.nbytes + status.nbytes
+    # 5. the decode (when every file failed, nothing is decoded and no result is read)
+    out, results, status = torch.empty(0, dtype=getattr(torch, _TORCH_DTYPES[fmt]), device=dev), None, np.zeros(0, dtype=np.uint8)
+    if len(setups):
+        def decode(out_t, results_t, status_t):
+            engine.vorbis_decode_dev(headers, setups, audio_t, jobs_t, groups, fmt, out_t, results_t, status_t)
+            mark("decode", {})
+        out, results, status, _, nread = _decode_dev(engine, dev, fmt, out_at, n, nat.VORBIS_RESULT_DTYPE, job_at, decode)
+        read += nread
     if stats is not None:
         stats.update(status=status, n_setups=len(setups), read_back_bytes=read)
     return _per_file(out, groups, failed, lambda g: (int(results[g]["frames"]), int(results[g]["channels"]), int(results[g]["sample_rate"])))

@@ -261,108 +261,95 @@ class Engine:
                                                          n_groups, int(fmt), _dev_ptr(out_t), out_t.numel(), _dev_ptr(group_frames_t),
                                                          _dev_ptr(status_t)))
 
-    # -- MPEG Layer I / II decoded on the device ----------------------------------------------------------
+    # -- many files decoded on the device: one calling convention for MPEG Layer I / II, Layer III, AAC-LC and Vorbis -------------
+    def _batch_decode_host(self, fn, lead, dtypes, counted, data, jobs, groups, fmt, out_samples, out):
+        """fn(ctx, *lead, bytes, jobs, groups, fmt, out, results, status[, &count]) on host arrays; dtypes: (job, group, result).
+        Returns (out, results, status[, count])."""
+        job_dtype, group_dtype, result_dtype = dtypes
+        a = _byte_view(data)
+        jobs = np.ascontiguousarray(jobs, dtype=job_dtype)
+        groups = np.ascontiguousarray(groups, dtype=group_dtype)
+        if out is None:
+            out = np.zeros(int(out_samples), dtype=FMT_NUMPY[fmt])
+        assert out.flags.c_contiguous
+        results = np.zeros(len(groups), dtype=result_dtype)
+        status = np.zeros(len(jobs), dtype=np.uint8)
+        count = ctypes.c_uint32(0)
+        self._check(fn(self._ctx, *lead, _host_ptr(a), a.size, _host_ptr(jobs), len(jobs), _host_ptr(groups), len(groups), int(fmt),
+                       _host_ptr(out), out.nbytes, _host_ptr(results), _host_ptr(status), *([ctypes.byref(count)] if counted else [])))
+        return (out, results, status, count.value) if counted else (out, results, status)
+
+    def _batch_decode_dev(self, fn, lead, dtypes, counted, data_t, jobs_t, groups, fmt, out_t, results_t, status_t):
+        """fn(ctx, *lead, bytes, jobs, groups, fmt, out, results, status[, &count]) on torch CUDA tensors, `groups` a host array;
+        dtypes: (job, group, result).  Returns count, or None."""
+        job_dtype, group_dtype, result_dtype = dtypes
+        ts = (data_t, jobs_t, out_t, results_t, status_t)
+        assert all(t.is_cuda and t.is_contiguous() for t in ts)
+        groups = np.ascontiguousarray(groups, dtype=group_dtype)
+        n_jobs = jobs_t.numel() * jobs_t.element_size() // job_dtype.itemsize
+        assert results_t.numel() * results_t.element_size() >= len(groups) * result_dtype.itemsize and status_t.numel() >= n_jobs
+        count = ctypes.c_uint32(0)
+        self._check(fn(self._ctx, *lead, _dev_ptr(data_t), data_t.numel(), _dev_ptr(jobs_t), n_jobs, _host_ptr(groups), len(groups), int(fmt),
+                       _dev_ptr(out_t), out_t.numel() * out_t.element_size(), _dev_ptr(results_t), _dev_ptr(status_t),
+                       *([ctypes.byref(count)] if counted else [])))
+        return count.value if counted else None
+
     def mpa12_decode_host(self, data, jobs, groups, fmt, out_samples, out=None):
         """Device Layer I / II decoding of many files in one call: `data` (bytes / uint8 array) holds the packets, jobs MPA12_JOB_DTYPE
         (one per packet), groups MPA12_GROUP_DTYPE (one per file: its jobs, layer, state slot and output offset).  Returns (out [out_samples]
         of `fmt`, results MPA12_RESULT_DTYPE [groups], status uint8 [jobs]); file g's samples are out[out_offset:][:frames * channels]."""
         from ._native import MPA12_GROUP_DTYPE, MPA12_JOB_DTYPE, MPA12_RESULT_DTYPE
-        a = _byte_view(data)
-        jobs = np.ascontiguousarray(jobs, dtype=MPA12_JOB_DTYPE)
-        groups = np.ascontiguousarray(groups, dtype=MPA12_GROUP_DTYPE)
-        if out is None:
-            out = np.zeros(int(out_samples), dtype=FMT_NUMPY[fmt])
-        assert out.flags.c_contiguous
-        results = np.zeros(len(groups), dtype=MPA12_RESULT_DTYPE)
-        status = np.zeros(len(jobs), dtype=np.uint8)
-        self._check(self._lib.symgpu_mpa12_decode_host(self._ctx, _host_ptr(a), a.size, _host_ptr(jobs), len(jobs), _host_ptr(groups), len(groups),
-                                                       int(fmt), _host_ptr(out), out.nbytes, _host_ptr(results), _host_ptr(status)))
-        return out, results, status
+        return self._batch_decode_host(self._lib.symgpu_mpa12_decode_host, (), (MPA12_JOB_DTYPE, MPA12_GROUP_DTYPE, MPA12_RESULT_DTYPE), False,
+                                 data, jobs, groups, fmt, out_samples, out)
 
     def mpa12_decode_dev(self, data_t, jobs_t, groups, fmt, out_t, results_t, status_t):
         """Device-resident variant: torch CUDA tensors (uint8 bytes, jobs / results as uint8 views of the records, `out` of the format's
         element size, uint8 status); `groups` stays a host array.  Asynchronous on the engine's stream."""
         from ._native import MPA12_GROUP_DTYPE, MPA12_JOB_DTYPE, MPA12_RESULT_DTYPE
-        ts = (data_t, jobs_t, out_t, results_t, status_t)
-        assert all(t.is_cuda and t.is_contiguous() for t in ts)
-        groups = np.ascontiguousarray(groups, dtype=MPA12_GROUP_DTYPE)
-        n_jobs = jobs_t.numel() * jobs_t.element_size() // MPA12_JOB_DTYPE.itemsize
-        assert results_t.numel() * results_t.element_size() >= len(groups) * MPA12_RESULT_DTYPE.itemsize and status_t.numel() >= n_jobs
-        self._check(self._lib.symgpu_mpa12_decode_dev(self._ctx, _dev_ptr(data_t), data_t.numel(), _dev_ptr(jobs_t), n_jobs,
-                                                      _host_ptr(groups), len(groups), int(fmt), _dev_ptr(out_t),
-                                                      out_t.numel() * out_t.element_size(), _dev_ptr(results_t), _dev_ptr(status_t)))
+        self._batch_decode_dev(self._lib.symgpu_mpa12_decode_dev, (), (MPA12_JOB_DTYPE, MPA12_GROUP_DTYPE, MPA12_RESULT_DTYPE), False,
+                         data_t, jobs_t, groups, fmt, out_t, results_t, status_t)
 
-    # -- MPEG Layer III decoded on the device -------------------------------------------------------------
     def mp3_decode_host(self, data, jobs, groups, fmt, out_samples, out=None):
         """Device Layer III decoding of many files in one call: `data` (bytes / uint8 array) holds the packets, jobs MP3_JOB_DTYPE (one per
         packet), groups MP3_GROUP_DTYPE (one per file: its jobs, granules, channels, state slot and output offset).  Returns (out
         [out_samples] of `fmt`, results MP3_RESULT_DTYPE [groups], status uint8 [jobs], rounds); file g's samples are
         out[out_offset:][:frames * channels]."""
         from ._native import MP3_GROUP_DTYPE, MP3_JOB_DTYPE, MP3_RESULT_DTYPE
-        a = _byte_view(data)
-        jobs = np.ascontiguousarray(jobs, dtype=MP3_JOB_DTYPE)
-        groups = np.ascontiguousarray(groups, dtype=MP3_GROUP_DTYPE)
-        if out is None:
-            out = np.zeros(int(out_samples), dtype=FMT_NUMPY[fmt])
-        assert out.flags.c_contiguous
-        results = np.zeros(len(groups), dtype=MP3_RESULT_DTYPE)
-        status = np.zeros(len(jobs), dtype=np.uint8)
-        rounds = ctypes.c_uint32(0)
-        self._check(self._lib.symgpu_mp3_decode_host(self._ctx, _host_ptr(a), a.size, _host_ptr(jobs), len(jobs), _host_ptr(groups), len(groups),
-                                                     int(fmt), _host_ptr(out), out.nbytes, _host_ptr(results), _host_ptr(status), ctypes.byref(rounds)))
-        return out, results, status, rounds.value
+        return self._batch_decode_host(self._lib.symgpu_mp3_decode_host, (), (MP3_JOB_DTYPE, MP3_GROUP_DTYPE, MP3_RESULT_DTYPE), True,
+                                 data, jobs, groups, fmt, out_samples, out)
 
     def mp3_decode_dev(self, data_t, jobs_t, groups, fmt, out_t, results_t, status_t):
         """Device-resident variant: torch CUDA tensors (uint8 bytes, jobs / results as uint8 views of the records, `out` of the format's
         element size, uint8 status); `groups` stays a host array.  Waits for the engine's stream once per round (a 4-byte flag); the
         synthesis and the output stage are left queued on it.  Returns the number of rounds."""
         from ._native import MP3_GROUP_DTYPE, MP3_JOB_DTYPE, MP3_RESULT_DTYPE
-        ts = (data_t, jobs_t, out_t, results_t, status_t)
-        assert all(t.is_cuda and t.is_contiguous() for t in ts)
-        groups = np.ascontiguousarray(groups, dtype=MP3_GROUP_DTYPE)
-        n_jobs = jobs_t.numel() * jobs_t.element_size() // MP3_JOB_DTYPE.itemsize
-        assert results_t.numel() * results_t.element_size() >= len(groups) * MP3_RESULT_DTYPE.itemsize and status_t.numel() >= n_jobs
-        rounds = ctypes.c_uint32(0)
-        self._check(self._lib.symgpu_mp3_decode_dev(self._ctx, _dev_ptr(data_t), data_t.numel(), _dev_ptr(jobs_t), n_jobs,
-                                                    _host_ptr(groups), len(groups), int(fmt), _dev_ptr(out_t),
-                                                    out_t.numel() * out_t.element_size(), _dev_ptr(results_t), _dev_ptr(status_t), ctypes.byref(rounds)))
-        return rounds.value
+        return self._batch_decode_dev(self._lib.symgpu_mp3_decode_dev, (), (MP3_JOB_DTYPE, MP3_GROUP_DTYPE, MP3_RESULT_DTYPE), True,
+                                data_t, jobs_t, groups, fmt, out_t, results_t, status_t)
 
-    # -- AAC-LC decoded on the device -------------------------------------------------------------------
     def aac_decode_host(self, data, jobs, groups, fmt, out_samples, out=None):
         """Device AAC-LC decoding of many files in one call: `data` (bytes / uint8 array) holds the raw_data_blocks, jobs PIECE_DTYPE
         (one per packet), groups AAC_GROUP_DTYPE (one per file: its jobs, sample rate, channels, state slot and output offset).
         Returns (out [out_samples] of `fmt`, results AAC_RESULT_DTYPE [groups], status uint8 [jobs], n_redecoded); file g's samples
         are out[out_offset:][:frames * channels]."""
         from ._native import AAC_GROUP_DTYPE, AAC_RESULT_DTYPE, PIECE_DTYPE
-        a = _byte_view(data)
-        jobs = np.ascontiguousarray(jobs, dtype=PIECE_DTYPE)
-        groups = np.ascontiguousarray(groups, dtype=AAC_GROUP_DTYPE)
-        if out is None:
-            out = np.zeros(int(out_samples), dtype=FMT_NUMPY[fmt])
-        assert out.flags.c_contiguous
-        results = np.zeros(len(groups), dtype=AAC_RESULT_DTYPE)
-        status = np.zeros(len(jobs), dtype=np.uint8)
-        redone = ctypes.c_uint32(0)
-        self._check(self._lib.symgpu_aac_decode_host(self._ctx, _host_ptr(a), a.size, _host_ptr(jobs), len(jobs), _host_ptr(groups), len(groups),
-                                                     int(fmt), _host_ptr(out), out.nbytes, _host_ptr(results), _host_ptr(status), ctypes.byref(redone)))
-        return out, results, status, redone.value
+        return self._batch_decode_host(self._lib.symgpu_aac_decode_host, (), (PIECE_DTYPE, AAC_GROUP_DTYPE, AAC_RESULT_DTYPE), True,
+                                 data, jobs, groups, fmt, out_samples, out)
 
     def aac_decode_dev(self, data_t, jobs_t, groups, fmt, out_t, results_t, status_t):
         """Device-resident variant: torch CUDA tensors (uint8 bytes, jobs / results as uint8 views of the records, `out` of the format's
         element size, uint8 status); `groups` stays a host array.  Waits for the engine's stream for one 8-byte readback (and once
         more when pulses need the host); the synthesis and the output stage are left queued on it.  Returns n_redecoded."""
         from ._native import AAC_GROUP_DTYPE, AAC_RESULT_DTYPE, PIECE_DTYPE
-        ts = (data_t, jobs_t, out_t, results_t, status_t)
-        assert all(t.is_cuda and t.is_contiguous() for t in ts)
-        groups = np.ascontiguousarray(groups, dtype=AAC_GROUP_DTYPE)
-        n_jobs = jobs_t.numel() * jobs_t.element_size() // PIECE_DTYPE.itemsize
-        assert results_t.numel() * results_t.element_size() >= len(groups) * AAC_RESULT_DTYPE.itemsize and status_t.numel() >= n_jobs
-        redone = ctypes.c_uint32(0)
-        self._check(self._lib.symgpu_aac_decode_dev(self._ctx, _dev_ptr(data_t), data_t.numel(), _dev_ptr(jobs_t), n_jobs,
-                                                    _host_ptr(groups), len(groups), int(fmt), _dev_ptr(out_t),
-                                                    out_t.numel() * out_t.element_size(), _dev_ptr(results_t), _dev_ptr(status_t), ctypes.byref(redone)))
-        return redone.value
+        return self._batch_decode_dev(self._lib.symgpu_aac_decode_dev, (), (PIECE_DTYPE, AAC_GROUP_DTYPE, AAC_RESULT_DTYPE), True,
+                                data_t, jobs_t, groups, fmt, out_t, results_t, status_t)
+
+    @staticmethod
+    def _vorbis_setup_args(headers, setups):
+        """The leading arguments of symgpu_vorbis_decode_host / _dev: the header bytes and the setups that name them."""
+        from ._native import VORBIS_SETUP_REF_DTYPE
+        h = _byte_view(headers)
+        setups = np.ascontiguousarray(setups, dtype=VORBIS_SETUP_REF_DTYPE)
+        return _host_ptr(h), h.size, _host_ptr(setups), len(setups)   # (a numpy pointer keeps its array alive)
 
     def vorbis_decode_host(self, headers, setups, data, jobs, groups, fmt, out_samples, out=None):
         """Device Ogg Vorbis decoding of many files in one call: `headers` (bytes) holds the identification / setup packets that
@@ -370,37 +357,17 @@ class Engine:
         packet, with the reader's discard / end trim), groups VORBIS_GROUP_DTYPE (one per file: its jobs, setup and output
         offset).  Returns (out [out_samples] of `fmt`, results VORBIS_RESULT_DTYPE [groups], status uint8 [jobs]); file g's
         samples are out[out_offset:][:frames * channels].  Replaces the engine's Vorbis stream and floor registration."""
-        from ._native import VORBIS_GROUP_DTYPE, VORBIS_JOB_DTYPE, VORBIS_RESULT_DTYPE, VORBIS_SETUP_REF_DTYPE
-        h = _byte_view(headers)
-        a = _byte_view(data)
-        setups = np.ascontiguousarray(setups, dtype=VORBIS_SETUP_REF_DTYPE)
-        jobs = np.ascontiguousarray(jobs, dtype=VORBIS_JOB_DTYPE)
-        groups = np.ascontiguousarray(groups, dtype=VORBIS_GROUP_DTYPE)
-        if out is None:
-            out = np.zeros(int(out_samples), dtype=FMT_NUMPY[fmt])
-        assert out.flags.c_contiguous
-        results = np.zeros(len(groups), dtype=VORBIS_RESULT_DTYPE)
-        status = np.zeros(len(jobs), dtype=np.uint8)
-        self._check(self._lib.symgpu_vorbis_decode_host(self._ctx, _host_ptr(h), h.size, _host_ptr(setups), len(setups), _host_ptr(a), a.size,
-                                                        _host_ptr(jobs), len(jobs), _host_ptr(groups), len(groups), int(fmt),
-                                                        _host_ptr(out), out.nbytes, _host_ptr(results), _host_ptr(status)))
-        return out, results, status
+        from ._native import VORBIS_GROUP_DTYPE, VORBIS_JOB_DTYPE, VORBIS_RESULT_DTYPE
+        return self._batch_decode_host(self._lib.symgpu_vorbis_decode_host, self._vorbis_setup_args(headers, setups),
+                                 (VORBIS_JOB_DTYPE, VORBIS_GROUP_DTYPE, VORBIS_RESULT_DTYPE), False, data, jobs, groups, fmt, out_samples, out)
 
     def vorbis_decode_dev(self, headers, setups, data_t, jobs_t, groups, fmt, out_t, results_t, status_t):
         """Device-resident variant: torch CUDA tensors (uint8 bytes, jobs / results as uint8 views of the records, `out` of the
         format's element size, uint8 status); `headers`, `setups` and `groups` stay on the host.  The host waits only for the
         stream / floor registration; the decode, the synthesis and the output stage are left queued on the engine's stream."""
-        from ._native import VORBIS_GROUP_DTYPE, VORBIS_JOB_DTYPE, VORBIS_RESULT_DTYPE, VORBIS_SETUP_REF_DTYPE
-        ts = (data_t, jobs_t, out_t, results_t, status_t)
-        assert all(t.is_cuda and t.is_contiguous() for t in ts)
-        h = _byte_view(headers)
-        setups = np.ascontiguousarray(setups, dtype=VORBIS_SETUP_REF_DTYPE)
-        groups = np.ascontiguousarray(groups, dtype=VORBIS_GROUP_DTYPE)
-        n_jobs = jobs_t.numel() * jobs_t.element_size() // VORBIS_JOB_DTYPE.itemsize
-        assert results_t.numel() * results_t.element_size() >= len(groups) * VORBIS_RESULT_DTYPE.itemsize and status_t.numel() >= n_jobs
-        self._check(self._lib.symgpu_vorbis_decode_dev(self._ctx, _host_ptr(h), h.size, _host_ptr(setups), len(setups), _dev_ptr(data_t), data_t.numel(),
-                                                       _dev_ptr(jobs_t), n_jobs, _host_ptr(groups), len(groups), int(fmt), _dev_ptr(out_t),
-                                                       out_t.numel() * out_t.element_size(), _dev_ptr(results_t), _dev_ptr(status_t)))
+        from ._native import VORBIS_GROUP_DTYPE, VORBIS_JOB_DTYPE, VORBIS_RESULT_DTYPE
+        self._batch_decode_dev(self._lib.symgpu_vorbis_decode_dev, self._vorbis_setup_args(headers, setups),
+                         (VORBIS_JOB_DTYPE, VORBIS_GROUP_DTYPE, VORBIS_RESULT_DTYPE), False, data_t, jobs_t, groups, fmt, out_t, results_t, status_t)
 
     # -- Ogg pages indexed on the device --------------------------------------------------------
     def ogg_index_dev(self, data_t, ranges, cap_packets=None, cap_pieces=None):
@@ -439,6 +406,24 @@ class Engine:
                                                    packets_t.numel() // OGG_PACKET_DTYPE.itemsize, _dev_ptr(pieces_t),
                                                    pieces_t.numel() // PIECE_DTYPE.itemsize, _dev_ptr(index_t)))
 
+    def _index_dev(self, queue, data_t, ranges, cap, min_frame, per_cap, per_file):
+        """Allocate, queue, wait and read back, for a device index whose queue(data_t, ranges, cap, *tables, *records) writes
+        `cap` records of each dtype of per_cap (None: that table is not written) and one record per file of each dtype of
+        per_file.  cap=None: the lengths // min_frame, summed.  Returns the tables, on the device, and the records, read back.
+        adts_index_dev, mpa_index_dev and the device-files decoders of decode.py index through it."""
+        import torch
+        assert data_t.is_cuda and data_t.is_contiguous() and data_t.dtype == torch.uint8
+        r = file_ranges(ranges)
+        if cap is None:
+            cap = int((r["len"] // min_frame).sum())
+        d = data_t.device
+        kept = [None if dt is None else torch.empty(cap * dt.itemsize, dtype=torch.uint8, device=d) for dt in per_cap]
+        read = [torch.empty(len(r) * dt.itemsize, dtype=torch.uint8, device=d) for dt in per_file]
+        torch.cuda.current_stream(d).synchronize()  # data_t and the outputs are torch's: written / allocated on its stream
+        queue(data_t, r, cap, *kept, *read)
+        self.sync()
+        return (*kept, *(t.cpu().numpy().view(dt) for t, dt in zip(read, per_file)))
+
     # -- ADTS frames indexed on the device ---------------------------------------------------------
     def adts_index_dev(self, data_t, ranges, cap=None):
         """(packets_t, jobs_t, index) for the files data_t[offset : offset + len] of `ranges` (FILE_RANGE_DTYPE records, or
@@ -446,20 +431,8 @@ class Engine:
         records on the device, index the files' ADTS_FILE_INDEX_DTYPE records on the host.  File i's packets, [first_packet,
         first_packet + n_packets), equal packetizer.adts_index of its bytes, with its stop; its jobs are the same payloads as
         byte ranges of data_t.  cap=None: the lengths // 7, summed, which every file fits (a frame is at least 7 bytes)."""
-        import torch
         from ._native import ADTS_FILE_INDEX_DTYPE, ADTS_PACKET_DTYPE, PIECE_DTYPE
-        assert data_t.is_cuda and data_t.is_contiguous() and data_t.dtype == torch.uint8
-        r = file_ranges(ranges)
-        if cap is None:
-            cap = int((r["len"] // 7).sum())
-        d = data_t.device
-        packets_t = torch.empty(cap * ADTS_PACKET_DTYPE.itemsize, dtype=torch.uint8, device=d)
-        jobs_t = torch.empty(cap * PIECE_DTYPE.itemsize, dtype=torch.uint8, device=d)
-        index_t = torch.empty(len(r) * ADTS_FILE_INDEX_DTYPE.itemsize, dtype=torch.uint8, device=d)
-        torch.cuda.current_stream(d).synchronize()  # data_t and the outputs are torch's: written / allocated on its stream
-        self.adts_index_dev_queue(data_t, r, cap, packets_t, jobs_t, index_t)
-        self.sync()
-        return packets_t, jobs_t, index_t.cpu().numpy().view(ADTS_FILE_INDEX_DTYPE)
+        return self._index_dev(self.adts_index_dev_queue, data_t, ranges, cap, 7, (ADTS_PACKET_DTYPE, PIECE_DTYPE), (ADTS_FILE_INDEX_DTYPE,))
 
     def adts_index_dev_queue(self, data_t, ranges, cap, packets_t, jobs_t, index_t):
         """symgpu_adts_index_dev on uint8 CUDA tensors (packets_t / jobs_t, either None, holding `cap` records; index_t one record
@@ -480,21 +453,9 @@ class Engine:
         File i's track and packets, [first_packet, first_packet + n_packets), equal packetizer.mpa_index(bytes, seekable) (status
         MPA_NO_FRAME where that raises); its jobs are the same frames as byte ranges of data_t.  cap=None: the lengths // 24, summed,
         which every file fits (a frame is at least 24 bytes)."""
-        import torch
         from ._native import MP3_JOB_DTYPE, MPA_FILE_INDEX_DTYPE, MPA_MIN_FRAME, MPA_PACKET_DTYPE, MPA_TRACK_DTYPE
-        assert data_t.is_cuda and data_t.is_contiguous() and data_t.dtype == torch.uint8
-        r = file_ranges(ranges)
-        if cap is None:
-            cap = int((r["len"] // MPA_MIN_FRAME).sum())
-        d = data_t.device
-        packets_t = torch.empty(cap * MPA_PACKET_DTYPE.itemsize, dtype=torch.uint8, device=d)
-        jobs_t = torch.empty(cap * MP3_JOB_DTYPE.itemsize, dtype=torch.uint8, device=d)
-        index_t = torch.empty(len(r) * MPA_FILE_INDEX_DTYPE.itemsize, dtype=torch.uint8, device=d)
-        tracks_t = torch.empty(len(r) * MPA_TRACK_DTYPE.itemsize, dtype=torch.uint8, device=d)
-        torch.cuda.current_stream(d).synchronize()  # data_t and the outputs are torch's: written / allocated on its stream
-        self.mpa_index_dev_queue(data_t, r, cap, packets_t, jobs_t, index_t, tracks_t, seekable)
-        self.sync()
-        return packets_t, jobs_t, index_t.cpu().numpy().view(MPA_FILE_INDEX_DTYPE), tracks_t.cpu().numpy().view(MPA_TRACK_DTYPE)
+        return self._index_dev(lambda *args: self.mpa_index_dev_queue(*args, seekable), data_t, ranges, cap, MPA_MIN_FRAME,
+                               (MPA_PACKET_DTYPE, MP3_JOB_DTYPE), (MPA_FILE_INDEX_DTYPE, MPA_TRACK_DTYPE))
 
     def mpa_index_dev_queue(self, data_t, ranges, cap, packets_t, jobs_t, index_t, tracks_t, seekable=True):
         """symgpu_mpa_index_dev on uint8 CUDA tensors (packets_t / jobs_t, either None, holding `cap` records; index_t and tracks_t
