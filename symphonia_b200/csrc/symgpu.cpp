@@ -282,6 +282,20 @@ symgpu_status build_plan(symgpu_ctx* ctx, const symgpu_mp3_run* runs, uint32_t n
                           n_runs, n_frames, plan, whole_batch);
 }
 
+// The Layer I / II plan for a grid of `grid` CTAs: whole frames are the planner's units, mpa12_tile_frames(n_slots) of them per
+// tile (a halo tile too), no groups.
+symgpu_status mpa12_plan_for(int grid, uint32_t n_streams, const symgpu_mpa12_run* runs, uint32_t n_runs, uint32_t n_frames,
+                             uint32_t n_slots, Mp3Plan& plan) {
+    if (n_slots != 12 && n_slots != 36) return SYMGPU_ERR_ARG;
+    std::vector<symgpu_mp3_run> as_frames(n_runs); // units of the planner = frames
+    for (uint32_t r = 0; r < n_runs; ++r) {
+        if (runs[r].reserved[0] || runs[r].reserved[1] || runs[r].reserved[2]) return SYMGPU_ERR_ARG;
+        as_frames[r] = symgpu_mp3_run{runs[r].stream, runs[r].first_frame, runs[r].n_frames, 1, runs[r].channels, 0};
+    }
+    const uint32_t T = (uint32_t)mpa12_tile_frames((int)n_slots);
+    return build_plan_for(grid, T, T, false, n_streams, as_frames.data(), n_runs, n_frames, plan, true);
+}
+
 // Launches the Layer III kernel the context is configured for over a plan whose entries sit at `d_plan`.
 cudaError_t launch_plan(symgpu_ctx* ctx, const Mp3Tile* d_plan, int hdr, int n_tiles, int n_ctas, bool multi, bool v2,
                         const symgpu_mp3_gc* units, const float* spectra, float* pcm, cudaStream_t stream) {
@@ -433,6 +447,24 @@ size_t symgpu_debug_mp3_plan_v2(int max_shares, uint32_t n_streams, const symgpu
     if (build_plan_v2_for(max_shares, n_streams, runs, n_runs, n_frames, plan, true) != SYMGPU_OK) return 0;
     if (out) std::memcpy(out, plan.buf.data(), std::min(cap, plan.buf.size()) * sizeof(Mp3Tile));
     if (n_shares) *n_shares = plan.n_ctas;
+    if (n_tiles) *n_tiles = plan.n_tiles;
+    if (hdr) *hdr = plan.hdr;
+    return plan.buf.size();
+}
+
+// Same for Layer I / II (n_slots 12 / 36): the plan symgpu_mpa12_synth_dev launches.  grid <= 0: the grid of a launch on the
+// current device (needs one); 0 on an argument error or when that grid cannot be found.
+size_t symgpu_debug_mpa12_plan(int grid, uint32_t n_streams, const symgpu_mpa12_run* runs, uint32_t n_runs, uint32_t n_frames,
+                               uint32_t n_slots, void* out, size_t cap, int* n_ctas, int* n_tiles, int* hdr) {
+    if (grid <= 0) {
+        cudaError_t ce = cudaSuccess;
+        grid = mp3_grid_size(&ce);
+        if (ce != cudaSuccess || grid <= 0) return 0;
+    }
+    Mp3Plan plan;
+    if (mpa12_plan_for(grid, n_streams, runs, n_runs, n_frames, n_slots, plan) != SYMGPU_OK) return 0;
+    if (out) std::memcpy(out, plan.buf.data(), std::min(cap, plan.buf.size()) * sizeof(Mp3Tile));
+    if (n_ctas) *n_ctas = plan.n_ctas;
     if (n_tiles) *n_tiles = plan.n_tiles;
     if (hdr) *hdr = plan.hdr;
     return plan.buf.size();
@@ -1091,13 +1123,7 @@ static symgpu_status mpa12_plan(symgpu_ctx* ctx, const symgpu_mpa12_run* runs, u
     cudaError_t ce = cudaSuccess;
     const int grid = mp3_grid_size(&ce);
     if (ce != cudaSuccess || grid <= 0) return cuda_fail(ctx, ce, "mp3_grid_size");
-    std::vector<symgpu_mp3_run> as_frames(n_runs); // units of the planner = frames
-    for (uint32_t r = 0; r < n_runs; ++r) {
-        if (runs[r].reserved[0] || runs[r].reserved[1] || runs[r].reserved[2]) return SYMGPU_ERR_ARG;
-        as_frames[r] = symgpu_mp3_run{runs[r].stream, runs[r].first_frame, runs[r].n_frames, 1, runs[r].channels, 0};
-    }
-    const uint32_t T = (uint32_t)mpa12_tile_frames((int)n_slots);
-    return build_plan_for(grid, T, T, false, ctx->n_mp3_streams, as_frames.data(), n_runs, n_frames, plan, true);
+    return mpa12_plan_for(grid, ctx->n_mp3_streams, runs, n_runs, n_frames, n_slots, plan);
 }
 
 symgpu_status symgpu_mpa12_synth_dev(symgpu_ctx* ctx, const float* subbands, const symgpu_mpa12_run* runs, uint32_t n_runs,
