@@ -1307,6 +1307,43 @@ symgpu_status symgpu_flac_decode_fmt_dev(symgpu_ctx* ctx, const uint8_t* bytes, 
                                          uint64_t* group_frames, uint8_t* status);
 
 /* ===================================================================================================
+ * FLAC frames indexed on the device (DESIGN 5b): many native FLAC files already in device memory, one call.  The metadata walk,
+ * the header rules and the CRC-16 that proves a frame's end are those of symgpu_flac_index, as the same host / device code
+ * (packetizer.hpp).  No file's frames are walked by one thread: every sync position gets its CRC key from per-tile CRC states
+ * combined by a scan, each frame's end is found by a binary search among the positions sorted by key and a descent of a max tree,
+ * and the frame chain is ranked by pointer doubling, in rounds logarithmic in the longest file.  Only open()'s metadata walk runs
+ * one thread per file.
+ * ================================================================================================= */
+#define SYMGPU_FLAC_MAX_FILES 65536
+typedef struct symgpu_flac_file_index { /* 24 bytes: one file's share of the tables                                     */
+    uint64_t first_packet;   /* its packets start here in `packets` and `jobs` (the n_packets of the files before it, summed) */
+    uint64_t samples;        /* its packets' dur, summed                                                                */
+    uint32_t n_packets;
+    uint8_t open;            /* what symgpu_flac_index returns for these bytes: SYMGPU_OK, SYMGPU_ERR_UNSUPPORTED (no "fLaC")
+                                or SYMGPU_ERR_DECODE (bad or missing STREAMINFO, cut metadata)                          */
+    uint8_t status;          /* SYMGPU_FLAC_NOT_WRITTEN: first_packet + n_packets passes the capacity, so none of the
+                                file's packets and jobs were written                                                    */
+    uint8_t reserved[2];
+} symgpu_flac_file_index;
+enum { SYMGPU_FLAC_NOT_WRITTEN = 1 };
+/* For every file data[files[i].offset ..][.. len): what symgpu_flac_index returns for those bytes alone -- infos[i] byte for byte
+ * (zeros when the file does not open), its packets at packets[index[i].first_packet ..] with offsets relative to the file's first
+ * byte, and the same frames at jobs[...] as symgpu_flac_job records with absolute offsets into data, group = i and slot = dur
+ * (what symgpu_flac_decode_fmt_dev takes).  packets and jobs hold cap_packets records each; either may be NULL.  data, packets,
+ * jobs, index and infos are device memory; files host memory.  SYMGPU_ERR_ARG for a range outside data[0 .. n_bytes) or a
+ * missing pointer, SYMGPU_ERR_LIMIT for more than SYMGPU_FLAC_MAX_FILES files or a file of 2^32 bytes or more; both before
+ * anything is launched.  A frame is at least 8 bytes, so a capacity of the files' lengths / 8, summed, always suffices: one
+ * call.  No file: no launch.  Otherwise 28 + 2 T + R launches, T = bit_length(L / 2) and R = bit_length(L / 8) for the longest
+ * file's length L, whatever the number of files, and one host wait, for the 8-byte number of nodes (sync positions and one end
+ * per file), which sizes the scratch from the context's staging buffer: about 130 bytes per node, about 100 per file and 12
+ * per 4 KiB of file bytes.  SYMGPU_ERR_LIMIT, after that wait, for 2^32 - 1 nodes or more.  The call returns with the rest
+ * queued. */
+symgpu_status symgpu_flac_index_dev(symgpu_ctx* ctx, const uint8_t* data, size_t n_bytes, const symgpu_file_range* files, size_t n_files,
+                                    symgpu_flac_packet* packets, symgpu_flac_job* jobs, size_t cap_packets, symgpu_flac_file_index* index,
+                                    symgpu_flac_stream_info* infos);
+
+
+/* ===================================================================================================
  * Vorbis entropy front-end (SURVEY 8f N1): audio packets -> the batch format of symgpu_vorbis_synth_* (unit, floor-1 Y
  * values, residue vectors BEFORE inverse coupling).  CPU only; one object per stream (codebooks, setup, previous block).
  *   VorbisCodebook::read, synthesize_codewords, VQ unpack   symphonia-codec-vorbis/src/codebook.rs:16-400

@@ -10,9 +10,9 @@
 // skipped as junk, which frames are tags, how packets continue across pages, where the time stamps and trims come
 // from) are the reference's, cited at each function, and are checked bit for bit against oracle/packetizer_oracle.py.
 //
-// Header-only C++17, no dependencies.  The MPEG and ADTS rules are also device functions when the header is compiled by nvcc
-// (SYMGPU_PACKET_HD), so the Layer I / II device decoder and the device MPEG and ADTS indexes parse headers and tags with this
-// very code; C++ compilers see plain inline functions.
+// Header-only C++17, no dependencies.  The MPEG, ADTS and FLAC rules are also device functions when the header is compiled by nvcc
+// (SYMGPU_PACKET_HD), so the Layer I / II device decoder and the device MPEG, ADTS and FLAC indexes parse headers and tags with
+// this very code; C++ compilers see plain inline functions.
 #pragma once
 #include <algorithm>
 #include <cstddef>
@@ -1769,7 +1769,9 @@ struct FlacStreamInfo {  // symphonia-common/src/xiph/audio/flac/mod.rs:78-186
     bool has_md5;
 };
 
-inline Status flac_read_stream_info(const uint8_t* p, size_t n, FlacStreamInfo& si) {
+// The FLAC rules below are host / device functions: FlacIndexer (symgpu_flac_index) and the device index (symgpu_flac_index_dev,
+// flac_index_kernel.cu) run this very code.  No memcmp / memchr and no double arithmetic in them.
+SYMGPU_PACKET_HD inline Status flac_read_stream_info(const uint8_t* p, size_t n, FlacStreamInfo& si) {
     if (n < 34) return Status::EndOfStream;
     si.block_min = uint16_t(detail::be16(p)), si.block_max = uint16_t(detail::be16(p + 2));
     if (si.block_min < 16 || si.block_max < 16 || si.block_max < si.block_min) return Status::DecodeError;
@@ -1782,13 +1784,38 @@ inline Status flac_read_stream_info(const uint8_t* p, size_t n, FlacStreamInfo& 
     si.bits_per_sample = uint8_t(((bits >> 36) & 31) + 1);
     if (si.bits_per_sample < 4) return Status::DecodeError;
     si.n_samples = bits & 0xfffffffffull;
-    std::memcpy(si.md5, p + 18, 16);
     si.has_md5 = false;
-    for (int k = 0; k < 16; ++k) si.has_md5 |= si.md5[k] != 0;
+    for (int k = 0; k < 16; ++k) si.md5[k] = p[18 + k], si.has_md5 |= p[18 + k] != 0;
     return Status::Ok;
 }
 
-inline uint8_t crc8_ccitt(const uint8_t* p, size_t n) {  // polynomial 0x07 (symphonia-core/src/checksum/crc8.rs:32-65)
+// demuxer.rs:60-170: the stream marker, then metadata blocks up to the one flagged last; the first must be STREAMINFO.  On Ok,
+// *first_frame is where the frames begin.  A walk over the block headers, one thread per file on the device.
+SYMGPU_PACKET_HD inline Status flac_open(const uint8_t* d, size_t n, FlacStreamInfo& info, size_t* first_frame) {
+    if (n < 4 || d[0] != 'f' || d[1] != 'L' || d[2] != 'a' || d[3] != 'C') return Status::Unsupported;
+    size_t at = 4;
+    bool first = true;
+    for (;;) {
+        if (at + 4 > n) return Status::EndOfStream;
+        const bool last = d[at] & 0x80;
+        const unsigned type = d[at] & 0x7f;
+        const size_t len = detail::be24(d + at + 1);
+        at += 4;
+        if (at + len > n) return Status::EndOfStream;
+        if (first) {
+            if (type != 0 || len != 34) return Status::DecodeError;
+            const Status s = flac_read_stream_info(d + at, len, info);
+            if (s != Status::Ok) return s;
+            first = false;
+        }
+        at += len;
+        if (last) break;
+    }
+    *first_frame = at;
+    return Status::Ok;
+}
+
+SYMGPU_PACKET_HD inline uint8_t crc8_ccitt(const uint8_t* p, size_t n) {  // polynomial 0x07 (symphonia-core/src/checksum/crc8.rs:32-65)
     uint8_t c = 0;
     for (size_t i = 0; i < n; ++i) {
         c ^= p[i];
@@ -1808,11 +1835,37 @@ struct Crc16Msb {
     }
 };
 }  // namespace detail
-inline uint16_t crc16_ansi_update(uint16_t state, const uint8_t* p, size_t n) {  // polynomial 0x8005, most-significant bit first
-    static constexpr detail::Crc16Msb tab{};
-    for (size_t i = 0; i < n; ++i) state = uint16_t((state << 8) ^ tab.t[(state >> 8) ^ p[i]]);
+// CRC-16, polynomial 0x8005, most-significant bit first, init 0, no final xor (the FLAC frame footer).  `t` is
+// detail::Crc16Msb::t: the device keeps its copy in constant memory.
+SYMGPU_PACKET_HD inline uint16_t crc16_ansi_update_with(const uint16_t* t, uint16_t state, const uint8_t* p, size_t n) {
+    for (size_t i = 0; i < n; ++i) state = uint16_t((state << 8) ^ t[(state >> 8) ^ p[i]]);
     return state;
 }
+inline const uint16_t* crc16_ansi_table() {
+    static constexpr detail::Crc16Msb tab{};
+    return tab.t;
+}
+inline uint16_t crc16_ansi_update(uint16_t state, const uint8_t* p, size_t n) { return crc16_ansi_update_with(crc16_ansi_table(), state, p, n); }
+
+// The CRC-16 state as an element of GF(2)[x] / (x^16 + x^15 + x^2 + 1): a zero byte multiplies it by x^8, so the state of A || B is
+// crc(A) x^(8 |B|) + crc(B).  a x b in that ring:
+SYMGPU_PACKET_HD inline uint16_t crc16_mulmod(uint16_t a, uint16_t b) {
+    uint32_t p = 0;
+    for (int i = 0; i < 16; ++i)
+        if ((b >> i) & 1) p ^= uint32_t(a) << i;
+    for (int i = 30; i >= 16; --i)
+        if ((p >> i) & 1) p ^= 0x18005u << (i - 16);
+    return uint16_t(p);
+}
+// x^(8 k): what k zero bytes multiply a state by.
+SYMGPU_PACKET_HD inline uint16_t crc16_xpow8(uint64_t k) {
+    uint16_t r = 1, base = 0x100;
+    for (; k; k >>= 1, base = crc16_mulmod(base, base))
+        if (k & 1) r = crc16_mulmod(r, base);
+    return r;
+}
+// (a, la) o (b, lb) = (x^(8 lb) a + b, la + lb): the state of two spans one after the other, from their states alone.
+SYMGPU_PACKET_HD inline uint16_t crc16_combine(uint16_t a, uint16_t b, uint64_t lb) { return uint16_t(crc16_mulmod(a, crc16_xpow8(lb)) ^ b); }
 
 struct FlacFrameHeader {
     uint64_t sequence;
@@ -1822,8 +1875,39 @@ struct FlacFrameHeader {
     uint8_t size;  // bytes, sync code to CRC-8
 };
 
+namespace detail {
+SYMGPU_PACKET_HD inline uint32_t flac_rate_code(unsigned sr) {  // codes 0-11
+    switch (sr) {
+        case 1: return 88200;
+        case 2: return 176400;
+        case 3: return 192000;
+        case 4: return 8000;
+        case 5: return 16000;
+        case 6: return 22050;
+        case 7: return 24000;
+        case 8: return 32000;
+        case 9: return 44100;
+        case 10: return 48000;
+        case 11: return 96000;
+        default: return 0;
+    }
+}
+SYMGPU_PACKET_HD inline uint32_t flac_depth_code(unsigned bd) {  // 255: reserved
+    switch (bd) {
+        case 1: return 8;
+        case 2: return 12;
+        case 3: return 255;
+        case 4: return 16;
+        case 5: return 20;
+        case 6: return 24;
+        case 7: return 32;
+        default: return 0;
+    }
+}
+}  // namespace detail
+
 // frame.rs:81-233 at p[0..n): false unless a complete header with a matching CRC-8 starts here.
-inline bool flac_parse_frame_header(const uint8_t* p, size_t n, FlacFrameHeader& h) {
+SYMGPU_PACKET_HD inline bool flac_parse_frame_header(const uint8_t* p, size_t n, FlacFrameHeader& h) {
     if (n < 6 || p[0] != 0xff || (p[1] & 0xfc) != 0xf8 || (p[3] & 1)) return false;
     size_t at = 4;
     h.by_sample = p[1] & 1;
@@ -1857,8 +1941,7 @@ inline bool flac_parse_frame_header(const uint8_t* p, size_t n, FlacFrameHeader&
         if (x == 0xffff) return false;
         h.block = x + 1;
     } else h.block = 256u << (bs - 8);
-    static constexpr uint32_t rates[12] = {0, 88200, 176400, 192000, 8000, 16000, 22050, 24000, 32000, 44100, 48000, 96000};
-    if (sr < 12) h.sample_rate = rates[sr];
+    if (sr < 12) h.sample_rate = detail::flac_rate_code(sr);
     else if (sr == 12) {
         if (at + 1 > n) return false;
         h.sample_rate = uint32_t(p[at++]) * 1000;
@@ -1869,9 +1952,8 @@ inline bool flac_parse_frame_header(const uint8_t* p, size_t n, FlacFrameHeader&
         at += 2;
     }
     if (sr != 0 && (h.sample_rate < 1 || h.sample_rate > 655350)) return false;
-    static constexpr uint8_t widths[8] = {0, 8, 12, 255, 16, 20, 24, 32};
-    if (widths[bd] == 255) return false;
-    h.bits_per_sample = widths[bd];
+    if (detail::flac_depth_code(bd) == 255) return false;
+    h.bits_per_sample = detail::flac_depth_code(bd);
     if (ch <= 7) h.channels = uint8_t(ch + 1);
     else if (ch <= 10) h.channels = 2;
     else return false;
@@ -1880,6 +1962,33 @@ inline bool flac_parse_frame_header(const uint8_t* p, size_t n, FlacFrameHeader&
     return true;
 }
 
+// parser.rs:586-648, the header against the stream: rate, depth, block size, channel count and blocking strategy.
+SYMGPU_PACKET_HD inline bool flac_fits_stream(const FlacFrameHeader& h, const FlacStreamInfo& info) {
+    if (h.sample_rate && h.sample_rate != info.sample_rate) return false;
+    if (h.bits_per_sample && h.bits_per_sample != info.bits_per_sample) return false;
+    if (h.block > info.block_max || h.channels != info.channels) return false;
+    const bool fixed = info.block_min == info.block_max;
+    return h.by_sample != fixed;
+}
+// A plausible frame start at d[q ..] of a file of n bytes: a header that parses, checks out and fits the stream.
+SYMGPU_PACKET_HD inline bool flac_plausible(const uint8_t* d, size_t n, size_t q, const FlacStreamInfo& info, FlacFrameHeader& h) {
+    return q + 6 <= n && flac_parse_frame_header(d + q, n - q, h) && flac_fits_stream(h, info);
+}
+// The sequence rule: a header follows a frame numbered last_seq when its number is larger, or 0.
+SYMGPU_PACKET_HD inline bool flac_follows(uint64_t seq, uint64_t last_seq) { return seq > last_seq || seq == 0; }
+// v(h): the number the sequence rule compares, with 0 (which follows everything) as the largest.
+SYMGPU_PACKET_HD inline uint64_t flac_value(uint64_t seq) { return seq == 0 ? ~uint64_t(0) : seq; }
+
+// parser.rs:566-584: the frame's first sample.
+SYMGPU_PACKET_HD inline uint64_t flac_packet_ts(const FlacFrameHeader& h, const FlacStreamInfo& info) {
+    const bool fixed = info.block_min == info.block_max;
+    return h.by_sample ? h.sequence : h.sequence * (fixed ? info.block_min : h.block);
+}
+
+constexpr size_t kFlacMaxFrame = 16u * 1024 * 1024;  // frame.rs:17: how far past its start a frame's end is looked for
+// The smallest frame: a 6-byte header and the 2-byte CRC-16, so a file of n bytes holds at most n / 8 packets.
+constexpr uint32_t kFlacMinFrame = 8;
+
 struct FlacPacket {
     uint64_t offset;
     uint32_t size;
@@ -1887,32 +1996,157 @@ struct FlacPacket {
     uint32_t dur;  // block size
 };
 
+// ---- the splitter as a chain: shared by FlacIndexer and the device index (symgpu_flac_index_dev) -------------------------------
+// FlacIndexer::next is sequential, but what it returns is a function of each frame start alone (DESIGN §5b).  The files of a
+// device call lie back to back in one virtual byte space; its nodes, in position order, are
+//   * every sync position q of a file (q + 2 <= n, d[q] = 0xff, d[q + 1] & 0xfc = 0xf8), and
+//   * one end node per non-empty file, stored at its last byte q = n - 1 (never a sync position) and standing for position n.
+// A node is named by its 32-bit index in that order; npos is the file position it stands for.
+SYMGPU_PACKET_HD inline bool flac_is_sync(const uint8_t* d, size_t n, size_t q) { return q + 2 <= n && d[q] == 0xff && (d[q + 1] & 0xfc) == 0xf8; }
+constexpr uint32_t kFlacEndNode = 1;  // the node word of an end node (0: a sync position)
+SYMGPU_PACKET_HD inline bool flac_is_node(const uint8_t* d, size_t n, size_t q) { return q + 1 == n || flac_is_sync(d, n, q); }
+SYMGPU_PACKET_HD inline uint32_t flac_node(size_t n, size_t q) { return q + 1 == n ? kFlacEndNode : 0; }
+SYMGPU_PACKET_HD inline uint64_t flac_npos(const uint64_t* vpos, const uint32_t* node, uint32_t c, uint64_t vbase) {
+    return vpos[c] - vbase + (node[c] & kFlacEndNode);
+}
+constexpr uint32_t kFlacNone = 0xffffffffu;
+
+// The first node of [lo, hi) (one file's, starting at vbase) whose npos is at least x >= 1; hi when there is none.
+SYMGPU_PACKET_HD inline uint32_t flac_first_node_at(const uint64_t* vpos, const uint32_t* node, uint32_t lo, uint32_t hi, uint64_t vbase, uint64_t x) {
+    uint32_t i = detail::first_at_or_after(vpos, lo, hi, vbase + x - 1);
+    if (i < hi && !(node[i] & kFlacEndNode) && vpos[i] == vbase + x - 1) ++i;  // a sync position at x - 1 stands for itself
+    return i;
+}
+
+// 1. The CRC key.  key(x) = the CRC-16 state of file bytes [0, x), continued over n - x zero bytes.  With init 0 and no final xor,
+//    appending a frame's big-endian CRC-16 brings the state to 0, so crc16[s, q - 2) == be16(q - 2) exactly when
+//    key(s) == key(q).  key(x) is the xor of x^(8 (n - 1 - p)) crc(byte p) over p < x: an exclusive xor-scan.  A span [a, b) of
+//    the file contributes flac_key_part; a position q inside a span that began with prefix `pre` and has CRC state s over [a, q)
+//    has key pre ^ flac_key_inside.
+SYMGPU_PACKET_HD inline uint16_t flac_key_part(const uint16_t* t, const uint8_t* d, size_t n, size_t a, size_t b) {
+    return crc16_mulmod(crc16_ansi_update_with(t, 0, d + a, b - a), crc16_xpow8(n - b));
+}
+SYMGPU_PACKET_HD inline uint16_t flac_key_inside(uint16_t s, size_t n, size_t q) { return crc16_mulmod(s, crc16_xpow8(n - q)); }
+
+// 2. The search trees: a max tree over a table of values v[0 .. n) (level 0), level k holding the maxima of aligned runs of 2^k.
+//    flac_tree_levels(L) levels above level 0 make every query over one file of at most L bytes logarithmic: a file has at most
+//    L / 2 + 1 nodes.
+struct FlacTree {
+    const uint64_t* level[34];
+    uint32_t n, top;
+};
+SYMGPU_PACKET_HD inline uint32_t flac_tree_levels(uint64_t max_len) {
+    uint32_t k = 0;
+    for (uint64_t m = max_len / 2; m; m >>= 1) ++k;
+    return k;
+}
+SYMGPU_PACKET_HD inline uint64_t flac_tree_max(const uint64_t* below, uint64_t n_below, uint64_t j) {
+    const uint64_t a = below[2 * j], b = 2 * j + 1 < n_below ? below[2 * j + 1] : 0;
+    return a > b ? a : b;
+}
+// The first i of [a, b] with v[i] > thr, kFlacNone when there is none: up the tree past runs at most thr, then down into the first
+// run above it.  b - a < 2^top.
+SYMGPU_PACKET_HD inline uint32_t flac_first_above(const FlacTree& t, uint32_t a, uint32_t b, uint64_t thr) {
+    uint64_t i = a;
+    uint32_t k = 0;
+    while (i <= b && i < t.n) {  // nothing of [a, i) is above thr, and 2^k divides i
+        if (t.level[k][i >> k] > thr) {
+            while (k > 0) {
+                --k;
+                if (t.level[k][i >> k] <= thr) i += uint64_t(1) << k;
+            }
+            return i <= b ? uint32_t(i) : kFlacNone;
+        }
+        i += uint64_t(1) << k;
+        if (k < t.top && !((i >> k) & 1)) ++k;
+    }
+    return kFlacNone;
+}
+
+// 3. Each node's values.  A node is plausible when it is a sync position at or after the first frame of a file that opened, whose
+//    header flac_plausible accepts; ev (the end search's table) is flac_value of a plausible node, ~0 for an end node and 0 for the
+//    rest.
+struct FlacHead {
+    uint64_t seq;
+    uint32_t block;
+    uint8_t size, by_sample, plausible, reserved;
+};
+SYMGPU_PACKET_HD inline FlacHead flac_head(const uint8_t* d, size_t n, size_t q, uint32_t node, bool opened, size_t first_frame,
+                                           const FlacStreamInfo& info) {
+    FlacHead r{};
+    FlacFrameHeader h;
+    if (!(node & kFlacEndNode) && opened && q >= first_frame && flac_plausible(d, n, q, info, h))
+        r.seq = h.sequence, r.block = h.block, r.size = h.size, r.by_sample = h.by_sample, r.plausible = 1;
+    return r;
+}
+SYMGPU_PACKET_HD inline uint64_t flac_end_value(const FlacHead& h, uint32_t node) {
+    return (node & kFlacEndNode) ? ~uint64_t(0) : h.plausible ? flac_value(h.seq) : 0;
+}
+
+// 4. end(s) of the plausible node c at file position q (its file's nodes [c, c1), the last its end node): the first node of the
+//    window with c's key, at least size + 2 bytes on, that is the end node or follows c.  The window is FlacIndexer::next's
+//    kMaxFrame rule: the sync positions up to and including the first one past q + kFlacMaxFrame, and the end node only when no
+//    sync position lies past it.  The nodes with one key lie together in (skey, sid), sorted by key and, within a key, by node;
+//    the tree is over their ev.  Returns the end node, kFlacNone when there is none.
+SYMGPU_PACKET_HD inline uint32_t flac_key_lower(const uint32_t* skey, const uint32_t* sid, uint32_t n, uint32_t key, uint32_t id) {
+    uint32_t lo = 0, hi = n;
+    while (lo < hi) {
+        const uint32_t mid = lo + (hi - lo) / 2;
+        if (skey[mid] < key || (skey[mid] == key && sid[mid] < id)) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo;
+}
+SYMGPU_PACKET_HD inline uint32_t flac_end(const uint64_t* vpos, const uint32_t* node, uint32_t c, uint32_t c1, uint64_t vbase, const FlacHead& h,
+                                          uint32_t key, const uint32_t* skey, const uint32_t* sid, const FlacTree& tree) {
+    const uint64_t q = vpos[c] - vbase;
+    const uint32_t lo = flac_first_node_at(vpos, node, c + 1, c1, vbase, q + h.size + 2);
+    const uint32_t cut = flac_first_node_at(vpos, node, c + 1, c1, vbase, q + kFlacMaxFrame + 1);
+    const uint32_t hi = cut < c1 ? cut : c1 - 1;
+    if (lo > hi) return kFlacNone;
+    const uint32_t a = flac_key_lower(skey, sid, tree.n, key, lo), e = flac_key_lower(skey, sid, tree.n, key, hi + 1);
+    if (a >= e) return kFlacNone;
+    const uint32_t i = flac_first_above(tree, a, e - 1, h.seq);
+    return i == kFlacNone ? kFlacNone : sid[i];
+}
+
+// 5. good(c) = plausible with an end; the next frame's table gv is flac_value of a good node, 0 for the rest.  After the frame c
+//    (ending at its end node e) the next frame is the first good node of [e, c1) that follows c -- none (kAdtsEnd) when e is the
+//    end node.  A file's first frame is the first good node at or after its first frame position.  The successors form one chain
+//    per file, ranked by adts_double.
+SYMGPU_PACKET_HD inline uint32_t flac_successor(const uint32_t* node, uint32_t e, uint32_t c1, uint64_t seq, const FlacTree& good) {
+    if (e == kFlacNone || (node[e] & kFlacEndNode)) return kFlacNone;
+    return flac_first_above(good, e, c1 - 1, seq);
+}
+SYMGPU_PACKET_HD inline uint32_t flac_first_frame(const uint64_t* vpos, const uint32_t* node, uint32_t c0, uint32_t c1, uint64_t vbase,
+                                                  size_t first_frame, const FlacTree& good) {
+    const uint32_t a = flac_first_node_at(vpos, node, c0, c1, vbase, first_frame);
+    return a < c1 ? flac_first_above(good, a, c1 - 1, 0) : kFlacNone;
+}
+// The rounds that rank every chain of files of at most max_len bytes: a frame is at least 8 bytes.
+SYMGPU_PACKET_HD inline uint32_t flac_chain_rounds(uint64_t max_len) {
+    uint32_t k = 0;
+    for (uint64_t m = max_len / kFlacMinFrame; m; m >>= 1) ++k;
+    return k;
+}
+
+// 6. The packet of the chain node c at q, ending at file position end.
+SYMGPU_PACKET_HD inline FlacPacket flac_chain_packet(uint64_t q, uint64_t end, const FlacHead& h, const FlacStreamInfo& info) {
+    FlacFrameHeader fh{};
+    fh.sequence = h.seq, fh.by_sample = h.by_sample, fh.block = h.block;
+    FlacPacket p;
+    p.offset = q, p.size = uint32_t(end - q), p.dur = h.block, p.ts = flac_packet_ts(fh, info);
+    return p;
+}
+
 class FlacIndexer {
   public:
     FlacIndexer(const uint8_t* data, size_t n) : d_(data), n_(n) {}
 
-    // demuxer.rs:60-170: the stream marker, then metadata blocks up to the one flagged last; the first must be STREAMINFO.
     Status open() {
-        if (n_ < 4 || std::memcmp(d_, "fLaC", 4) != 0) return Status::Unsupported;
-        size_t at = 4;
-        bool first = true;
-        for (;;) {
-            if (at + 4 > n_) return Status::EndOfStream;
-            const bool last = d_[at] & 0x80;
-            const unsigned type = d_[at] & 0x7f;
-            const size_t len = detail::be24(d_ + at + 1);
-            at += 4;
-            if (at + len > n_) return Status::EndOfStream;
-            if (first) {
-                if (type != 0 || len != 34) return Status::DecodeError;
-                const Status s = flac_read_stream_info(d_ + at, len, info_);
-                if (s != Status::Ok) return s;
-                first = false;
-            }
-            at += len;
-            if (last) break;
-        }
-        pos_ = first_frame_ = at;
+        const Status s = flac_open(d_, n_, info_, &first_frame_);
+        if (s != Status::Ok) return s;
+        pos_ = first_frame_;
         have_last_ = false;
         return Status::Ok;
     }
@@ -1940,13 +2174,12 @@ class FlacIndexer {
                     crc = crc16_ansi_update(crc, d_ + done, q - 2 - done), done = q - 2;
                     if (crc == detail::be16(d_ + q - 2)) {
                         pk.offset = start, pk.size = uint32_t(q - start), pk.dur = h.block;
-                        const bool fixed = info_.block_min == info_.block_max;
-                        pk.ts = h.by_sample ? h.sequence : h.sequence * (fixed ? info_.block_min : h.block);
+                        pk.ts = flac_packet_ts(h, info_);
                         last_ = h, have_last_ = true, pos_ = q;
                         return Status::Ok;
                     }
                 }
-                if (at_end || q - start > kMaxFrame) break;
+                if (at_end || q - start > kFlacMaxFrame) break;
             }
             const size_t q = next_sync(start + 1);  // no end vouched for: this was not a frame
             skipped_ += q - start;
@@ -1966,30 +2199,22 @@ class FlacIndexer {
     }
 
   private:
-    static constexpr size_t kMaxFrame = 16u * 1024 * 1024;  // frame.rs:17
-
     size_t next_sync(size_t from) const {
         for (size_t q = from; q + 2 <= n_;) {
-            const void* hit = std::memchr(d_ + q, 0xff, n_ - q);
+            const void* hit = std::memchr(d_ + q, 0xff, n_ - q);  // (host only: the device visits every byte once in its tiles)
             if (!hit) break;
             q = size_t(static_cast<const uint8_t*>(hit) - d_);
+            if (flac_is_sync(d_, n_, q)) return q;
             if (q + 2 > n_) break;
-            if ((d_[q + 1] & 0xfc) == 0xf8) return q;
             ++q;
         }
         return n_;
     }
-    // A header at `at` that fits the stream (parser.rs:586-648) and follows `prev` (default: the last accepted frame).
+    // A header at `at` that fits the stream and follows `prev` (default: the last accepted frame).
     bool candidate(size_t at, FlacFrameHeader& h, const FlacFrameHeader* prev = nullptr) const {
-        if (at + 6 > n_ || !flac_parse_frame_header(d_ + at, n_ - at, h)) return false;
-        if (h.sample_rate && h.sample_rate != info_.sample_rate) return false;
-        if (h.bits_per_sample && h.bits_per_sample != info_.bits_per_sample) return false;
-        if (h.block > info_.block_max || h.channels != info_.channels) return false;
-        const bool fixed = info_.block_min == info_.block_max;
-        if (h.by_sample == fixed) return false;
+        if (!flac_plausible(d_, n_, at, info_, h)) return false;
         const FlacFrameHeader* before = prev ? prev : (have_last_ ? &last_ : nullptr);
-        const uint64_t last_seq = before ? before->sequence : 0;
-        return h.sequence > last_seq || h.sequence == 0;
+        return flac_follows(h.sequence, before ? before->sequence : 0);
     }
 
     const uint8_t* d_;

@@ -150,6 +150,13 @@ assert MPA_FILE_INDEX_DTYPE.itemsize == 16 and MP3_JOB_DTYPE == MPA12_JOB_DTYPE
 MPA_MAX_FILES = 65536
 MPA_NO_FRAME, MPA_NOT_WRITTEN = 1, 2
 MPA_MIN_FRAME = 24   # the smallest frame a header can express: the files' lengths / 24, summed, hold every packet
+# native FLAC frames indexed on the device: `symgpu_flac_file_index` (24 bytes); packets are FLAC_PACKET_DTYPE, jobs FLAC_JOB_DTYPE
+FLAC_FILE_INDEX_DTYPE = np.dtype([("first_packet", "<u8"), ("samples", "<u8"), ("n_packets", "<u4"), ("open", "u1"), ("status", "u1"),
+                                  ("reserved", "u1", (2,))])
+assert FLAC_FILE_INDEX_DTYPE.itemsize == 24
+FLAC_MAX_FILES = 65536
+FLAC_NOT_WRITTEN = 1
+FLAC_MIN_FRAME = 8   # a 6-byte header and the CRC-16: the files' lengths / 8, summed, hold every packet
 # Vorbis jobs built on the device: `symgpu_vorbis_file_heads` (32 bytes), `symgpu_vorbis_packet_rank` (24),
 # `symgpu_ogg_packet_ref` (16), `symgpu_vorbis_file_jobs` (40)
 VORBIS_FILE_HEADS_DTYPE = np.dtype([("audio_bytes", "<u8"), ("n_stream", "<u4"), ("ident_len", "<u4"), ("setup", "<u4"), ("setup_len", "<u4"),
@@ -350,6 +357,8 @@ def lib():
     L.symgpu_vorbis_fe_decode.argtypes = [vp, vp, sz, u32, u32, vp, vp, vp]
     L.symgpu_adts_index_dev.restype = ctypes.c_int
     L.symgpu_adts_index_dev.argtypes = [vp, vp, sz, vp, sz, vp, vp, sz, vp]
+    L.symgpu_flac_index_dev.restype = ctypes.c_int
+    L.symgpu_flac_index_dev.argtypes = [vp, vp, sz, vp, sz, vp, vp, sz, vp, vp]
     L.symgpu_mpa_index_dev.restype = ctypes.c_int
     L.symgpu_mpa_index_dev.argtypes = [vp, vp, sz, vp, sz, ctypes.c_int, vp, vp, sz, vp, vp]
     L.symgpu_ogg_index_dev.restype = ctypes.c_int

@@ -5,6 +5,7 @@
 
 #include "../../include/symgpu.h"
 #include "../../include/symgpu/packetizer.hpp"
+#include "flac_records.h"
 #include "mpa_records.h"
 
 using namespace symgpu::packet;
@@ -193,16 +194,11 @@ extern "C" symgpu_status symgpu_flac_index(const uint8_t* data, size_t n, symgpu
     FlacIndexer ix(data, n);
     const Status s = ix.open();
     if (s != Status::Ok) return *n_out = 0, s == Status::Unsupported ? SYMGPU_ERR_UNSUPPORTED : SYMGPU_ERR_DECODE;
-    const FlacStreamInfo& si = ix.info();
-    *info = symgpu_flac_stream_info{};
-    info->n_samples = si.n_samples, info->first_frame_pos = ix.first_frame_pos(), info->sample_rate = si.sample_rate;
-    info->frame_min = si.frame_min, info->frame_max = si.frame_max, info->block_min = si.block_min, info->block_max = si.block_max;
-    info->channels = si.channels, info->bits_per_sample = si.bits_per_sample, info->has_md5 = si.has_md5;
-    std::memcpy(info->md5, si.md5, 16);
+    *info = symgpu_detail::flac_info_record(ix.info(), ix.first_frame_pos());
     size_t count = 0;
     FlacPacket p;
     while (ix.next(p) == Status::Ok) {
-        if (count < cap) packets[count] = symgpu_flac_packet{p.offset, p.ts, p.size, p.dur};
+        if (count < cap) packets[count] = symgpu_detail::flac_packet_record(p);
         ++count;
     }
     *n_out = count;

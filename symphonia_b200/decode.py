@@ -677,6 +677,50 @@ def decode_flac_files(engine, files, threads=None, device=False, errors=None, fm
     return _per_file(out, groups, plan["failed"], lambda g: (int(group_frames[g]), int(groups[g]["channels"]), int(rates[g])))
 
 
+def decode_flac_files_dev(engine, data_t, ranges, fmt=nat.FMT_S32, errors=None, stats=None):
+    """decode_flac_files(engine, files, device=True, fmt=fmt) for native FLAC files already in device memory: file i is
+    data_t[offset : offset + len] of ranges[i] ((offset, len) pairs or FILE_RANGE_DTYPE records) in a uint8 CUDA tensor, and its
+    result and its message in errors[i] are what decode_flac_files gives for those bytes.  The frames are found on the device
+    (symgpu_flac_index_dev) into a job table the decode reads in place; only the per-file index records and stream infos, the
+    frames written per file and the per-packet status come back to the host.  stats: a dict that receives `read_back_bytes`, every
+    byte the call copies from the device.  At most 65 536 files."""
+    import torch
+
+    from .engine import SymgpuError
+    r = _resident_files(data_t, ranges, "decode_flac_files_dev", nat.FLAC_MAX_FILES)
+    n = len(r)
+    if n == 0:
+        return []
+    dev = data_t.device
+    # 1. every file's frames as jobs, the table sized by the bound (a frame is at least 8 bytes)
+    _, jobs_t, ix, infos = engine._index_dev(engine.flac_index_dev_queue, data_t, r, None, nat.FLAC_MIN_FRAME, (None, nat.FLAC_JOB_DTYPE),
+                                             (nat.FLAC_FILE_INDEX_DTYPE, nat.FLAC_STREAM_INFO_DTYPE))
+    messages = {i: f"SymgpuError: {SymgpuError(int(ix['open'][i]), 'symgpu_flac_index')}" for i in range(n) if ix["open"][i]}
+    if errors is not None:
+        errors.update(messages)
+    # 2. the groups, as flac_files_plan lays them out
+    groups = np.zeros(n, dtype=nat.FLAC_GROUP_DTYPE)
+    groups["channels"] = 1
+    parts = []
+    for i in range(n):
+        if i not in messages:
+            info = infos[i]
+            fields = dict(max_block=int(info["block_max"]), bits_per_sample=int(info["bits_per_sample"]), channels=int(info["channels"]))
+            parts.append((i, int(ix["n_packets"][i]), fields, int(ix["samples"][i]) * int(info["channels"])))
+    out_at, failed = _place(groups, parts, None)
+    # 3. the decode, on the job table in place
+    n_jobs = int(ix["first_packet"][-1]) + int(ix["n_packets"][-1])
+    groups_t = torch.from_numpy(groups.view(np.uint8).copy()).to(dev)
+    torch.cuda.current_stream(dev).synchronize()   # the copy is on torch's stream, the decode on the engine's
+    out, frames, _, _, read = _decode_dev(
+        engine, dev, fmt, out_at, n, np.dtype(np.int64), n_jobs,
+        lambda out_t, results_t, status_t: engine.flac_decode_dev(data_t, jobs_t[:n_jobs * nat.FLAC_JOB_DTYPE.itemsize], groups_t, out_t,
+                                                                   results_t.view(torch.int64), status_t, fmt))
+    if stats is not None:
+        stats["read_back_bytes"] = ix.nbytes + infos.nbytes + read
+    return _per_file(out, groups, failed, lambda g: (int(frames[g]), int(groups[g]["channels"]), int(infos["sample_rate"][g])))
+
+
 # ---- MPEG Layer I / II, many files decoded on the device (header, side information and samples in device code) ----------------
 
 def mpa_index_files(files, threads=None):
@@ -1159,4 +1203,46 @@ def decode_any_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False,
             stats[kind] = kind_stats
     if stats is not None:
         stats["calls"] = calls
+    return result
+
+
+def decode_any_files_dev(engine, data_t, ranges, fmt=nat.FMT_S16, errors=None, stats=None):
+    """decode_any_files(engine, files, fmt, device=True) for files already in device memory: file i is data_t[offset : offset + len]
+    of ranges[i] ((offset, len) pairs or FILE_RANGE_DTYPE records) in a uint8 CUDA tensor.  Each file is sniffed from its first 4
+    bytes (sniff's rules; the heads come back in one gather), and the files of each kind go, at most once per kind and in
+    decode_any_files' order, to decode_flac_files_dev, decode_aac_files_dev, decode_vorbis_files_dev and decode_mpeg_files_dev,
+    over their ranges on the same data_t: nothing is copied.  Results and messages (errors[i], i its place in `ranges`) are what
+    decode_any_files gives for those bytes.  stats: a dict that receives `calls`, under each kind that ran that decoder's `stats`,
+    and `read_back_bytes`, every byte the call copies from the device.  The per-kind limits and the effects on the engine's state
+    slots and Vorbis registration are decode_any_files'."""
+    import torch
+
+    from .engine import file_ranges
+    r = _resident_files(data_t, ranges, "decode_any_files_dev", len(file_ranges(ranges)))
+    n = len(r)
+    lens = np.minimum(r["len"], 4).astype(np.int64)
+    heads = np.zeros((n, 4), dtype=np.uint8)
+    if n and data_t.numel():
+        at = r["offset"].astype(np.int64)[:, None] + np.minimum(np.arange(4)[None, :], np.maximum(lens[:, None] - 1, 0))
+        heads = data_t[torch.from_numpy(np.minimum(at, data_t.numel() - 1)).to(data_t.device)].cpu().numpy()
+    read = heads.nbytes
+    kinds = [sniff(heads[i, :lens[i]].tobytes()) for i in range(n)]
+    decoders = (("flac", decode_flac_files_dev), ("aac", decode_aac_files_dev), ("vorbis", decode_vorbis_files_dev), ("mpa", decode_mpeg_files_dev))
+    result, calls = [None] * n, []
+    for kind, decode in decoders:
+        mine = [i for i, k in enumerate(kinds) if k == kind]
+        if not mine:
+            continue
+        messages, kind_stats = {}, {}
+        got = decode(engine, data_t, r[mine], fmt, messages, kind_stats)
+        for i, res in zip(mine, got):
+            result[i] = res
+        if errors is not None:
+            errors.update({mine[k]: m for k, m in messages.items()})
+        calls.append(kind)
+        read += kind_stats.get("read_back_bytes", 0)
+        if stats is not None:
+            stats[kind] = kind_stats
+    if stats is not None:
+        stats.update(calls=calls, read_back_bytes=read)
     return result

@@ -410,7 +410,7 @@ class Engine:
         """Allocate, queue, wait and read back, for a device index whose queue(data_t, ranges, cap, *tables, *records) writes
         `cap` records of each dtype of per_cap (None: that table is not written) and one record per file of each dtype of
         per_file.  cap=None: the lengths // min_frame, summed.  Returns the tables, on the device, and the records, read back.
-        adts_index_dev, mpa_index_dev and the device-files decoders of decode.py index through it."""
+        adts_index_dev, mpa_index_dev, flac_index_dev and the device-files decoders of decode.py index through it."""
         import torch
         assert data_t.is_cuda and data_t.is_contiguous() and data_t.dtype == torch.uint8
         r = file_ranges(ranges)
@@ -467,6 +467,29 @@ class Engine:
         self._check(self._lib.symgpu_mpa_index_dev(self._ctx, _dev_ptr(data_t), data_t.numel(), _host_ptr(r), len(r), int(bool(seekable)),
                                                    None if packets_t is None else _dev_ptr(packets_t),
                                                    None if jobs_t is None else _dev_ptr(jobs_t), cap, _dev_ptr(index_t), _dev_ptr(tracks_t)))
+
+    # -- native FLAC frames indexed on the device ---------------------------------------------------------
+    def flac_index_dev(self, data_t, ranges, cap=None):
+        """(packets_t, jobs_t, index, infos) for the native FLAC files data_t[offset : offset + len] of `ranges` (FILE_RANGE_DTYPE
+        records, or (offset, len) pairs) in a uint8 CUDA tensor: packets_t / jobs_t the uint8 bytes of `cap` FLAC_PACKET_DTYPE /
+        FLAC_JOB_DTYPE records on the device, index the files' FLAC_FILE_INDEX_DTYPE records and infos their FLAC_STREAM_INFO_DTYPE
+        records on the host.  File i's info and packets, [first_packet, first_packet + n_packets), equal packetizer.flac_index of its
+        bytes (index["open"] the status where that raises, its info zeros); its jobs are the same frames as byte ranges of data_t,
+        group i, slot = dur.  cap=None: the lengths // 8, summed, which every file fits (a frame is at least 8 bytes)."""
+        from ._native import FLAC_FILE_INDEX_DTYPE, FLAC_JOB_DTYPE, FLAC_MIN_FRAME, FLAC_PACKET_DTYPE, FLAC_STREAM_INFO_DTYPE
+        return self._index_dev(self.flac_index_dev_queue, data_t, ranges, cap, FLAC_MIN_FRAME, (FLAC_PACKET_DTYPE, FLAC_JOB_DTYPE),
+                               (FLAC_FILE_INDEX_DTYPE, FLAC_STREAM_INFO_DTYPE))
+
+    def flac_index_dev_queue(self, data_t, ranges, cap, packets_t, jobs_t, index_t, infos_t):
+        """symgpu_flac_index_dev on uint8 CUDA tensors (packets_t / jobs_t, either None, holding `cap` records; index_t and infos_t
+        one record per file), left queued on the engine's stream after the call's one wait: no wait for torch's stream before it."""
+        from ._native import FLAC_JOB_DTYPE, FLAC_PACKET_DTYPE
+        r = file_ranges(ranges)
+        assert packets_t is None or packets_t.numel() >= cap * FLAC_PACKET_DTYPE.itemsize
+        assert jobs_t is None or jobs_t.numel() >= cap * FLAC_JOB_DTYPE.itemsize
+        self._check(self._lib.symgpu_flac_index_dev(self._ctx, _dev_ptr(data_t), data_t.numel(), _host_ptr(r), len(r),
+                                                    None if packets_t is None else _dev_ptr(packets_t),
+                                                    None if jobs_t is None else _dev_ptr(jobs_t), cap, _dev_ptr(index_t), _dev_ptr(infos_t)))
 
     # -- Vorbis jobs built on the device from the device Ogg index (uint8 CUDA tensors holding the records; queued, no wait) -----
     def vorbis_heads_dev(self, data_t, ranges, packets_t, pieces_t, index_t, heads_t, ranks_t):

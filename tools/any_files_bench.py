@@ -6,6 +6,8 @@ in one call to interleaved samples of one format.
 Measured, each as a host clock around a call that ends in engine.sync(), after every shape has run once, `--repeats` times with the
 variants alternating inside every repeat (median, min and max printed):
   any_host / any_device            the whole corpus, device=False / device=True
+  any_resident                     the whole corpus already in device memory (uploaded once before timing), through
+                                   decode_any_files_dev: sniffed, indexed and decoded on the device
   any_host_lossy / any_device_lossy / decode_files_lossy
                                    the corpus without its FLAC files (decode_files does not take them) through decode_any_files
                                    and through decode_files (front-ends on host threads, one synthesis launch per codec)
@@ -97,10 +99,17 @@ def main():
     if not torch.cuda.is_available():
         sys.exit("any_files_bench: no CUDA device; the timings need one (--plan-only counts without)")
     out["device"] = card()
+    # the corpus resident on the device, back to back, for decode_any_files_dev
+    ranges, at = [], 0
+    for f in files:
+        ranges.append((at, len(f)))
+        at += len(f)
+    resident = torch.from_numpy(np.frombuffer(b"".join(files), dtype=np.uint8).copy()).cuda()
     with sb.Engine(0) as eng:
         kw = dict(threads=args.threads)
         variants = {"any_host": lambda: decode.decode_any_files(eng, files, fmt, **kw),
                     "any_device": lambda: decode.decode_any_files(eng, files, fmt, device=True, **kw),
+                    "any_resident": lambda: decode.decode_any_files_dev(eng, resident, ranges, fmt),
                     "any_host_lossy": lambda: decode.decode_any_files(eng, lossy, fmt, **kw),
                     "any_device_lossy": lambda: decode.decode_any_files(eng, lossy, fmt, device=True, **kw),
                     "decode_files_lossy": lambda: decode.decode_files(eng, lossy, fmt, **kw),
