@@ -1342,6 +1342,69 @@ symgpu_status symgpu_flac_index_dev(symgpu_ctx* ctx, const uint8_t* data, size_t
                                     symgpu_flac_packet* packets, symgpu_flac_job* jobs, size_t cap_packets, symgpu_flac_file_index* index,
                                     symgpu_flac_stream_info* infos);
 
+/* ===================================================================================================
+ * FLAC in Ogg (.oga, and .ogg files written by flac --ogg; DESIGN 5b / 5e): the Ogg packetiser's logical stream mapped to the
+ * FLAC decoder's jobs, as symphonia-format-ogg/src/mappings/flac.rs maps it.  The rules are packetizer.hpp's (ogg_flac_ident,
+ * ogg_flac_is_audio, ogg_flac_packet_block), shared by the host call and the device calls below.
+ *   detection      the stream's first packet is exactly 51 bytes: 0x7f "FLAC", major version 1, minor version and header
+ *                  count (ignored), "fLaC", a STREAMINFO block header of length 34 and the block      flac.rs:43-125
+ *   audio packets  first byte 0xff; 0x00 / 0x80 and metadata packets carry no audio                flac.rs:299-345
+ *   slot           the block size of the packet's frame header under the decoder's rules (its first sync code, then
+ *                  read_frame_header; frame.rs:66-233), 0 when the decoder refuses the header
+ * The decoder applies no Ogg trim (symphonia-bundle-flac has none): a file's output is every frame the decoder accepts, back to
+ * back, as for native FLAC.
+ * ================================================================================================= */
+#define SYMGPU_OGG_FLAC_IDENT_LEN 51
+/* One logical stream, gathered (symgpu_ogg_gather's blob and table): packet k is blob[table[k].offset ..][.. len).  Packet 0 is
+ * the identification packet: SYMGPU_ERR_UNSUPPORTED when it is not Ogg FLAC, SYMGPU_ERR_DECODE when its STREAMINFO is refused
+ * (flac_read_stream_info), and nothing else is written then.  On SYMGPU_OK: *info (first_frame_pos 0), and per packet audio[k]
+ * (1: an audio packet) and slot[k] (its block size; 0 for a packet that is not audio or whose header the decoder refuses). */
+symgpu_status symgpu_ogg_flac_packets(const uint8_t* blob, size_t n, const symgpu_piece* table, size_t n_packets, symgpu_flac_stream_info* info,
+                                      uint8_t* audio, uint32_t* slot);
+
+/* FLAC-in-Ogg jobs built on the device from the tables of symgpu_ogg_index_dev (data, files, packets, pieces, index as it wrote
+ * them; their argument rules: data, packets, pieces and index device memory, files host memory; SYMGPU_ERR_ARG for a range
+ * outside data[0 .. n_bytes) or a missing pointer, SYMGPU_ERR_LIMIT for more than SYMGPU_OGG_MAX_FILES files; both before
+ * anything is launched).  group_of (host memory, one per file) names each file's group: SYMGPU_OGG_FLAC_NO_GROUP leaves the file
+ * out (no record, no audio packet), and the named groups rise with the file index, so that a call can take the Ogg FLAC files
+ * out of a mixed list indexed once.  Each call queues a fixed number of launches, whatever the number of files or packets, and
+ * returns without a host wait. */
+#define SYMGPU_OGG_FLAC_NO_GROUP 0xffffffffu
+typedef struct symgpu_ogg_flac_file {   /* 88 bytes: one group's file                                                          */
+    symgpu_flac_stream_info info;       /* its identification packet's STREAMINFO (first_frame_pos 0); zeros unless status is 0  */
+    uint64_t audio_bytes;               /* its audio packets' lengths, summed                                                     */
+    uint64_t samples;                   /* their slots, summed: the samples per channel the decode may write                      */
+    uint32_t n_stream;                  /* the stream: the file's packets [0, n_stream), those of its first packet's serial       */
+    uint32_t n_audio;                   /* its audio packets: its jobs, in stream order                                           */
+    uint8_t status;                     /* 0, SYMGPU_OGG_FLAC_NO_PACKETS, _NOT_FLAC or _BAD_STREAMINFO (then n_audio is 0)          */
+    uint8_t reserved[7];
+} symgpu_ogg_flac_file;
+enum { SYMGPU_OGG_FLAC_NO_PACKETS = 1, SYMGPU_OGG_FLAC_NOT_FLAC = 2, SYMGPU_OGG_FLAC_BAD_STREAMINFO = 3 };
+typedef struct symgpu_ogg_flac_packet_rank { /* 32 bytes: one packet of the table                                              */
+    uint64_t byte_at;                   /* audio bytes of the packets before it in the table, every file's                         */
+    uint64_t rank;                      /* audio packets before it in the table: an audio packet's job                             */
+    uint64_t samples_at;                /* slots of the audio packets before it                                                     */
+    uint32_t slot;                      /* an audio packet's block size (ogg_flac_packet_block), else 0                             */
+    uint8_t audio;                      /* 1: an audio packet of a file with a group and status 0                                    */
+    uint8_t reserved[3];
+} symgpu_ogg_flac_packet_rank;
+/* heads[g] for every group g < n_groups (a group no file names is left as it was) and ranks[k] for every packet of the table.
+ * One thread per file checks its identification packet, one per packet decides and reads the frame header, one block scans the
+ * table, one thread per file sums.  Four launches.  Scratch from the context's staging buffer: 20 bytes per file. */
+symgpu_status symgpu_ogg_flac_heads_dev(symgpu_ctx* ctx, const uint8_t* data, size_t n_bytes, const symgpu_file_range* files, size_t n_files,
+                                        const symgpu_ogg_packet* packets, size_t n_packets, const symgpu_piece* pieces,
+                                        const symgpu_ogg_file_index* index, const uint32_t* group_of, size_t n_groups,
+                                        symgpu_ogg_flac_file* heads, symgpu_ogg_flac_packet_rank* ranks);
+/* Every audio packet's bytes gathered to out[byte_at ..] and its symgpu_flac_job written to jobs[rank] (offset into `out`,
+ * length, group group_of[file], slot), ranks as symgpu_ogg_flac_heads_dev wrote them: a group's jobs are consecutive and in
+ * stream order, and jobs[0 .. n_jobs) with out[0 .. out_cap) is what symgpu_flac_decode_fmt_dev takes.  A packet whose job or
+ * bytes would pass n_jobs or out_cap is skipped.  One launch, one warp per packet.  Scratch: 20 bytes per file. */
+symgpu_status symgpu_ogg_flac_jobs_dev(symgpu_ctx* ctx, const uint8_t* data, size_t n_bytes, const symgpu_file_range* files, size_t n_files,
+                                       const symgpu_ogg_packet* packets, size_t n_packets, const symgpu_piece* pieces,
+                                       const symgpu_ogg_file_index* index, const uint32_t* group_of,
+                                       const symgpu_ogg_flac_packet_rank* ranks, uint8_t* out, size_t out_cap, symgpu_flac_job* jobs,
+                                       size_t n_jobs);
+
 
 /* ===================================================================================================
  * Vorbis entropy front-end (SURVEY 8f N1): audio packets -> the batch format of symgpu_vorbis_synth_* (unit, floor-1 Y

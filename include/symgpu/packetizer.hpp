@@ -1665,10 +1665,10 @@ SYMGPU_PACKET_HD inline uint32_t ogg_packet_head(const uint8_t* d, const P* piec
 struct VorbisStreamHeads {
     uint32_t n_stream, setup;
 };
-template <class Pk, class P>
-SYMGPU_PACKET_HD inline VorbisStreamHeads vorbis_stream_heads(const uint8_t* d, const Pk* packets, uint32_t n_packets, const P* pieces) {
-    VorbisStreamHeads h{0, 0};
-    if (n_packets == 0) return h;
+// The chosen stream's packets, [0, n): those of the first packet's serial, found by bisection (0 for an empty table).
+template <class Pk>
+SYMGPU_PACKET_HD inline uint32_t ogg_first_stream_len(const Pk* packets, uint32_t n_packets) {
+    if (n_packets == 0) return 0;
     const uint32_t serial = packets[0].serial;
     uint32_t lo = 1, hi = n_packets;
     while (lo < hi) {
@@ -1676,6 +1676,13 @@ SYMGPU_PACKET_HD inline VorbisStreamHeads vorbis_stream_heads(const uint8_t* d, 
         if (packets[mid].serial == serial) lo = mid + 1;
         else hi = mid;
     }
+    return lo;
+}
+template <class Pk, class P>
+SYMGPU_PACKET_HD inline VorbisStreamHeads vorbis_stream_heads(const uint8_t* d, const Pk* packets, uint32_t n_packets, const P* pieces) {
+    VorbisStreamHeads h{0, 0};
+    if (n_packets == 0) return h;
+    const uint32_t lo = ogg_first_stream_len(packets, n_packets);
     h.n_stream = h.setup = lo;
     for (uint32_t k = 1; k < lo; ++k) {
         uint8_t b[7];
@@ -1983,6 +1990,44 @@ SYMGPU_PACKET_HD inline uint64_t flac_value(uint64_t seq) { return seq == 0 ? ~u
 SYMGPU_PACKET_HD inline uint64_t flac_packet_ts(const FlacFrameHeader& h, const FlacStreamInfo& info) {
     const bool fixed = info.block_min == info.block_max;
     return h.by_sample ? h.sequence : h.sequence * (fixed ? info.block_min : h.block);
+}
+
+// ---- FLAC in Ogg (symphonia-format-ogg/src/mappings/flac.rs): the rules of the host index (decode.ogg_flac_index through
+// symgpu_ogg_flac_packets) and of the device job build (ogg_flac_jobs_kernel.cu), on a stream chosen as the Vorbis rules choose it
+// (ogg_first_stream_len).  The mapper's own frame-header parse only times packets; the decoder takes STREAMINFO as its extra data
+// and decodes every audio packet with flac_entropy.h's rules, applying no Ogg trim.
+constexpr uint32_t kOggFlacIdentLen = 51;
+// flac.rs:43-125 on the stream's first packet: exactly 51 bytes of 0x7f "FLAC", major version 1 (minor version and header count
+// ignored), "fLaC", a metadata block header of type STREAMINFO (the last-block flag ignored) and length 34, and the block.
+// Unsupported: not Ogg FLAC (detect() gives no mapper).  Otherwise what flac_read_stream_info gives for the block: an Ogg FLAC
+// stream whose STREAMINFO is refused is DecodeError, as detect() fails then.
+SYMGPU_PACKET_HD inline Status ogg_flac_ident(const uint8_t* p, size_t n, FlacStreamInfo& si) {
+    if (n != kOggFlacIdentLen || p[0] != 0x7f || p[1] != 'F' || p[2] != 'L' || p[3] != 'A' || p[4] != 'C' || p[5] != 1) return Status::Unsupported;
+    if (p[9] != 'f' || p[10] != 'L' || p[11] != 'a' || p[12] != 'C') return Status::Unsupported;
+    if ((p[13] & 0x7f) != 0 || detail::be24(p + 14) != 34) return Status::Unsupported;
+    return flac_read_stream_info(p + 17, 34, si);
+}
+// flac.rs:299-345: a packet is audio when its first byte is 0xff; 0x00 / 0x80 and metadata blocks (any other first byte) are not.
+SYMGPU_PACKET_HD inline bool ogg_flac_is_audio(uint32_t len, uint8_t first) { return len > 0 && first == 0xff; }
+// The most bytes a frame header takes, sync code to CRC-8: 4 + a 7-byte sequence number + 2 (block) + 2 (rate) + 1.
+constexpr uint32_t kFlacMaxHeader = 16;
+// The block size of a packet as the decoder reads it (flac_entropy.h decode_packet: the first sync code of the packet, then
+// read_frame_header, whose rules flac_parse_frame_header restates); 0 where there is no sync code or the decoder refuses the
+// header.  The packet is pieces[0 .. n_pieces) of d.  This is the job's slot: a packet with slot 0 is refused.
+template <class P>
+SYMGPU_PACKET_HD inline uint32_t ogg_flac_packet_block(const uint8_t* d, const P* pieces, uint32_t n_pieces) {
+    uint8_t h[kFlacMaxHeader];
+    uint32_t got = 0;
+    bool prev_ff = false;
+    for (uint32_t k = 0; k < n_pieces && got < kFlacMaxHeader; ++k)
+        for (uint64_t b = 0; b < pieces[k].len && got < kFlacMaxHeader; ++b) {
+            const uint8_t x = d[pieces[k].offset + b];
+            if (got) h[got++] = x;
+            else if (prev_ff && (x & 0xfc) == 0xf8) h[0] = 0xff, h[1] = x, got = 2;
+            else prev_ff = x == 0xff;
+        }
+    FlacFrameHeader fh;
+    return got && flac_parse_frame_header(h, got, fh) ? fh.block : 0;
 }
 
 constexpr size_t kFlacMaxFrame = 16u * 1024 * 1024;  // frame.rs:17: how far past its start a frame's end is looked for

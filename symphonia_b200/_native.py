@@ -168,6 +168,14 @@ VORBIS_FILE_JOBS_DTYPE = np.dtype([("long_block_mask", "<u8"), ("byte_at", "<u8"
 assert VORBIS_FILE_HEADS_DTYPE.itemsize == 32 and VORBIS_PACKET_RANK_DTYPE.itemsize == 24
 assert OGG_PACKET_REF_DTYPE.itemsize == 16 and VORBIS_FILE_JOBS_DTYPE.itemsize == 40
 VORBIS_NO_PACKETS, VORBIS_NO_SETUP = 1, 2
+# FLAC in Ogg: `symgpu_ogg_flac_file` (88 bytes), `symgpu_ogg_flac_packet_rank` (32); jobs are FLAC_JOB_DTYPE
+OGG_FLAC_FILE_DTYPE = np.dtype([("info", FLAC_STREAM_INFO_DTYPE), ("audio_bytes", "<u8"), ("samples", "<u8"), ("n_stream", "<u4"), ("n_audio", "<u4"),
+                                ("status", "u1"), ("reserved", "u1", (7,))])
+OGG_FLAC_PACKET_RANK_DTYPE = np.dtype([("byte_at", "<u8"), ("rank", "<u8"), ("samples_at", "<u8"), ("slot", "<u4"), ("audio", "u1"), ("reserved", "u1", (3,))])
+assert OGG_FLAC_FILE_DTYPE.itemsize == 88 and OGG_FLAC_PACKET_RANK_DTYPE.itemsize == 32
+OGG_FLAC_NO_PACKETS, OGG_FLAC_NOT_FLAC, OGG_FLAC_BAD_STREAMINFO = 1, 2, 3
+OGG_FLAC_NO_GROUP = 0xFFFFFFFF
+OGG_FLAC_IDENT_LEN = 51
 MP3_FILE_DTYPE = np.dtype([("data", "<u8"), ("n", "<u8"), ("packets", "<u8"), ("n_packets", "<u8"), ("stream", "<u4"), ("reserved", "<u4")])
 assert MP3_FILE_DTYPE.itemsize == 40
 VORBIS_SETUP_INFO_DTYPE = np.dtype([("n_codebooks", "<u4"), ("n_floors", "<u4"), ("n_residues", "<u4"), ("n_mappings", "<u4"), ("n_modes", "<u4"),
@@ -369,6 +377,12 @@ def lib():
     L.symgpu_ogg_gather_dev.argtypes = [vp, vp, sz, vp, sz, vp, vp, vp, vp, sz, vp, sz]
     L.symgpu_vorbis_jobs_dev.restype = ctypes.c_int
     L.symgpu_vorbis_jobs_dev.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, vp, vp, vp, vp, sz, vp, sz]
+    L.symgpu_ogg_flac_packets.restype = ctypes.c_int
+    L.symgpu_ogg_flac_packets.argtypes = [vp, sz, vp, sz, vp, vp, vp]
+    L.symgpu_ogg_flac_heads_dev.restype = ctypes.c_int
+    L.symgpu_ogg_flac_heads_dev.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, vp, vp, sz, vp, vp]
+    L.symgpu_ogg_flac_jobs_dev.restype = ctypes.c_int
+    L.symgpu_ogg_flac_jobs_dev.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, vp, vp, vp, vp, sz, vp, sz]
     L.symgpu_ogg_gather.restype = ctypes.c_int
     L.symgpu_ogg_gather.argtypes = [vp, sz, vp, sz, vp, sz, vp, sz, vp, ctypes.POINTER(sz)]
     L.symgpu_ogg_page_end_trims.restype = ctypes.c_int

@@ -205,6 +205,24 @@ extern "C" symgpu_status symgpu_flac_index(const uint8_t* data, size_t n, symgpu
     return SYMGPU_OK;
 }
 
+extern "C" symgpu_status symgpu_ogg_flac_packets(const uint8_t* blob, size_t n, const symgpu_piece* table, size_t n_packets,
+                                                 symgpu_flac_stream_info* info, uint8_t* audio, uint32_t* slot) {
+    if ((!blob && n) || !info || (n_packets && (!table || !audio || !slot))) return SYMGPU_ERR_ARG;
+    for (size_t k = 0; k < n_packets; ++k)
+        if (table[k].offset > n || table[k].len > n - table[k].offset) return SYMGPU_ERR_ARG;
+    if (n_packets == 0) return SYMGPU_ERR_UNSUPPORTED;
+    FlacStreamInfo si{};
+    const Status s = ogg_flac_ident(blob + table[0].offset, table[0].len, si);
+    if (s != Status::Ok) return to_status(s);
+    *info = symgpu_detail::flac_info_record(si, 0);
+    for (size_t k = 0; k < n_packets; ++k) {
+        audio[k] = ogg_flac_is_audio(table[k].len, table[k].len ? blob[table[k].offset] : 0);
+        slot[k] = audio[k] ? ogg_flac_packet_block(blob, table + k, 1) : 0;
+    }
+    return SYMGPU_OK;
+}
+
+static_assert(sizeof(symgpu_ogg_flac_file) == 88 && sizeof(symgpu_ogg_flac_packet_rank) == 32, "record sizes are ABI");
 static_assert(sizeof(symgpu_flac_stream_info) == 56 && sizeof(symgpu_flac_packet) == 24, "record sizes are ABI");
 static_assert(sizeof(symgpu_mpa_track) == 48 && sizeof(symgpu_mpa_packet) == 48 && sizeof(symgpu_adts_packet) == 32, "record sizes are ABI");
 static_assert(sizeof(symgpu_piece) == 16 && sizeof(symgpu_ogg_packet) == 40 && sizeof(symgpu_vorbis_ident) == 8, "record sizes are ABI");

@@ -16,29 +16,15 @@
 
 #include "../../include/symgpu/packetizer.hpp"
 #include "batch_call.h"
+#include "ogg_device.cuh"
 
 namespace {
 
 using namespace symgpu::packet;
 using symgpu_detail::Carver;
+using namespace symgpu_detail::ogg_dev;
 
 constexpr uint32_t kNoFile = 0xffffffffu;
-
-// The file that owns packet p of the table: the last whose first_packet <= p (an empty file shares first_packet with the next).
-__device__ inline uint32_t file_of_packet(const symgpu_ogg_file_index* index, uint32_t n_files, uint64_t p) {
-    uint32_t lo = 0, hi = n_files;
-    while (hi - lo > 1) {
-        const uint32_t mid = (lo + hi) / 2;
-        if (index[mid].first_packet <= p) lo = mid;
-        else hi = mid;
-    }
-    return lo;
-}
-
-// A file's tables are usable when they were written and lie inside the table of n_packets.
-__device__ inline bool tables_ok(const symgpu_ogg_file_index& ix, uint64_t n_packets) {
-    return !(ix.status & SYMGPU_OGG_NOT_WRITTEN) && ix.first_packet + ix.n_packets <= n_packets;
-}
 
 __device__ inline VorbisStreamHeads stream_heads(const symgpu_vorbis_file_heads& h) {
     return VorbisStreamHeads{h.n_stream, h.status ? h.n_stream : h.setup};
@@ -141,17 +127,6 @@ __global__ void vorbis_heads_total_kernel(const symgpu_ogg_packet* __restrict__ 
 }
 
 // ---- gathers --------------------------------------------------------------------------------------------------------------
-
-// One warp copies a packet's pieces back to back to dst.
-__device__ inline void warp_copy_packet(uint8_t* dst, const uint8_t* d, const symgpu_piece* pc, uint32_t n_pieces) {
-    const uint32_t lane = threadIdx.x & 31;
-    uint64_t at = 0;
-    for (uint32_t k = 0; k < n_pieces; ++k) {
-        const symgpu_piece q = pc[k];
-        for (uint32_t b = lane; b < q.len; b += 32) dst[at + b] = d[q.offset + b];
-        at += q.len;
-    }
-}
 
 __global__ void ogg_gather_kernel(const uint8_t* __restrict__ data, const symgpu_file_range* __restrict__ files, uint32_t n_files,
                                   const symgpu_ogg_packet* __restrict__ packets, const symgpu_piece* __restrict__ pieces,
@@ -264,20 +239,6 @@ __global__ void vorbis_job_trim_kernel(uint32_t n_jobs, JobScratch s, symgpu_vor
     const int64_t start = ogg_run_start(have_prev, s.seq[ph], int64_t(s.absgp[ph]), s.seq[h], h == first && next_head == last, tot, disc, end);
     jobs[j].discard = s.discard[j];
     jobs[j].trim_end = ogg_packet_end_trim(start + (s.dur_sum[j] - dur_before), end, s.dur[j], s.discard[j]);
-}
-
-// The argument rules the three calls share with symgpu_ogg_index_dev.
-symgpu_status check_files(const uint8_t* data, size_t n_bytes, const symgpu_file_range* files, size_t n_files) {
-    if ((n_bytes && !data) || (n_files && !files)) return SYMGPU_ERR_ARG;
-    if (n_files > SYMGPU_OGG_MAX_FILES) return SYMGPU_ERR_LIMIT;
-    for (size_t i = 0; i < n_files; ++i)
-        if (files[i].offset > n_bytes || files[i].len > n_bytes - files[i].offset) return SYMGPU_ERR_ARG;
-    return SYMGPU_OK;
-}
-
-unsigned blocks_for(uint64_t threads, unsigned per_block) {
-    const uint64_t b = (threads + per_block - 1) / per_block;
-    return unsigned(b == 0 ? 1 : b < 65535 * 8 ? b : 65535 * 8);
 }
 
 }  // namespace

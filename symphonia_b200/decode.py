@@ -47,17 +47,39 @@ def decode_mpeg_audio(engine, data, fmt=nat.FMT_S16, stream=0):
     return engine.pcm_pack_host(pcm, spans, channels, fmt, total), rate
 
 
-def ogg_vorbis_index(data, serial=None):
-    """Everything about a Vorbis-in-Ogg file short of decoding its audio packets: pages -> packets (symgpu_ogg_index), the logical
-    stream gathered back to back, identification / setup headers, the front-end object (codebooks, floors, ...), per audio packet its
-    place, duration, leading discard (mappings/vorbis.rs:45-107) and end trim against the page granule positions
-    (symphonia-format-ogg/src/logical.rs:164-302)."""
+def ogg_logical_stream(data, serial=None):
+    """(packets, blob, table) of one logical stream of an Ogg file: pages -> packets (symgpu_ogg_index), those of `serial` (by
+    default the first packet's) and their bytes gathered back to back (table[k]: where packet k lies in blob).  ValueError for a
+    file without packets.  Both Ogg mappings, Vorbis and FLAC, start from it."""
     packets, pieces = packetizer.ogg_index(data)
     if len(packets) == 0:
         raise ValueError("no Ogg packets")
     serial = int(packets["serial"][0]) if serial is None else serial
     mine = packets[packets["serial"] == serial]
-    blob, table = packetizer.ogg_gather(data, mine, pieces)       # the logical stream, packets back to back
+    blob, table = packetizer.ogg_gather(data, mine, pieces)
+    return mine, blob, table
+
+
+def _stream_of(data, streams, i):
+    """ogg_logical_stream(data) for file i of a many-file call, unless decode_any_files has already indexed it: then streams[i]
+    is what that gave, or the exception it raised, raised again here."""
+    stream = None if streams is None else streams[i]
+    if isinstance(stream, Exception):
+        raise stream
+    return ogg_logical_stream(data) if stream is None else stream
+
+
+def ogg_vorbis_index(data, serial=None):
+    """Everything about a Vorbis-in-Ogg file short of decoding its audio packets: pages -> packets (symgpu_ogg_index), the logical
+    stream gathered back to back, identification / setup headers, the front-end object (codebooks, floors, ...), per audio packet its
+    place, duration, leading discard (mappings/vorbis.rs:45-107) and end trim against the page granule positions
+    (symphonia-format-ogg/src/logical.rs:164-302)."""
+    return _vorbis_index_of(ogg_logical_stream(data, serial))
+
+
+def _vorbis_index_of(stream):
+    """ogg_vorbis_index of a stream ogg_logical_stream has gathered."""
+    mine, blob, table = stream
     off, ln = table["offset"].astype(np.int64), table["len"].astype(np.int64)
     padded = np.concatenate([blob, np.zeros(8, dtype=np.uint8)])
     b0, b1 = padded[off], padded[off + 1]                           # (bytes beyond a short packet are masked by `ln` below)
@@ -721,6 +743,183 @@ def decode_flac_files_dev(engine, data_t, ranges, fmt=nat.FMT_S32, errors=None, 
     return _per_file(out, groups, failed, lambda g: (int(frames[g]), int(groups[g]["channels"]), int(infos["sample_rate"][g])))
 
 
+# ---- FLAC in Ogg, many files decoded on the device (the native FLAC decoder on jobs made from the Ogg packets) ----------------
+
+def _is_ogg_flac_ident(packet):
+    """Whether a stream whose first packet is `packet` is FLAC in Ogg (mappings/flac.rs detect(): the 51-byte identification
+    packet), whatever its STREAMINFO holds -- a refused STREAMINFO fails the file as Ogg FLAC, as the reference's reader fails.
+    A packet of another length or lead-in (every Vorbis identification header) is decided without a library call."""
+    from .engine import SymgpuError
+    if len(packet) != nat.OGG_FLAC_IDENT_LEN or bytes(packet[:5]) != b"\x7fFLAC":
+        return False
+    table = np.zeros(1, dtype=nat.PIECE_DTYPE)
+    table["len"] = len(packet)
+    try:
+        packetizer.ogg_flac_packets(packet, table)
+    except SymgpuError as e:
+        if e.status == 2:      # SYMGPU_ERR_UNSUPPORTED: not Ogg FLAC
+            return False
+        if e.status != 1:      # (SYMGPU_ERR_DECODE: Ogg FLAC whose STREAMINFO is refused)
+            raise
+    return True
+
+
+def ogg_flac_index(data):
+    """Everything about a FLAC-in-Ogg file short of decoding its frames (symphonia-format-ogg/src/mappings/flac.rs): the logical
+    stream of the first packet's serial gathered back to back (ogg_logical_stream), its identification packet's STREAMINFO, and
+    its audio packets -- dict(info, blob, table (where each audio packet lies in blob), slot (each one's block size from its
+    frame header, 0 where the decoder refuses the header)).  Metadata packets carry no audio, and no Ogg granule trim applies:
+    the reference's FLAC decoder has none.  ValueError without packets; SymgpuError status 2 when the stream is not Ogg FLAC, 1
+    when its STREAMINFO is refused."""
+    return _ogg_flac_index_of(ogg_logical_stream(data))
+
+
+def _ogg_flac_index_of(stream):
+    """ogg_flac_index of a stream ogg_logical_stream has gathered."""
+    _, blob, table = stream
+    info, audio, slot = packetizer.ogg_flac_packets(blob, table)
+    return dict(info=info, blob=blob, table=table[audio], slot=slot[audio])
+
+
+def _flac_fields(info):
+    """A FLAC group's fields from STREAMINFO."""
+    return dict(max_block=int(info["block_max"]), bits_per_sample=int(info["bits_per_sample"]), channels=int(info["channels"]))
+
+
+def ogg_flac_files_plan(files, threads=None, errors=None):
+    """Host half of decode_ogg_flac_files: every file indexed (ogg_flac_index, on `threads` host threads), the gathered logical
+    streams concatenated once, one job per audio packet (slot: its block size) and one group per file, in decode_flac_files'
+    layout.  Returns dict(data, jobs, groups, rates, out_cap, failed).  A file that cannot be indexed (listed in `failed`) gets a
+    group without jobs; its message goes to errors[i] when `errors` is a dict."""
+    return _ogg_flac_files_plan(files, threads, errors, None)
+
+
+def _ogg_flac_files_plan(files, threads, errors, streams):
+    """ogg_flac_files_plan; streams: as _stream_of takes them."""
+    ix, messages = _index_files(range(len(files)), lambda i: _ogg_flac_index_of(_stream_of(files[i], streams, i)), threads)
+    if errors is not None:
+        errors.update(messages)
+    groups = np.zeros(len(files), dtype=nat.FLAC_GROUP_DTYPE)
+    groups["channels"] = 1
+    rates = np.zeros(len(files), dtype=np.int64)
+    parts = []
+    for i, x in enumerate(ix):
+        if x is None:
+            continue
+        info = x["info"]
+        rates[i] = int(info["sample_rate"])
+        j = np.zeros(len(x["table"]), dtype=nat.FLAC_JOB_DTYPE)
+        j["offset"], j["len"], j["group"], j["slot"] = x["table"]["offset"], x["table"]["len"], i, x["slot"]
+        parts.append((i, x["blob"], j, _flac_fields(info), int(x["slot"].astype(np.int64).sum()) * int(info["channels"])))
+    data, jobs, cap, failed = _batch(groups, parts, nat.FLAC_JOB_DTYPE)
+    return dict(data=data, jobs=jobs, groups=groups, rates=rates, out_cap=cap, failed=failed)
+
+
+def decode_ogg_flac_files(engine, files, threads=None, device=False, errors=None, fmt=nat.FMT_S32, stats=None):
+    """[(samples [frames, channels] of `fmt`, sample_rate)] for a list of FLAC-in-Ogg files (.oga, flac --ogg), each what
+    decode_flac_files gives for a native FLAC file holding the same STREAMINFO and frames: the files are indexed on host threads,
+    and ONE device call decodes every audio packet of every file with the native FLAC decoder (frame headers and Rice residuals
+    in device code, restoration and interleaving with the conversion to `fmt` on the GPU).  Every frame the decoder accepts is
+    output, back to back; no Ogg granule trim applies.  device=True: the bytes go to the device once and the samples are CUDA
+    tensors, views of one output tensor.  A file that cannot be indexed -- no packets, not Ogg FLAC, a refused STREAMINFO --
+    yields an empty result with sample rate 0 (its message in errors[i] when `errors` is a dict), and the others still decode.
+    stats: a dict that receives the per-packet `status` (SYMGPU_FLAC_JOB_*).  At most 65 536 files per call."""
+    return _decode_ogg_flac_files(engine, files, threads, device, errors, fmt, stats, None)
+
+
+def _decode_ogg_flac_files(engine, files, threads, device, errors, fmt, stats, streams):
+    """decode_ogg_flac_files; streams: as _stream_of takes them."""
+    if len(files) > nat.FLAC_MAX_FILES:
+        raise ValueError(f"decode_ogg_flac_files takes at most {nat.FLAC_MAX_FILES} files per call, not {len(files)}")
+    plan = _ogg_flac_files_plan(files, threads, errors, streams)
+    groups, rates, cap = plan["groups"], plan["rates"], plan["out_cap"]
+
+    def dev(data_t, jobs_t, groups_t, out_t, frames_t, status_t):
+        import torch
+        engine.flac_decode_dev(data_t, jobs_t, groups_t, out_t, frames_t.view(torch.int64), status_t, fmt)
+    out, group_frames, status, _ = _decode_batch(engine, device, (plan["data"], plan["jobs"], groups), cap, fmt, len(groups), np.dtype(np.int64),
+                                                 lambda: (*engine.flac_decode_host(plan["data"], plan["jobs"], groups, cap, fmt=fmt), None), dev)
+    if stats is not None:
+        stats["status"] = status
+    return _per_file(out, groups, plan["failed"], lambda g: (int(group_frames[g]), int(groups[g]["channels"]), int(rates[g])))
+
+
+def _ogg_flac_refusal(status):
+    """The message ogg_flac_index gives for a file whose device record has this status."""
+    from .engine import SymgpuError
+    if status == nat.OGG_FLAC_NO_PACKETS:
+        return "ValueError: no Ogg packets"
+    return f"SymgpuError: {SymgpuError(2 if status == nat.OGG_FLAC_NOT_FLAC else 1, 'symgpu_ogg_flac_packets')}"
+
+
+def decode_ogg_flac_files_dev(engine, data_t, ranges, fmt=nat.FMT_S32, errors=None, stats=None):
+    """decode_ogg_flac_files(engine, files, device=True, fmt=fmt) for FLAC-in-Ogg files already in device memory: file i is
+    data_t[offset : offset + len] of ranges[i] ((offset, len) pairs or FILE_RANGE_DTYPE records) in a uint8 CUDA tensor, and its
+    result, its message in errors[i] and `stats["status"]` are what decode_ogg_flac_files gives for those bytes.  The pages are
+    indexed, the identification packets checked and every audio packet's job built on the device (symgpu_ogg_index_dev,
+    symgpu_ogg_flac_heads_dev, symgpu_ogg_flac_jobs_dev), and the FLAC decode reads that job table in place; only the per-file
+    records, the frames written per file and the per-packet status come back to the host.  stats also receives
+    `read_back_bytes`, every byte the call copies from the device.  A constant number of launches and host waits per call.  At
+    most 65 536 files."""
+    import torch
+    r = _resident_files(data_t, ranges, "decode_ogg_flac_files_dev", nat.FLAC_MAX_FILES)
+    n = len(r)
+    if n == 0:
+        return []
+    dev = data_t.device
+    torch.cuda.current_stream(dev).synchronize()   # data_t is torch's: written on its stream
+    index_t = _u8(dev, n * nat.OGG_FILE_INDEX_DTYPE.itemsize)
+    engine.ogg_index_dev_queue(data_t, r, _u8(dev, 0), _u8(dev, 0), index_t)
+    engine.sync()
+    ix = index_t.cpu().numpy().view(nat.OGG_FILE_INDEX_DTYPE)
+    n_packets, n_pieces = int(ix["first_packet"][-1]) + int(ix["n_packets"][-1]), int(ix["first_piece"][-1]) + int(ix["n_pieces"][-1])
+    packets_t, pieces_t = _u8(dev, n_packets * nat.OGG_PACKET_DTYPE.itemsize), _u8(dev, n_pieces * nat.PIECE_DTYPE.itemsize)
+    engine.ogg_index_dev_queue(data_t, r, packets_t, pieces_t, index_t)
+    messages, kind_stats = {}, {}
+    out = _ogg_flac_dev(engine, data_t, r, (packets_t, pieces_t, index_t), list(range(n)), fmt, messages, kind_stats)
+    kind_stats["read_back_bytes"] += ix.nbytes
+    if errors is not None:
+        errors.update(messages)
+    if stats is not None:
+        stats.update(kind_stats)
+    return out
+
+
+def _ogg_flac_dev(engine, data_t, r, tables, mine, fmt, messages, stats):
+    """The files r[mine] (indices rising) decoded as FLAC in Ogg from the page index tables (packets_t, pieces_t, index_t) that
+    symgpu_ogg_index_dev wrote for all of r: one group per file of `mine`, the jobs built on the device and decoded in place.
+    Returns the results in the order of `mine`; messages[k] and stats (`status`, `read_back_bytes`: the records, frames and
+    status this reads back) as decode_ogg_flac_files_dev gives them."""
+    import torch
+    packets_t, pieces_t, index_t = tables
+    dev, n = data_t.device, len(mine)
+    group_of = np.full(len(r), nat.OGG_FLAC_NO_GROUP, dtype=np.uint32)
+    group_of[mine] = np.arange(n)
+    # 1. each file's identification packet and audio packets, the slots read from their frame headers
+    heads_t = _u8(dev, n * nat.OGG_FLAC_FILE_DTYPE.itemsize)
+    ranks_t = _u8(dev, packets_t.numel() // nat.OGG_PACKET_DTYPE.itemsize * nat.OGG_FLAC_PACKET_RANK_DTYPE.itemsize)
+    engine.ogg_flac_heads_dev(data_t, r, packets_t, pieces_t, index_t, group_of, heads_t, ranks_t)
+    engine.sync()
+    heads = heads_t.cpu().numpy().view(nat.OGG_FLAC_FILE_DTYPE)
+    messages.update({g: _ogg_flac_refusal(int(h["status"])) for g, h in enumerate(heads) if h["status"]})
+    # 2. the groups, as ogg_flac_files_plan lays them out, and every audio packet's bytes and job
+    groups = np.zeros(n, dtype=nat.FLAC_GROUP_DTYPE)
+    groups["channels"] = 1
+    parts = [(g, int(h["n_audio"]), _flac_fields(h["info"]), int(h["samples"]) * int(h["info"]["channels"])) for g, h in enumerate(heads) if not h["status"]]
+    out_at, failed = _place(groups, parts, None)
+    n_jobs, n_bytes = int(heads["n_audio"].astype(np.int64).sum()), int(heads["audio_bytes"].astype(np.int64).sum())
+    audio_t, jobs_t = _u8(dev, n_bytes), _u8(dev, n_jobs * nat.FLAC_JOB_DTYPE.itemsize)
+    engine.ogg_flac_jobs_dev(data_t, r, packets_t, pieces_t, index_t, group_of, ranks_t, audio_t, jobs_t)
+    # 3. the decode, on the job table in place
+    groups_t = torch.from_numpy(groups.view(np.uint8).copy()).to(dev)
+    torch.cuda.current_stream(dev).synchronize()   # the copy is on torch's stream, the decode on the engine's
+    out, frames, status, _, read = _decode_dev(
+        engine, dev, fmt, out_at, n, np.dtype(np.int64), n_jobs,
+        lambda out_t, results_t, status_t: engine.flac_decode_dev(audio_t, jobs_t, groups_t, out_t, results_t.view(torch.int64), status_t, fmt))
+    stats.update(status=status, read_back_bytes=heads.nbytes + read)
+    return _per_file(out, groups, failed, lambda g: (int(frames[g]), int(groups[g]["channels"]), int(heads["info"]["sample_rate"][g])))
+
+
 # ---- MPEG Layer I / II, many files decoded on the device (header, side information and samples in device code) ----------------
 
 def mpa_index_files(files, threads=None):
@@ -1006,11 +1205,16 @@ def vorbis_files_plan(files, threads=None, errors=None):
     byte-identical identification and setup headers sharing one setup, and one group per file.  Returns dict(data, headers,
     setups, jobs, groups, out_samples, failed).  A file that cannot be indexed or opened -- not Ogg, more than two channels, floor
     type 0, ... (listed in `failed`) -- gets a group without jobs; its message goes to errors[i] when `errors` is a dict."""
-    def index(f):
-        ix = ogg_vorbis_index(f)
+    return _vorbis_files_plan(files, threads, errors, None)
+
+
+def _vorbis_files_plan(files, threads, errors, streams):
+    """vorbis_files_plan; streams: as _stream_of takes them."""
+    def index(i):
+        ix = _vorbis_index_of(_stream_of(files[i], streams, i))
         ix["fe"].close()   # (it checked the setup; the device call builds its own)
         return ix
-    ix, messages = _index_files(files, index, threads)
+    ix, messages = _index_files(range(len(files)), index, threads)
     if errors is not None:
         errors.update(messages)
     groups = np.zeros(len(files), dtype=nat.VORBIS_GROUP_DTYPE)
@@ -1036,9 +1240,14 @@ def decode_vorbis_files(engine, files, fmt=nat.FMT_S16, threads=None, device=Fal
     opened yields an empty result with sample rate 0 (its message in errors[i] when `errors` is a dict), and the others still
     decode.  stats: a dict that receives the per-packet `status` and `n_setups`, the number of distinct setups.  Replaces the
     engine's Vorbis stream and floor registration, as decode_ogg_vorbis does.  At most 65 536 files per call."""
+    return _decode_vorbis_files(engine, files, fmt, threads, device, errors, stats, None)
+
+
+def _decode_vorbis_files(engine, files, fmt, threads, device, errors, stats, streams):
+    """decode_vorbis_files; streams: as _stream_of takes them."""
     if len(files) > nat.VORBIS_MAX_FILES:
         raise ValueError(f"decode_vorbis_files takes at most {nat.VORBIS_MAX_FILES} files per call, not {len(files)}")
-    plan = vorbis_files_plan(files, threads, errors)
+    plan = _vorbis_files_plan(files, threads, errors, streams)
     groups, cap, setups = plan["groups"], plan["out_samples"], plan["setups"]
 
     def host():
@@ -1072,8 +1281,26 @@ def _vorbis_files_dev(engine, data_t, ranges, fmt, errors, stats, mark=None):
     """decode_vorbis_files_dev; mark(phase, state), when given, is called as each phase has been queued: 'start', 'index',
     'heads', 'setup' (the host's work on the headers), 'jobs' (state: the gathered audio bytes, the job table and the groups,
     on the device), 'decode'; state is {} for the others."""
-    import torch
     r = _resident_files(data_t, ranges, "decode_vorbis_files_dev", nat.VORBIS_MAX_FILES)
+    out, parts = _ogg_files_dev(engine, data_t, r, fmt, mark, route_flac=False)
+    _, _, messages, kind_stats = parts[0]
+    if errors is not None:
+        errors.update(messages)
+    if stats is not None:
+        stats.update(kind_stats)
+    return out
+
+
+def _ogg_files_dev(engine, data_t, r, fmt, mark, route_flac):
+    """The Ogg files r (FILE_RANGE_DTYPE records, checked) of data_t decoded on the device, their pages indexed once.  With
+    route_flac, a file whose chosen stream's first packet is an Ogg FLAC identification packet goes to the FLAC decoder (the
+    device has already gathered that packet for the Vorbis header checks, so classifying costs no read), every other file to
+    the Vorbis decoder; without, every file goes to Vorbis.  Returns (results, parts): parts lists ('vorbis', ...) and then
+    ('oggflac', ...) for each kind with a file, as (kind, members (indices into r), {k: message} (k an index into members),
+    stats).  Each kind's stats `read_back_bytes` holds its own files' share of the shared reads -- their page-index and Vorbis
+    head records and their gathered header packets -- plus what its decode reads back, so that the kinds' counts sum to every
+    byte read."""
+    import torch
     n = len(r)
     mark = mark or (lambda phase, state: None)
     dev = data_t.device
@@ -1084,7 +1311,6 @@ def _vorbis_files_dev(engine, data_t, ranges, fmt, errors, stats, mark=None):
     engine.ogg_index_dev_queue(data_t, r, _u8(dev, 0), _u8(dev, 0), index_t)
     engine.sync()
     ix = index_t.cpu().numpy().view(nat.OGG_FILE_INDEX_DTYPE)
-    read = ix.nbytes
     n_packets = int(ix["first_packet"][-1]) + int(ix["n_packets"][-1]) if n else 0
     n_pieces = int(ix["first_piece"][-1]) + int(ix["n_pieces"][-1]) if n else 0
     packets_t, pieces_t = _u8(dev, n_packets * nat.OGG_PACKET_DTYPE.itemsize), _u8(dev, n_pieces * nat.PIECE_DTYPE.itemsize)
@@ -1096,7 +1322,7 @@ def _vorbis_files_dev(engine, data_t, ranges, fmt, errors, stats, mark=None):
     mark("heads", {})
     engine.sync()
     heads = heads_t.cpu().numpy().view(nat.VORBIS_FILE_HEADS_DTYPE)
-    read += heads.nbytes
+    per_file = np.full(n, nat.OGG_FILE_INDEX_DTYPE.itemsize + nat.VORBIS_FILE_HEADS_DTYPE.itemsize, dtype=np.int64)   # each file's share of the reads
     # 3. the header packets gathered into one buffer, read back, and checked on the host as ogg_vorbis_index checks them
     refs, spans, at = [], {}, 0
     for i in range(n):
@@ -1110,11 +1336,14 @@ def _vorbis_files_dev(engine, data_t, ranges, fmt, errors, stats, mark=None):
             refs.append((at, i, int(h["setup"])))
             spans[i].append((at, int(h["setup_len"])))
             at += int(h["setup_len"])
+        per_file[i] += sum(ln for _, ln in spans[i])
     head_t = _u8(dev, at)
     engine.ogg_gather_dev(data_t, r, packets_t, pieces_t, index_t, np.array(refs, dtype=nat.OGG_PACKET_REF_DTYPE), head_t)
     engine.sync()
     head_bytes = head_t.cpu().numpy().tobytes()
-    read += len(head_bytes)
+    flac = [i for i in spans if route_flac and _is_ogg_flac_ident(head_bytes[spans[i][0][0]:spans[i][0][0] + spans[i][0][1]])]
+    flac_set = set(flac)
+    vor = [i for i in range(n) if i not in flac_set]
     messages, opened = {}, {}
 
     def check(ident_b, setup_b):
@@ -1125,75 +1354,111 @@ def _vorbis_files_dev(engine, data_t, ranges, fmt, errors, stats, mark=None):
         except Exception as e:  # noqa: BLE001 -- one bad file must not abort the batch; its message is kept
             return f"{type(e).__name__}: {e}"
     keys = {}
-    for i in range(n):
+    for g, i in enumerate(vor):
         if i not in spans:
-            messages[i] = "ValueError: no Ogg packets"
+            messages[g] = "ValueError: no Ogg packets"
             continue
         parts = [head_bytes[a:a + ln] for a, ln in spans[i]]
         key = (parts[0], parts[1] if len(parts) > 1 else None)
         if key not in opened:    # identical headers are checked once: the checks depend on nothing else
             opened[key] = check(*key)
         if isinstance(opened[key], str):
-            messages[i] = opened[key]
+            messages[g] = opened[key]
         else:
-            keys[i] = key
-    if errors is not None:
-        errors.update(messages)
-    # setups shared by identical headers, groups and each file's share of the jobs, as vorbis_files_plan lays them out
+            keys[g] = key
+    # setups shared by identical headers, groups (one per Vorbis file) and each file's share of the jobs, as vorbis_files_plan
+    # lays them out
     setup_of, setups, headers = _vorbis_setups(list(keys.values()))
     file_jobs = np.zeros(n, dtype=nat.VORBIS_FILE_JOBS_DTYPE)
     placed, job_at, byte_at = [], 0, 0
-    for (i, key), setup in zip(keys.items(), setup_of):
+    for (g, key), setup in zip(keys.items(), setup_of):
+        i = vor[g]
         ident, n_modes, mask = opened[key]
         n_audio, n_bytes = int(heads[i]["n_audio"]), int(heads[i]["audio_bytes"])
-        placed.append((i, n_audio, *_vorbis_group(ident, n_audio, setup)))
+        placed.append((g, n_audio, *_vorbis_group(ident, n_audio, setup)))
         file_jobs[i] = (mask, byte_at, n_bytes, job_at, n_audio, n_modes, ident["bs0_exp"], ident["bs1_exp"], 0)
         job_at, byte_at = job_at + n_audio, byte_at + n_bytes
-    groups = np.zeros(n, dtype=nat.VORBIS_GROUP_DTYPE)
-    out_at, failed = _place(groups, placed, _packed(n, list(keys), [p[1] for p in placed]))
+    groups = np.zeros(len(vor), dtype=nat.VORBIS_GROUP_DTYPE)
+    out_at, failed = _place(groups, placed, _packed(len(vor), list(keys), [p[1] for p in placed]))
     mark("setup", {})
     # 4. every audio packet's bytes and job
-    audio_t, jobs_t = _u8(dev, byte_at), _u8(dev, job_at * nat.VORBIS_JOB_DTYPE.itemsize)
-    engine.vorbis_jobs_dev(data_t, r, packets_t, pieces_t, index_t, ranks_t, file_jobs, audio_t, jobs_t)
-    mark("jobs", dict(audio=audio_t, jobs=jobs_t, groups=groups))
-    # 5. the decode (when every file failed, nothing is decoded and no result is read)
-    out, results, status = torch.empty(0, dtype=getattr(torch, _TORCH_DTYPES[fmt]), device=dev), None, np.zeros(0, dtype=np.uint8)
-    if len(setups):
-        def decode(out_t, results_t, status_t):
-            engine.vorbis_decode_dev(headers, setups, audio_t, jobs_t, groups, fmt, out_t, results_t, status_t)
-            mark("decode", {})
-        out, results, status, _, nread = _decode_dev(engine, dev, fmt, out_at, n, nat.VORBIS_RESULT_DTYPE, job_at, decode)
-        read += nread
-    if stats is not None:
-        stats.update(status=status, n_setups=len(setups), read_back_bytes=read)
-    return _per_file(out, groups, failed, lambda g: (int(results[g]["frames"]), int(results[g]["channels"]), int(results[g]["sample_rate"])))
+    result, parts = [None] * n, []
+    if vor or not route_flac:
+        audio_t, jobs_t = _u8(dev, byte_at), _u8(dev, job_at * nat.VORBIS_JOB_DTYPE.itemsize)
+        engine.vorbis_jobs_dev(data_t, r, packets_t, pieces_t, index_t, ranks_t, file_jobs, audio_t, jobs_t)
+        mark("jobs", dict(audio=audio_t, jobs=jobs_t, groups=groups))
+        # 5. the decode (when every file failed, nothing is decoded and no result is read)
+        out, results, status = torch.empty(0, dtype=getattr(torch, _TORCH_DTYPES[fmt]), device=dev), None, np.zeros(0, dtype=np.uint8)
+        read = int(per_file[vor].sum())
+        if len(setups):
+            def decode(out_t, results_t, status_t):
+                engine.vorbis_decode_dev(headers, setups, audio_t, jobs_t, groups, fmt, out_t, results_t, status_t)
+                mark("decode", {})
+            out, results, status, _, nread = _decode_dev(engine, dev, fmt, out_at, len(vor), nat.VORBIS_RESULT_DTYPE, job_at, decode)
+            read += nread
+        got = _per_file(out, groups, failed, lambda g: (int(results[g]["frames"]), int(results[g]["channels"]), int(results[g]["sample_rate"])))
+        for i, res in zip(vor, got):
+            result[i] = res
+        parts.append(("vorbis", vor, messages, dict(status=status, n_setups=len(setups), read_back_bytes=read)))
+    if flac:
+        flac_messages, flac_stats = {}, {}
+        got = _ogg_flac_dev(engine, data_t, r, (packets_t, pieces_t, index_t), flac, fmt, flac_messages, flac_stats)
+        flac_stats["read_back_bytes"] += int(per_file[flac].sum())
+        for i, res in zip(flac, got):
+            result[i] = res
+        parts.append(("oggflac", flac, flac_messages, flac_stats))
+    return result, parts
 
 
 # ---- a mixed list: every file to the device decoder of its kind ----------------------------------------------------------------
 
+def _stream_or_error(data):
+    """ogg_logical_stream(data), or the exception it raises."""
+    try:
+        return ogg_logical_stream(data)
+    except Exception as e:  # noqa: BLE001 -- kept, and raised again where the file is decoded
+        return e
+
+
 def decode_any_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False, errors=None, stats=None):
     """[(samples [frames, channels] of `fmt`, sample_rate)], one per file in input order, for a list of native FLAC, ADTS AAC-LC,
-    Ogg Vorbis and MPEG audio (Layers I-III) files in any mix: every file is sniffed, and the files of each kind go, at most once
-    per kind, to decode_flac_files, decode_aac_files, decode_vorbis_files and decode_mpeg_files; a kind without a file makes no
-    call.  Every result is what that decoder returns for the file alone with the same `fmt` and `device`.  device=True: the
-    samples are CUDA tensors, views of their kind's output tensor.  A file its decoder cannot index or open yields an empty [0, 0]
-    result with sample rate 0, and its message goes to errors[i], i its place in `files`, when `errors` is a dict.  stats: a dict
-    that receives `calls`, the kinds that ran ('flac', 'aac', 'vorbis', 'mpa'), and under each such kind a dict of what that
-    decoder's `stats` gives (`status`, `n_redecoded`, `n_setups`, `rounds`).  The decoders' limits hold per kind: more than
-    65 536 AAC or Vorbis files is their ValueError.  As those decoders do, the call (re)allocates the engine's MP3 and AAC state
+    Ogg Vorbis, FLAC-in-Ogg and MPEG audio (Layers I-III) files in any mix: every file is sniffed, and the files of each kind go,
+    at most once per kind, to decode_flac_files, decode_aac_files, decode_vorbis_files, decode_ogg_flac_files and
+    decode_mpeg_files; a kind without a file makes no call.  An Ogg file's pages are indexed once: it is FLAC in Ogg when its
+    chosen stream's first packet is an Ogg FLAC identification packet (mappings/flac.rs detect()), else Vorbis.  Every result is
+    what that decoder returns for the file alone with the same `fmt` and `device`.  device=True: the samples are CUDA tensors,
+    views of their kind's output tensor.  A file its decoder cannot index or open yields an empty [0, 0] result with sample rate
+    0, and its message goes to errors[i], i its place in `files`, when `errors` is a dict.  stats: a dict that receives `calls`,
+    the kinds that ran ('flac', 'aac', 'vorbis', 'oggflac', 'mpa'), and under each such kind a dict of what that decoder's
+    `stats` gives (`status`, `n_redecoded`, `n_setups`, `rounds`).  The decoders' limits hold per kind: more than 65 536 AAC,
+    Vorbis or Ogg FLAC files is their ValueError.  As those decoders do, the call (re)allocates the engine's MP3 and AAC state
     slots and replaces its Vorbis stream and floor registration: streaming decoders on the same engine lose their state."""
-    decoders = (("flac", lambda fs, e, st: decode_flac_files(engine, fs, threads, device, e, fmt)),
-                ("aac", lambda fs, e, st: decode_aac_files(engine, fs, fmt, threads, device, e, st)),
-                ("vorbis", lambda fs, e, st: decode_vorbis_files(engine, fs, fmt, threads, device, e, st)),
-                ("mpa", lambda fs, e, st: decode_mpeg_files(engine, fs, fmt, threads, device, e, st)))
+    import concurrent.futures
+    import os
     kinds = [sniff(f) for f in files]
+    ogg = [i for i, k in enumerate(kinds) if k == "vorbis"]
+    streams = {}
+    if ogg:
+        with concurrent.futures.ThreadPoolExecutor(max_workers=threads or os.cpu_count()) as pool:
+            streams = dict(zip(ogg, pool.map(lambda i: _stream_or_error(files[i]), ogg)))
+    for i, st in streams.items():
+        if not isinstance(st, Exception) and len(st[2]) and _is_ogg_flac_ident(st[1][int(st[2]["offset"][0]):][:int(st[2]["len"][0])]):
+            kinds[i] = "oggflac"
+
+    def pick(mine):
+        return [files[i] for i in mine]
+    decoders = (("flac", lambda mine, e, st: decode_flac_files(engine, pick(mine), threads, device, e, fmt)),
+                ("aac", lambda mine, e, st: decode_aac_files(engine, pick(mine), fmt, threads, device, e, st)),
+                ("vorbis", lambda mine, e, st: _decode_vorbis_files(engine, pick(mine), fmt, threads, device, e, st, [streams[i] for i in mine])),
+                ("oggflac", lambda mine, e, st: _decode_ogg_flac_files(engine, pick(mine), threads, device, e, fmt, st, [streams[i] for i in mine])),
+                ("mpa", lambda mine, e, st: decode_mpeg_files(engine, pick(mine), fmt, threads, device, e, st)))
     result, calls = [None] * len(files), []
     for kind, decode in decoders:
         mine = [i for i, k in enumerate(kinds) if k == kind]
         if not mine:
             continue
         messages, kind_stats = {}, {}
-        got = decode([files[i] for i in mine], messages, kind_stats)
+        got = decode(mine, messages, kind_stats)
         for i, r in zip(mine, got):
             result[i] = r
         if errors is not None:
@@ -1210,11 +1475,16 @@ def decode_any_files_dev(engine, data_t, ranges, fmt=nat.FMT_S16, errors=None, s
     """decode_any_files(engine, files, fmt, device=True) for files already in device memory: file i is data_t[offset : offset + len]
     of ranges[i] ((offset, len) pairs or FILE_RANGE_DTYPE records) in a uint8 CUDA tensor.  Each file is sniffed from its first 4
     bytes (sniff's rules; the heads come back in one gather), and the files of each kind go, at most once per kind and in
-    decode_any_files' order, to decode_flac_files_dev, decode_aac_files_dev, decode_vorbis_files_dev and decode_mpeg_files_dev,
-    over their ranges on the same data_t: nothing is copied.  Results and messages (errors[i], i its place in `ranges`) are what
-    decode_any_files gives for those bytes.  stats: a dict that receives `calls`, under each kind that ran that decoder's `stats`,
-    and `read_back_bytes`, every byte the call copies from the device.  The per-kind limits and the effects on the engine's state
-    slots and Vorbis registration are decode_any_files'."""
+    decode_any_files' order, to decode_flac_files_dev, decode_aac_files_dev, decode_vorbis_files_dev, decode_ogg_flac_files_dev
+    and decode_mpeg_files_dev, over their ranges on the same data_t: nothing is copied.  The Ogg files' pages are indexed once, on
+    the device, and the identification packets the Vorbis header step gathers anyway tell FLAC in Ogg from Vorbis (the rule of
+    decode_any_files); the Ogg FLAC files' jobs are then built from the same index.  Results and messages (errors[i], i its place
+    in `ranges`) are what decode_any_files gives for those bytes.  stats: a dict that receives `calls`, under each kind that ran
+    that decoder's `stats`, and `read_back_bytes`, every byte the call copies from the device: the 4-byte heads of every file
+    plus each kind's `read_back_bytes`, where the reads the Ogg kinds share (page-index and Vorbis head records, gathered header
+    packets) count under the kind of the file they belong to.  The per-kind limits and the effects on the engine's state slots
+    and Vorbis registration are decode_any_files', with one difference: the Ogg files are indexed in one device call before they
+    are told apart, so Ogg Vorbis and Ogg FLAC files share one limit of 65 536 files (SYMGPU_OGG_MAX_FILES), counted together."""
     import torch
 
     from .engine import file_ranges
@@ -1227,22 +1497,35 @@ def decode_any_files_dev(engine, data_t, ranges, fmt=nat.FMT_S16, errors=None, s
         heads = data_t[torch.from_numpy(np.minimum(at, data_t.numel() - 1)).to(data_t.device)].cpu().numpy()
     read = heads.nbytes
     kinds = [sniff(heads[i, :lens[i]].tobytes()) for i in range(n)]
-    decoders = (("flac", decode_flac_files_dev), ("aac", decode_aac_files_dev), ("vorbis", decode_vorbis_files_dev), ("mpa", decode_mpeg_files_dev))
+
+    def ogg(data_t, rr, fmt):
+        if len(rr) > nat.OGG_MAX_FILES:
+            raise ValueError(f"decode_any_files_dev takes at most {nat.OGG_MAX_FILES} Ogg files (Vorbis and FLAC in Ogg together) per call, "
+                             f"not {len(rr)}")
+        return _ogg_files_dev(engine, data_t, rr, fmt, None, route_flac=True)
+
+    def one(decode):
+        def run(data_t, rr, fmt):
+            messages, kind_stats = {}, {}
+            got = decode(engine, data_t, rr, fmt, messages, kind_stats)
+            return got, [(None, list(range(len(rr))), messages, kind_stats)]
+        return run
+    decoders = (("flac", one(decode_flac_files_dev)), ("aac", one(decode_aac_files_dev)), ("vorbis", ogg), ("mpa", one(decode_mpeg_files_dev)))
     result, calls = [None] * n, []
     for kind, decode in decoders:
         mine = [i for i, k in enumerate(kinds) if k == kind]
         if not mine:
             continue
-        messages, kind_stats = {}, {}
-        got = decode(engine, data_t, r[mine], fmt, messages, kind_stats)
+        got, parts = decode(data_t, r[mine], fmt)
         for i, res in zip(mine, got):
             result[i] = res
-        if errors is not None:
-            errors.update({mine[k]: m for k, m in messages.items()})
-        calls.append(kind)
-        read += kind_stats.get("read_back_bytes", 0)
-        if stats is not None:
-            stats[kind] = kind_stats
+        for part_kind, members, messages, kind_stats in parts:
+            if errors is not None:
+                errors.update({mine[members[k]]: m for k, m in messages.items()})
+            calls.append(part_kind or kind)
+            read += kind_stats.get("read_back_bytes", 0)
+            if stats is not None:
+                stats[part_kind or kind] = kind_stats
     if stats is not None:
         stats.update(calls=calls, read_back_bytes=read)
     return result

@@ -520,6 +520,32 @@ class Engine:
                                                      _dev_ptr(ranks_t), _host_ptr(file_jobs), _dev_ptr(out_t), out_t.numel(), _dev_ptr(jobs_t),
                                                      jobs_t.numel() // VORBIS_JOB_DTYPE.itemsize))
 
+    # -- FLAC-in-Ogg jobs built on the device from the device Ogg index (uint8 CUDA tensors holding the records; queued, no wait) -
+    def ogg_flac_heads_dev(self, data_t, ranges, packets_t, pieces_t, index_t, group_of, heads_t, ranks_t):
+        """symgpu_ogg_flac_heads_dev: per group (group_of, host uint32 per file, OGG_FLAC_NO_GROUP for a file left out) an
+        OGG_FLAC_FILE_DTYPE record in heads_t, per packet of packets_t an OGG_FLAC_PACKET_RANK_DTYPE record in ranks_t, from the
+        tables ogg_index_dev_queue wrote."""
+        from ._native import OGG_FLAC_FILE_DTYPE, OGG_PACKET_DTYPE
+        r = file_ranges(ranges)
+        group_of = np.ascontiguousarray(group_of, dtype=np.uint32)
+        assert len(group_of) == len(r)
+        self._check(self._lib.symgpu_ogg_flac_heads_dev(self._ctx, _dev_ptr(data_t), data_t.numel(), _host_ptr(r), len(r), _dev_ptr(packets_t),
+                                                        packets_t.numel() // OGG_PACKET_DTYPE.itemsize, _dev_ptr(pieces_t), _dev_ptr(index_t),
+                                                        _host_ptr(group_of), heads_t.numel() // OGG_FLAC_FILE_DTYPE.itemsize, _dev_ptr(heads_t),
+                                                        _dev_ptr(ranks_t)))
+
+    def ogg_flac_jobs_dev(self, data_t, ranges, packets_t, pieces_t, index_t, group_of, ranks_t, out_t, jobs_t):
+        """symgpu_ogg_flac_jobs_dev: every audio packet's bytes gathered to out_t and its FLAC_JOB_DTYPE record (group from
+        group_of) written to jobs_t, from the ranks ogg_flac_heads_dev wrote."""
+        from ._native import FLAC_JOB_DTYPE, OGG_PACKET_DTYPE
+        r = file_ranges(ranges)
+        group_of = np.ascontiguousarray(group_of, dtype=np.uint32)
+        assert len(group_of) == len(r)
+        self._check(self._lib.symgpu_ogg_flac_jobs_dev(self._ctx, _dev_ptr(data_t), data_t.numel(), _host_ptr(r), len(r), _dev_ptr(packets_t),
+                                                       packets_t.numel() // OGG_PACKET_DTYPE.itemsize, _dev_ptr(pieces_t), _dev_ptr(index_t),
+                                                       _host_ptr(group_of), _dev_ptr(ranks_t), _dev_ptr(out_t), out_t.numel(), _dev_ptr(jobs_t),
+                                                       jobs_t.numel() // FLAC_JOB_DTYPE.itemsize))
+
     # -- output stage -------------------------------------------------------------------------
     def pcm_pack_host(self, pcm, spans, channels, fmt, out_frames, plane_stride=0, frames=0, n_spans=None, out=None):
         """Trim + interleave + convert planar f32 `pcm` (any shape, flat indexing) into [out_frames, channels]

@@ -151,3 +151,18 @@ def ogg_gather(data, packets, pieces):
     _check(nat.lib().symgpu_ogg_gather(p, a.size, _vp(packets.ctypes.data), len(packets), _vp(pieces.ctypes.data), len(pieces),
                                        _vp(blob.ctypes.data) if blob.size else None, blob.size, _vp(table.ctypes.data), ctypes.byref(used)), "symgpu_ogg_gather")
     return blob, table
+
+
+def ogg_flac_packets(blob, table):
+    """(STREAMINFO record, audio, slot) of one gathered logical stream (ogg_gather's blob and table) read as FLAC in Ogg
+    (mappings/flac.rs): packet 0 must be the 51-byte identification packet -- SymgpuError status 2 when it is not Ogg FLAC, 1 when
+    its STREAMINFO is refused.  audio[k]: packet k carries a frame (first byte 0xff); slot[k]: that frame's block size under the
+    decoder's header rules, 0 where the decoder refuses the header (and for every other packet)."""
+    a, p = _buf(blob)
+    table = np.ascontiguousarray(table, dtype=nat.PIECE_DTYPE)
+    info = np.zeros(1, dtype=nat.FLAC_STREAM_INFO_DTYPE)
+    audio, slot = np.zeros(len(table), dtype=np.uint8), np.zeros(len(table), dtype=np.uint32)
+    _check(nat.lib().symgpu_ogg_flac_packets(p, a.size, _vp(table.ctypes.data) if len(table) else None, len(table), _vp(info.ctypes.data),
+                                             _vp(audio.ctypes.data) if len(table) else None, _vp(slot.ctypes.data) if len(table) else None),
+           "symgpu_ogg_flac_packets")
+    return info[0], audio.astype(bool), slot
