@@ -1494,6 +1494,99 @@ symgpu_status symgpu_aac_fe_decode_packets_jobs(uint32_t sample_rate, uint32_t c
 /* The dequantisation tables the front-end uses (for tests): x^(4/3) [8192], 2^((i-156)/4) [256], 0.5^((i-155)/4) [256]. */
 void symgpu_aac_fe_tables(float* pow43, float* normal_scf, float* intensity_scf);
 
+/* ===================================================================================================
+ * ALAC (Apple Lossless) in CAF (DESIGN 5b / 5h).  The packet rules are alac_entropy.h's, shared by the CPU front-end and the
+ * device decoder; the CAF rules are packetizer.hpp's (caf_open, caf_varint), shared by the host and the device index.
+ *   map_channels, ElementChannel, decode_inner, decode_sce_or_cpe   symphonia-codec-alac/src/lib.rs:56-264, :315-418, :471-671
+ *   MagicCookie::read                                               symphonia-common/src/apple/audio/alac.rs:34-171
+ *   CafReader::read_chunks, Chunk::read, PacketTable::read          symphonia-format-caf/src/demuxer.rs:362-560, chunks.rs:82-614
+ * A packet carries no state into the next one.  Its samples are the reference's AudioBuffer<i32>: scaled to 32 bits, every
+ * channel no element wrote silent, as many frames as the last element decoded.
+ * ================================================================================================= */
+typedef struct symgpu_alac_group {  /* 32 bytes: what a stream's magic cookie fixes, and where its output goes               */
+    uint64_t out_offset;            /* first sample of the file's [frames][channels] output in `out`                             */
+    uint32_t frame_length;          /* <= 65 536                                                                                */
+    uint8_t bit_depth, pb, mb, kb;
+    uint8_t channels;               /* 1..8; ALAC channel k goes to output channel map_channels[k] of the layout for the count   */
+    uint8_t reserved[15];
+} symgpu_alac_group;
+/* A stream's packets (packet i = data[packets[i].offset .. + len)) decoded on the CPU: status[i] one SYMGPU_FLAC_JOB_* value
+ * (DECODED or REFUSED), frames[i] the frames it gave (0 when refused), and the decoded packets' samples appended to `samples` as
+ * [frames][channels] int32 scaled to 32 bits.  SYMGPU_ERR_LIMIT when samples_cap is too small (frame_length * channels per
+ * packet always suffices); SYMGPU_ERR_ARG for a packet outside `data` or a group the decoder does not take. */
+symgpu_status symgpu_alac_fe_decode_packets(const uint8_t* data, size_t n, const symgpu_piece* packets, size_t n_packets,
+                                            const symgpu_alac_group* group, uint8_t* status, uint32_t* frames, int32_t* samples,
+                                            size_t samples_cap, size_t* n_samples);
+
+/* ALAC decoded on the device, many files per call.  Jobs are symgpu_flac_job records (offset, len, group, slot: the frames a
+ * packet may decode, frame_length for every packet of an index), status values SYMGPU_FLAC_JOB_*, and the layout and checks are
+ * those of symgpu_flac_decode_fmt_host / _dev with symgpu_alac_group for the group: one device thread decodes each packet's
+ * elements and residuals, one thread predicts each decoded channel, and one CTA per packet applies mid/side, splices the tail
+ * bits, scales to 32 bits and writes the file's region in `format`, with the conversions of symgpu_flac_decode_fmt_*.
+ * Host variant: SYMGPU_ERR_ARG also for a group with channels outside 1..8, bit_depth above 32 or frame_length above 65 536.
+ * Device variant: a job failing the kernels' checks gets SYMGPU_FLAC_JOB_INVALID.  Scratch of 6 bytes per slot sample
+ * (channels x slot per job) plus 656 bytes per job comes from the context's staging buffer. */
+typedef symgpu_flac_job symgpu_alac_job;
+symgpu_status symgpu_alac_decode_fmt_host(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_alac_job* jobs, size_t n_jobs,
+                                          const symgpu_alac_group* groups, size_t n_groups, int format, void* out, size_t out_cap,
+                                          uint64_t* group_frames, uint8_t* status);
+symgpu_status symgpu_alac_decode_fmt_dev(symgpu_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const symgpu_alac_job* jobs, size_t n_jobs,
+                                         const symgpu_alac_group* groups, size_t n_groups, int format, void* out, size_t out_cap,
+                                         uint64_t* group_frames, uint8_t* status);
+
+/* CAF index.  A file opens as CafReader::try_new and AlacDecoder::try_new open it, for ALAC with variable bytes and constant
+ * frames per packet; packets are read back to back from data_start, and the first whose end passes the end of the file ends
+ * them (as the reference's read fails there).  Priming and remainder frames are reported, not trimmed: the reference's CAF
+ * reader applies neither. */
+typedef struct symgpu_caf_info {    /* 96 bytes */
+    uint64_t data_start;            /* the first packet's byte in the file: the audio of a sized data chunk, else the file's end */
+    uint64_t n_packets;             /* packets that lie whole in the file                                                        */
+    uint64_t table_at;              /* the last pakt chunk's first integer, in the file                                          */
+    uint64_t table_bytes;           /* the bytes its integers take                                                               */
+    uint64_t table_packets;         /* its packet count                                                                          */
+    int64_t valid_frames;           /* pakt                                                                                      */
+    int32_t priming_frames, remainder_frames;
+    uint32_t frames_per_packet;     /* desc                                                                                      */
+    uint32_t frame_length, max_frame_bytes, avg_bit_rate, sample_rate;  /* the magic cookie                                      */
+    uint16_t max_run;
+    uint8_t compatible_version, bit_depth, pb, mb, kb, channels;
+    uint8_t open;                   /* SYMGPU_OK, SYMGPU_ERR_UNSUPPORTED or SYMGPU_ERR_DECODE                                    */
+    uint8_t reason;                 /* SYMGPU_CAF_*: why it did not open                                                          */
+    uint8_t reserved[10];
+} symgpu_caf_info;
+enum {
+    SYMGPU_CAF_OK = 0, SYMGPU_CAF_TRUNCATED = 1, SYMGPU_CAF_NOT_CAF = 2, SYMGPU_CAF_VERSION = 3, SYMGPU_CAF_BAD_CHUNK = 4,
+    SYMGPU_CAF_NO_DESC = 5, SYMGPU_CAF_BAD_DESC = 6, SYMGPU_CAF_NOT_ALAC = 7, SYMGPU_CAF_LAYOUT = 8, SYMGPU_CAF_BAD_TABLE = 9,
+    SYMGPU_CAF_NO_COOKIE = 10, SYMGPU_CAF_BAD_COOKIE = 11
+};
+typedef struct symgpu_caf_packet {  /* 16 bytes */
+    uint64_t offset;                /* in the file                                                                               */
+    uint32_t size;
+    uint32_t frames;                /* the desc's frames per packet                                                              */
+} symgpu_caf_packet;
+/* Host: *info (open and reason always written, the rest only for a file that opens) and the packets (two-call pattern); returns
+ * info->open. */
+symgpu_status symgpu_caf_index(const uint8_t* data, size_t n, symgpu_caf_info* info, symgpu_caf_packet* packets, size_t cap, size_t* n_out);
+/* CAF indexed on the device: many resident files, two calls.  data, infos, first_packet, packets and jobs are device memory, files
+ * host memory.  SYMGPU_ERR_ARG for a range outside data or a missing pointer, SYMGPU_ERR_LIMIT for more than SYMGPU_CAF_MAX_FILES
+ * files or a file of 2^32 bytes or more, both before any launch.
+ *   symgpu_caf_open_dev     one thread per file walks its chunks (caf_open): infos[i] is what symgpu_caf_index writes for the
+ *                           file's bytes, except n_packets, which is 0 here.  One launch and one host wait.
+ *   symgpu_caf_packets_dev  the packet tables those infos name, read one table byte per thread: a flag per terminating byte, a
+ *                           scan that numbers the integers, each integer assembled from its at most 9 bytes, and a scan by file
+ *                           that turns sizes into offsets.  Then infos[i].n_packets, first_packet[i] (the n_packets of the files
+ *                           before it, summed) and file i's packets at packets[first_packet[i] ..], as symgpu_caf_index gives them,
+ *                           with the same packets as jobs (absolute offsets into data, group i, slot frame_length).  Records at or
+ *                           past cap_packets are not written; the table_packets of the files, summed, always suffice.  One host wait,
+ *                           for the numbers of table bytes and integers, which size the scratch (about 40 bytes per integer and 4 per
+ *                           table byte) from the context's staging buffer. */
+#define SYMGPU_CAF_MAX_FILES 65536
+symgpu_status symgpu_caf_open_dev(symgpu_ctx* ctx, const uint8_t* data, size_t n_bytes, const symgpu_file_range* files, size_t n_files,
+                                  symgpu_caf_info* infos);
+symgpu_status symgpu_caf_packets_dev(symgpu_ctx* ctx, const uint8_t* data, size_t n_bytes, const symgpu_file_range* files, size_t n_files,
+                                     symgpu_caf_info* infos, uint64_t* first_packet, symgpu_caf_packet* packets, symgpu_alac_job* jobs,
+                                     size_t cap_packets);
+
 #ifdef __cplusplus
 }
 #endif

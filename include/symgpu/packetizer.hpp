@@ -2270,5 +2270,226 @@ class FlacIndexer {
     bool have_last_ = false;
 };
 
+// ---- CAF holding ALAC (symphonia-format-caf/src/demuxer.rs:362-560, chunks.rs:82-614; the magic cookie of
+// symphonia-common/src/apple/audio/alac.rs:34-171 and symphonia-codec-alac/src/lib.rs:295-300) -----------------------------
+// caf_open walks the chunks as CafReader::read_chunks does and reads the magic cookie as AlacDecoder::try_new does; the
+// packet table's integers are then read by caf_varint, serially (CafIndexer) or one integer per thread (the device index).
+// The host and device indexes run these functions, so their records are equal by construction.
+
+// Why a file does not open (SYMGPU_CAF_* in include/symgpu.h).
+enum CafReason : uint8_t {
+    kCafOk = 0,
+    kCafTruncated = 1,   // a header, chunk or the packet table runs past the end of the file
+    kCafNotCaf = 2,      // no "caff" marker
+    kCafVersion = 3,     // file version other than 1
+    kCafBadChunk = 4,    // a chunk size the reader refuses, or a second desc chunk
+    kCafNoDesc = 5,      // the first chunk is not desc
+    kCafBadDesc = 6,     // zero sample rate or channel count, or more channels than positions
+    kCafNotAlac = 7,     // a format other than ALAC
+    kCafLayout = 8,      // ALAC without variable bytes and constant frames per packet
+    kCafBadTable = 9,    // negative counts, or an integer of more than 9 bytes
+    kCafNoCookie = 10,   // no kuki chunk
+    kCafBadCookie = 11,  // the magic cookie breaks a rule of MagicCookie::read, or its frame length exceeds 65 536
+};
+
+struct CafAlac {  // what a CAF file holding ALAC says once opened
+    uint64_t data_start = 0;    // the first packet's byte: the audio of a sized data chunk, else the end of the file
+    uint64_t table_at = 0;      // the last pakt chunk's first integer
+    uint64_t table_packets = 0; // and its packet count
+    uint64_t table_bytes = 0;   // and the bytes its integers take
+    int64_t valid_frames = 0;
+    int32_t priming_frames = 0, remainder_frames = 0;
+    uint32_t frames_per_packet = 0;
+    uint32_t frame_length = 0, max_frame_bytes = 0, avg_bit_rate = 0, sample_rate = 0;
+    uint16_t max_run = 0;
+    uint8_t compatible_version = 0, bit_depth = 0, pb = 0, mb = 0, kb = 0, channels = 0;
+    uint8_t reason = kCafOk;
+};
+
+constexpr uint32_t kCaf_alac = detail::tag4("alac"), kCaf_caff = detail::tag4("caff"), kCaf_chan = detail::tag4("chan"), kCaf_data = detail::tag4("data"), kCaf_desc = detail::tag4("desc"), kCaf_frma = detail::tag4("frma"), kCaf_kuki = detail::tag4("kuki"), kCaf_pakt = detail::tag4("pakt");
+
+namespace detail {
+SYMGPU_PACKET_HD inline uint64_t be64(const uint8_t* p) { return uint64_t(be32(p)) << 32 | be32(p + 4); }
+}  // namespace detail
+
+// read_variable_length_integer (chunks.rs:599-615): 7 bits per byte, most significant first, a clear top bit ends it, at most 9
+// bytes.  Status::EndOfStream when the bytes end first (the reference's read_byte fails), DecodeError when the ninth byte does
+// not end it.
+SYMGPU_PACKET_HD inline Status caf_varint(const uint8_t* d, size_t n, uint64_t& at, uint64_t& v) {
+    v = 0;
+    for (int k = 0; k < 9; ++k) {
+        if (at >= n) return Status::EndOfStream;
+        const uint8_t byte = d[at++];
+        v |= byte & 0x7f;
+        if (!(byte & 0x80)) return Status::Ok;
+        v <<= 7;
+    }
+    return Status::DecodeError;
+}
+
+// The format ids AudioDescriptionFormatId::read knows (chunks.rs:282-311); any other fails the file.
+SYMGPU_PACKET_HD inline bool caf_known_format(uint32_t f) {
+    const uint32_t known[15] = {0x6c70636du /* lpcm */, 0x696d6134u /* ima4 */, 0x61616320u /* "aac " */, 0x4d414333u /* MAC3 */,
+                                0x4d414336u /* MAC6 */, 0x756c6177u /* ulaw */, 0x616c6177u /* alaw */, 0x2e6d7031u /* .mp1 */,
+                                0x2e6d7032u /* .mp2 */, 0x2e6d7033u /* .mp3 */, kCaf_alac, 0x666c6163u /* flac */, 0x6f707573u /* opus */, 0, 0};
+    for (int k = 0; k < 13; ++k)
+        if (f == known[k]) return true;
+    return false;
+}
+
+// MagicCookie::read (alac.rs:34-171) and the frame-length limit of AlacDecoder::try_new (lib.rs:295-300).
+SYMGPU_PACKET_HD inline Status caf_alac_cookie(const uint8_t* c, uint64_t len, CafAlac& a) {
+    using detail::be16;
+    using detail::be32;
+    a.reason = kCafBadCookie;
+    if (len < 24) return Status::Unsupported;
+    if (be32(c + 4) == kCaf_frma) c += 12, len -= 12;
+    if (be32(c + 4) == kCaf_alac) c += 12, len -= 12;
+    if (len != 24 && len != 48) return Status::Unsupported;
+    a.frame_length = be32(c), a.compatible_version = c[4], a.bit_depth = c[5], a.pb = c[6], a.mb = c[7], a.kb = c[8], a.channels = c[9];
+    a.max_run = uint16_t(be16(c + 10)), a.max_frame_bytes = be32(c + 12), a.avg_bit_rate = be32(c + 16), a.sample_rate = be32(c + 20);
+    if (a.compatible_version > 0) return Status::Unsupported;
+    if (a.bit_depth > 32 || a.channels < 1 || a.channels > 8) return Status::DecodeError;
+    if (len == 48) {
+        const uint8_t* l = c + 24;
+        if (be32(l) != 24 || be32(l + 4) != kCaf_chan || be32(l + 8) != 0) return Status::DecodeError;
+        // the eight layout tags and their channel counts: (100..127, 142) << 16 | count
+        const uint32_t tag = be32(l + 12), count = tag & 0xffff;
+        const uint32_t tags[8] = {100, 101, 113, 116, 120, 124, 142, 127};
+        if (count < 1 || count > 8 || (tag >> 16) != tags[count - 1]) return Status::DecodeError;
+        if (count != a.channels) return Status::DecodeError;
+        if (be32(l + 16) != 0 || be32(l + 20) != 0) return Status::DecodeError;
+    }
+    if (a.frame_length > 4096 * 16) return Status::Unsupported;
+    a.reason = kCafOk;
+    return Status::Ok;
+}
+
+// CafReader::check_file_header + read_chunks (demuxer.rs:362-560) with Chunk::read (chunks.rs:82-128) and each chunk's reader,
+// then the cookie.  The walk ends only where a chunk ends exactly at the end of the file, as the reference's does; after a data
+// chunk of size -1 the bytes that follow are read as chunks too.  The reader continues after a pakt chunk where its last
+// integer ends and after a chan chunk where its last description ends, whatever their declared sizes say.  Only ALAC with
+// variable bytes and constant frames per packet is taken, the layout every ALAC encoder writes.
+SYMGPU_PACKET_HD inline Status caf_open(const uint8_t* d, uint64_t n, CafAlac& a) {
+    using detail::be32;
+    using detail::be64;
+    a = CafAlac{};
+    auto fail = [&](Status s, uint8_t why) {
+        a.reason = why;
+        return s;
+    };
+    if (n < 4) return fail(Status::EndOfStream, kCafTruncated);
+    if (be32(d) != kCaf_caff) return fail(Status::Unsupported, kCafNotCaf);
+    if (n < 8) return fail(Status::EndOfStream, kCafTruncated);
+    if (detail::be16(d + 4) != 1) return fail(Status::Unsupported, kCafVersion);
+    bool have_desc = false, have_cookie = false, sized_data = false;
+    uint64_t cookie_at = 0, cookie_len = 0, at = 8;
+    for (;;) {
+        if (n - at < 12) return fail(Status::EndOfStream, kCafTruncated);
+        const uint32_t type = be32(d + at);
+        const int64_t size = int64_t(be64(d + at + 4));
+        const uint64_t body = at + 12, left = n - body;
+        if (type == kCaf_desc) {
+            if (size != 32) return fail(Status::DecodeError, kCafBadChunk);
+            if (left < 32) return fail(Status::EndOfStream, kCafTruncated);
+            const uint8_t* p = d + body;
+            if ((be64(p) & 0x7fffffffffffffffull) == 0) return fail(Status::DecodeError, kCafBadDesc);  // rate 0.0 or -0.0
+            const uint32_t bytes_per_packet = be32(p + 16), frames_per_packet = be32(p + 20), channels = be32(p + 24);
+            // AudioDescription::read: an unknown format id fails before the channel count is read; a known one that is not ALAC
+            // is refused here only after the reader's own checks, where the reference would go on to another decoder
+            const uint32_t fmt = be32(p + 8);
+            if (!caf_known_format(fmt)) return fail(Status::Unsupported, kCafNotAlac);
+            if (channels == 0) return fail(Status::DecodeError, kCafBadDesc);
+            if (fmt != kCaf_alac) return fail(Status::Unsupported, kCafNotAlac);
+            if (have_desc) return fail(Status::DecodeError, kCafBadChunk);
+            if (channels > 26) return fail(Status::Unsupported, kCafBadDesc);  // Position::from_count has 26 positions
+            if (bytes_per_packet != 0 || frames_per_packet == 0) return fail(Status::Unsupported, kCafLayout);
+            have_desc = true, a.frames_per_packet = frames_per_packet;
+            at = body + 32;
+        } else if (type == kCaf_data) {
+            if (size != -1 && size < 4) return fail(Status::DecodeError, kCafBadChunk);
+            if (left < 4) return fail(Status::EndOfStream, kCafTruncated);
+            a.data_start = body + 4;
+            sized_data = size != -1;
+            if (sized_data && uint64_t(size - 4) > n - a.data_start) return fail(Status::EndOfStream, kCafTruncated);
+            at = a.data_start + (sized_data ? uint64_t(size - 4) : 0);
+        } else if (type == kCaf_chan) {
+            if (size < 12) return fail(Status::DecodeError, kCafBadChunk);
+            if (left < 12 || uint64_t(be32(d + body + 8)) * 20 > left - 12) return fail(Status::EndOfStream, kCafTruncated);
+            at = body + 12 + uint64_t(be32(d + body + 8)) * 20;
+        } else if (type == kCaf_pakt) {
+            if (size < 24) return fail(Status::DecodeError, kCafBadChunk);
+            if (!have_desc) return fail(Status::DecodeError, kCafNoDesc);
+            if (left < 24) return fail(Status::EndOfStream, kCafTruncated);
+            const int64_t total = int64_t(be64(d + body)), valid = int64_t(be64(d + body + 8));
+            if (total < 0 || valid < 0) return fail(Status::DecodeError, kCafBadTable);
+            a.table_at = body + 24, a.table_packets = uint64_t(total), a.valid_frames = valid;
+            a.priming_frames = int32_t(be32(d + body + 16)), a.remainder_frames = int32_t(be32(d + body + 20));
+            at = a.table_at;
+            for (uint64_t k = 0; k < a.table_packets; ++k) {
+                uint64_t v;
+                const Status vs = caf_varint(d, n, at, v);
+                if (vs == Status::EndOfStream) return fail(vs, kCafTruncated);
+                if (vs != Status::Ok) return fail(vs, kCafBadTable);
+            }
+            a.table_bytes = at - a.table_at;
+        } else {  // kuki, free and every other chunk: skipped (a cookie is kept)
+            if (size < 0) return fail(Status::DecodeError, kCafBadChunk);
+            if (uint64_t(size) > left) return fail(Status::EndOfStream, kCafTruncated);
+            if (type == kCaf_kuki) have_cookie = true, cookie_at = body, cookie_len = uint64_t(size);
+            at = body + uint64_t(size);
+        }
+        if (!have_desc) return fail(Status::DecodeError, kCafNoDesc);
+        if (at == n) break;
+    }
+    if (!sized_data) a.data_start = n;  // no seek back to the audio: the packets are read from where the walk stopped
+    if (!have_cookie) return fail(Status::Unsupported, kCafNoCookie);
+    const uint64_t data_start = a.data_start, table_at = a.table_at, table_packets = a.table_packets, table_bytes = a.table_bytes;
+    const int64_t valid = a.valid_frames;
+    const int32_t priming = a.priming_frames, remainder = a.remainder_frames;
+    const uint32_t fpp = a.frames_per_packet;
+    const Status s = caf_alac_cookie(d + cookie_at, cookie_len, a);
+    a.data_start = data_start, a.table_at = table_at, a.table_packets = table_packets, a.table_bytes = table_bytes, a.valid_frames = valid;
+    a.priming_frames = priming, a.remainder_frames = remainder, a.frames_per_packet = fpp;
+    return s;
+}
+
+// Packets are read back to back from data_start (demuxer.rs:148-160); the first whose end passes the end of the file fails
+// its read and ends the file's packets.  A packet of 2^32 bytes or more ends them too (it cannot fit a file the device index
+// takes, and a decoder job's length is 32 bits).
+SYMGPU_PACKET_HD inline bool caf_packet_fits(uint64_t data_start, uint64_t offset, uint64_t size, uint64_t n) {
+    return size <= 0xffffffffull && data_start <= n && offset <= n - data_start && size <= n - data_start - offset;
+}
+
+struct CafPacket {
+    uint64_t offset;  // in the file
+    uint32_t size, frames;
+};
+
+// Host index: caf_open, then the packet table read integer by integer.
+class CafIndexer {
+public:
+    CafIndexer(const uint8_t* d, size_t n) : d_(d), n_(n) {}
+    Status open() { return caf_open(d_, n_, a_); }
+    const CafAlac& alac() const { return a_; }
+    // The packets in order, up to the first that does not fit.
+    template <class Sink>
+    void packets(Sink&& sink) const {
+        uint64_t at = a_.table_at, offset = 0;
+        for (uint64_t k = 0; k < a_.table_packets; ++k) {
+            uint64_t size;
+            caf_varint(d_, n_, at, size);  // caf_open read them all
+            if (!caf_packet_fits(a_.data_start, offset, size, n_)) return;
+            sink(CafPacket{a_.data_start + offset, uint32_t(size), a_.frames_per_packet});
+            offset += size;
+        }
+    }
+
+private:
+    const uint8_t* d_;
+    uint64_t n_;
+    CafAlac a_{};
+};
+
 }  // namespace packet
 }  // namespace symgpu

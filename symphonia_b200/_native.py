@@ -176,6 +176,22 @@ assert OGG_FLAC_FILE_DTYPE.itemsize == 88 and OGG_FLAC_PACKET_RANK_DTYPE.itemsiz
 OGG_FLAC_NO_PACKETS, OGG_FLAC_NOT_FLAC, OGG_FLAC_BAD_STREAMINFO = 1, 2, 3
 OGG_FLAC_NO_GROUP = 0xFFFFFFFF
 OGG_FLAC_IDENT_LEN = 51
+# ALAC in CAF: `symgpu_alac_group` (32 bytes; jobs are FLAC_JOB_DTYPE, status values FLAC_JOB_*), `symgpu_caf_info` (96),
+# `symgpu_caf_packet` (16), and why a CAF file did not open
+CAF_MAX_FILES = 65536
+ALAC_GROUP_DTYPE = np.dtype([("out_offset", "<u8"), ("frame_length", "<u4"), ("bit_depth", "u1"), ("pb", "u1"), ("mb", "u1"), ("kb", "u1"),
+                             ("channels", "u1"), ("reserved", "u1", (15,))])
+CAF_INFO_DTYPE = np.dtype([("data_start", "<u8"), ("n_packets", "<u8"), ("table_at", "<u8"), ("table_bytes", "<u8"), ("table_packets", "<u8"),
+                           ("valid_frames", "<i8"), ("priming_frames", "<i4"), ("remainder_frames", "<i4"),
+                           ("frames_per_packet", "<u4"), ("frame_length", "<u4"), ("max_frame_bytes", "<u4"), ("avg_bit_rate", "<u4"),
+                           ("sample_rate", "<u4"), ("max_run", "<u2"), ("compatible_version", "u1"), ("bit_depth", "u1"), ("pb", "u1"), ("mb", "u1"),
+                           ("kb", "u1"), ("channels", "u1"), ("open", "u1"), ("reason", "u1"), ("reserved", "u1", (10,))])
+CAF_PACKET_DTYPE = np.dtype([("offset", "<u8"), ("size", "<u4"), ("frames", "<u4")])
+assert ALAC_GROUP_DTYPE.itemsize == 32 and CAF_INFO_DTYPE.itemsize == 96 and CAF_PACKET_DTYPE.itemsize == 16
+CAF_REASONS = {1: "a header, chunk or the packet table runs past the end of the file", 2: "no 'caff' marker", 3: "unsupported CAF version",
+               4: "invalid chunk size or a second desc chunk", 5: "the first chunk is not desc", 6: "invalid audio description",
+               7: "the audio is not ALAC", 8: "ALAC without variable bytes and constant frames per packet", 9: "invalid packet table",
+               10: "no magic cookie", 11: "invalid ALAC magic cookie"}
 MP3_FILE_DTYPE = np.dtype([("data", "<u8"), ("n", "<u8"), ("packets", "<u8"), ("n_packets", "<u8"), ("stream", "<u4"), ("reserved", "<u4")])
 assert MP3_FILE_DTYPE.itemsize == 40
 VORBIS_SETUP_INFO_DTYPE = np.dtype([("n_codebooks", "<u4"), ("n_floors", "<u4"), ("n_residues", "<u4"), ("n_mappings", "<u4"), ("n_modes", "<u4"),
@@ -341,6 +357,18 @@ def lib():
         fn = getattr(L, name)
         fn.restype = ctypes.c_int
         fn.argtypes = [vp, vp, sz, vp, sz, vp, sz, ctypes.c_int, vp, sz, vp, vp]
+    for name in ("symgpu_alac_decode_fmt_host", "symgpu_alac_decode_fmt_dev"):
+        fn = getattr(L, name)
+        fn.restype = ctypes.c_int
+        fn.argtypes = [vp, vp, sz, vp, sz, vp, sz, ctypes.c_int, vp, sz, vp, vp]
+    L.symgpu_alac_fe_decode_packets.restype = ctypes.c_int
+    L.symgpu_alac_fe_decode_packets.argtypes = [vp, sz, vp, sz, vp, vp, vp, vp, sz, psz]
+    L.symgpu_caf_index.restype = ctypes.c_int
+    L.symgpu_caf_index.argtypes = [vp, sz, vp, vp, sz, psz]
+    L.symgpu_caf_open_dev.restype = ctypes.c_int
+    L.symgpu_caf_open_dev.argtypes = [vp, vp, sz, vp, sz, vp]
+    L.symgpu_caf_packets_dev.restype = ctypes.c_int
+    L.symgpu_caf_packets_dev.argtypes = [vp, vp, sz, vp, sz, vp, vp, vp, vp, sz]
     for name in ("symgpu_mpa12_decode_host", "symgpu_mpa12_decode_dev"):
         fn = getattr(L, name)
         fn.restype = ctypes.c_int

@@ -5,6 +5,7 @@
 
 #include "../../include/symgpu.h"
 #include "../../include/symgpu/packetizer.hpp"
+#include "caf_records.h"
 #include "flac_records.h"
 #include "mpa_records.h"
 
@@ -222,6 +223,24 @@ extern "C" symgpu_status symgpu_ogg_flac_packets(const uint8_t* blob, size_t n, 
     return SYMGPU_OK;
 }
 
+extern "C" symgpu_status symgpu_caf_index(const uint8_t* data, size_t n, symgpu_caf_info* info, symgpu_caf_packet* packets, size_t cap, size_t* n_out) {
+    if ((!data && n) || !info || !n_out || (cap && !packets)) return SYMGPU_ERR_ARG;
+    CafIndexer ix(data, n);
+    const Status s = ix.open();
+    *info = symgpu_detail::caf_info_record(ix.alac(), s);
+    *n_out = 0;
+    if (s != Status::Ok) return to_status(s);
+    size_t count = 0;
+    ix.packets([&](const CafPacket& p) {
+        if (count < cap) packets[count] = symgpu_caf_packet{p.offset, p.size, p.frames};
+        ++count;
+    });
+    info->n_packets = count;
+    *n_out = count;
+    return SYMGPU_OK;
+}
+
+static_assert(sizeof(symgpu_caf_info) == 96 && sizeof(symgpu_caf_packet) == 16, "record sizes are ABI");
 static_assert(sizeof(symgpu_ogg_flac_file) == 88 && sizeof(symgpu_ogg_flac_packet_rank) == 32, "record sizes are ABI");
 static_assert(sizeof(symgpu_flac_stream_info) == 56 && sizeof(symgpu_flac_packet) == 24, "record sizes are ABI");
 static_assert(sizeof(symgpu_mpa_track) == 48 && sizeof(symgpu_mpa_packet) == 48 && sizeof(symgpu_adts_packet) == 32, "record sizes are ABI");

@@ -234,13 +234,15 @@ def decode_adts_aac(engine, data, fmt=nat.FMT_S16, stream=0, threads=1):
 # ---- many files at once: one synthesis launch per codec --------------------------------------------------------------------
 
 def sniff(data):
-    """'vorbis' (Ogg capture pattern), 'flac' (native FLAC marker), 'aac' (ADTS: 12 sync bits, layer field 00) or 'mpa' (anything else:
-    the MPEG audio indexer looks for a frame, skipping tags and junk)."""
+    """'vorbis' (Ogg capture pattern), 'flac' (native FLAC marker), 'alac' (CAF marker), 'aac' (ADTS: 12 sync bits, layer field 00)
+    or 'mpa' (anything else: the MPEG audio indexer looks for a frame, skipping tags and junk)."""
     head = bytes(data[:4])
     if head == b"OggS":
         return "vorbis"
     if head == b"fLaC":
         return "flac"  # the integer path has its own entry point (decode_flac); plan_files reports it as an error for that file
+    if head == b"caff":
+        return "alac"
     if len(head) >= 2 and head[0] == 0xFF and (head[1] & 0xF6) == 0xF0:
         return "aac"
     return "mpa"
@@ -253,8 +255,9 @@ def plan_file(data):
         return dict(ogg_vorbis_plan(data), kind="vorbis")
     if kind == "aac":
         return dict(adts_aac_plan(data), kind="aac")
-    if kind == "flac":
-        raise ValueError("native FLAC goes through decode_flac (integer samples), not through the f32 synthesis batches")
+    if kind in ("flac", "alac"):
+        raise ValueError(f"{'native FLAC' if kind == 'flac' else 'ALAC in CAF'} goes through the integer decoders (decode_flac_files, "
+                         "decode_alac_files), not through the f32 synthesis batches")
     layer, payload, runs, spans, rate, channels, total = mpeg_audio_plan(data)
     return dict(kind={1: "mpa1", 2: "mpa2", 3: "mp3"}[layer], payload=payload, runs=runs, spans=spans, sample_rate=rate, channels=channels, total_frames=total)
 
@@ -740,6 +743,100 @@ def decode_flac_files_dev(engine, data_t, ranges, fmt=nat.FMT_S32, errors=None, 
                                                                    results_t.view(torch.int64), status_t, fmt))
     if stats is not None:
         stats["read_back_bytes"] = ix.nbytes + infos.nbytes + read
+    return _per_file(out, groups, failed, lambda g: (int(frames[g]), int(groups[g]["channels"]), int(infos["sample_rate"][g])))
+
+
+# ---- ALAC in CAF, many files decoded on the device (elements, residuals and the adaptive predictor in device code) -------------
+
+def alac_files_plan(files, threads=None, errors=None):
+    """Host half of decode_alac_files: every CAF file indexed (packetizer.caf_index, on `threads` host threads), their bytes
+    concatenated once, one job per packet (slot: the cookie's frame length) and one group per file.  Returns dict(data, jobs,
+    groups, rates, infos, out_cap, failed).  A file that cannot be opened (listed in `failed`) gets a group without jobs; its
+    message goes to errors[i] when `errors` is a dict."""
+    ix, messages = _index_files(files, packetizer.caf_index, threads)
+    if errors is not None:
+        errors.update(messages)
+    groups = np.zeros(len(files), dtype=nat.ALAC_GROUP_DTYPE)
+    groups["channels"] = 1
+    infos = np.zeros(len(files), dtype=nat.CAF_INFO_DTYPE)
+    parts = []
+    for i, x in enumerate(ix):
+        if x is None:
+            continue
+        info, packets = x
+        infos[i] = info
+        j = np.zeros(len(packets), dtype=nat.FLAC_JOB_DTYPE)
+        j["offset"], j["len"], j["group"], j["slot"] = packets["offset"], packets["size"], i, int(info["frame_length"])
+        fields = {k: int(info[k]) for k in ("frame_length", "bit_depth", "pb", "mb", "kb", "channels")}
+        parts.append((i, files[i], j, fields, len(packets) * int(info["frame_length"]) * int(info["channels"])))
+    data, jobs, cap, failed = _batch(groups, parts, nat.FLAC_JOB_DTYPE)
+    return dict(data=data, jobs=jobs, groups=groups, rates=infos["sample_rate"].astype(np.int64), infos=infos, out_cap=cap, failed=failed)
+
+
+def decode_alac_files(engine, files, fmt=nat.FMT_S32, threads=None, device=False, errors=None, stats=None):
+    """[(samples [frames, channels] of `fmt`, sample_rate)] for a list of CAF files holding ALAC: the files are indexed on host
+    threads, and ONE device call decodes every packet of every file -- elements and adaptive Golomb residuals (one thread per
+    packet), the adaptive predictor (one thread per channel of a packet), mid/side, tail bits and the conversion to `fmt` (int32
+    scaled to 32 bits by default) on the GPU.  device=True: the bytes go to the device once and the samples are CUDA tensors,
+    views of one output tensor.  A file that cannot be opened yields an empty result with sample rate 0 (its message in errors[i]
+    when `errors` is a dict); a refused packet adds no frames, as a caller of the reference drops it.  No priming or remainder
+    trim is applied: the reference's CAF reader applies none.  stats: a dict that receives `status`, the per-packet
+    FLAC_JOB_* values in job order."""
+    plan = alac_files_plan(files, threads, errors)
+    groups, rates, cap = plan["groups"], plan["rates"], plan["out_cap"]
+
+    def dev(data_t, jobs_t, groups_t, out_t, frames_t, status_t):
+        import torch
+        engine.alac_decode_dev(data_t, jobs_t, groups_t, out_t, frames_t.view(torch.int64), status_t, fmt)
+    out, group_frames, status, _ = _decode_batch(engine, device, (plan["data"], plan["jobs"], groups), cap, fmt, len(groups), np.dtype(np.int64),
+                                                 lambda: (*engine.alac_decode_host(plan["data"], plan["jobs"], groups, cap, fmt=fmt), None), dev)
+    if stats is not None:
+        stats["status"] = np.asarray(status)
+    return _per_file(out, groups, plan["failed"], lambda g: (int(group_frames[g]), int(groups[g]["channels"]), int(rates[g])))
+
+
+def _caf_message(info):
+    """The message decode_alac_files gives for a file whose index record did not open."""
+    from .engine import SymgpuError
+    e = SymgpuError(int(info["open"]), f"symgpu_caf_index: {nat.CAF_REASONS.get(int(info['reason']), 'refused')}")
+    return f"{type(e).__name__}: {e}"
+
+
+def decode_alac_files_dev(engine, data_t, ranges, fmt=nat.FMT_S32, errors=None, stats=None):
+    """decode_alac_files(engine, files, fmt, device=True) for CAF files already in device memory: file i is data_t[offset :
+    offset + len] of ranges[i] ((offset, len) pairs or FILE_RANGE_DTYPE records) in a uint8 CUDA tensor, and its result, its
+    message in errors[i] and its packets' status are what decode_alac_files gives for those bytes.  The chunks and packet tables
+    are read on the device (Engine.caf_index_dev) into a job table the decode reads in place; only the per-file records, the
+    frames written per file and the per-packet status come back.  stats: a dict that receives `status` and `read_back_bytes`,
+    every byte the call copies from the device.  At most 65 536 files."""
+    import torch
+    r = _resident_files(data_t, ranges, "decode_alac_files_dev", nat.CAF_MAX_FILES)
+    n = len(r)
+    if n == 0:
+        return []
+    dev = data_t.device
+    infos, first, _, jobs_t, read = engine.caf_index_dev(data_t, r)
+    messages = {i: _caf_message(infos[i]) for i in range(n) if infos["open"][i]}
+    if errors is not None:
+        errors.update(messages)
+    groups = np.zeros(n, dtype=nat.ALAC_GROUP_DTYPE)
+    groups["channels"] = 1
+    parts = []
+    for i in range(n):
+        if i not in messages:
+            info = infos[i]
+            fields = {k: int(info[k]) for k in ("frame_length", "bit_depth", "pb", "mb", "kb", "channels")}
+            parts.append((i, int(info["n_packets"]), fields, int(info["n_packets"]) * int(info["frame_length"]) * int(info["channels"])))
+    out_at, failed = _place(groups, parts, None)
+    n_jobs = int(first[-1]) + int(infos["n_packets"][-1])
+    groups_t = torch.from_numpy(groups.view(np.uint8).copy()).to(dev)
+    torch.cuda.current_stream(dev).synchronize()   # the copy is on torch's stream, the decode on the engine's
+    out, frames, status, _, read2 = _decode_dev(
+        engine, dev, fmt, out_at, n, np.dtype(np.int64), n_jobs,
+        lambda out_t, results_t, status_t: engine.alac_decode_dev(data_t, jobs_t[:n_jobs * nat.FLAC_JOB_DTYPE.itemsize], groups_t, out_t,
+                                                                   results_t.view(torch.int64), status_t, fmt))
+    if stats is not None:
+        stats.update(status=status, read_back_bytes=read + read2)
     return _per_file(out, groups, failed, lambda g: (int(frames[g]), int(groups[g]["channels"]), int(infos["sample_rate"][g])))
 
 
@@ -1422,14 +1519,14 @@ def _stream_or_error(data):
 
 def decode_any_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False, errors=None, stats=None):
     """[(samples [frames, channels] of `fmt`, sample_rate)], one per file in input order, for a list of native FLAC, ADTS AAC-LC,
-    Ogg Vorbis, FLAC-in-Ogg and MPEG audio (Layers I-III) files in any mix: every file is sniffed, and the files of each kind go,
-    at most once per kind, to decode_flac_files, decode_aac_files, decode_vorbis_files, decode_ogg_flac_files and
-    decode_mpeg_files; a kind without a file makes no call.  An Ogg file's pages are indexed once: it is FLAC in Ogg when its
+    Ogg Vorbis, FLAC-in-Ogg, MPEG audio (Layers I-III) and ALAC-in-CAF files in any mix: every file is sniffed, and the files of
+    each kind go, at most once per kind, to decode_flac_files, decode_aac_files, decode_vorbis_files, decode_ogg_flac_files,
+    decode_mpeg_files and decode_alac_files; a kind without a file makes no call.  An Ogg file's pages are indexed once: it is FLAC in Ogg when its
     chosen stream's first packet is an Ogg FLAC identification packet (mappings/flac.rs detect()), else Vorbis.  Every result is
     what that decoder returns for the file alone with the same `fmt` and `device`.  device=True: the samples are CUDA tensors,
     views of their kind's output tensor.  A file its decoder cannot index or open yields an empty [0, 0] result with sample rate
     0, and its message goes to errors[i], i its place in `files`, when `errors` is a dict.  stats: a dict that receives `calls`,
-    the kinds that ran ('flac', 'aac', 'vorbis', 'oggflac', 'mpa'), and under each such kind a dict of what that decoder's
+    the kinds that ran ('flac', 'aac', 'vorbis', 'oggflac', 'mpa', 'alac'), and under each such kind a dict of what that decoder's
     `stats` gives (`status`, `n_redecoded`, `n_setups`, `rounds`).  The decoders' limits hold per kind: more than 65 536 AAC,
     Vorbis or Ogg FLAC files is their ValueError.  As those decoders do, the call (re)allocates the engine's MP3 and AAC state
     slots and replaces its Vorbis stream and floor registration: streaming decoders on the same engine lose their state."""
@@ -1451,7 +1548,8 @@ def decode_any_files(engine, files, fmt=nat.FMT_S16, threads=None, device=False,
                 ("aac", lambda mine, e, st: decode_aac_files(engine, pick(mine), fmt, threads, device, e, st)),
                 ("vorbis", lambda mine, e, st: _decode_vorbis_files(engine, pick(mine), fmt, threads, device, e, st, [streams[i] for i in mine])),
                 ("oggflac", lambda mine, e, st: _decode_ogg_flac_files(engine, pick(mine), threads, device, e, fmt, st, [streams[i] for i in mine])),
-                ("mpa", lambda mine, e, st: decode_mpeg_files(engine, pick(mine), fmt, threads, device, e, st)))
+                ("mpa", lambda mine, e, st: decode_mpeg_files(engine, pick(mine), fmt, threads, device, e, st)),
+                ("alac", lambda mine, e, st: decode_alac_files(engine, pick(mine), fmt, threads, device, e, st)))
     result, calls = [None] * len(files), []
     for kind, decode in decoders:
         mine = [i for i, k in enumerate(kinds) if k == kind]
@@ -1476,7 +1574,7 @@ def decode_any_files_dev(engine, data_t, ranges, fmt=nat.FMT_S16, errors=None, s
     of ranges[i] ((offset, len) pairs or FILE_RANGE_DTYPE records) in a uint8 CUDA tensor.  Each file is sniffed from its first 4
     bytes (sniff's rules; the heads come back in one gather), and the files of each kind go, at most once per kind and in
     decode_any_files' order, to decode_flac_files_dev, decode_aac_files_dev, decode_vorbis_files_dev, decode_ogg_flac_files_dev
-    and decode_mpeg_files_dev, over their ranges on the same data_t: nothing is copied.  The Ogg files' pages are indexed once, on
+    and decode_mpeg_files_dev, then CAF files to decode_alac_files_dev, over their ranges on the same data_t: nothing is copied.  The Ogg files' pages are indexed once, on
     the device, and the identification packets the Vorbis header step gathers anyway tell FLAC in Ogg from Vorbis (the rule of
     decode_any_files); the Ogg FLAC files' jobs are then built from the same index.  Results and messages (errors[i], i its place
     in `ranges`) are what decode_any_files gives for those bytes.  stats: a dict that receives `calls`, under each kind that ran
@@ -1510,7 +1608,8 @@ def decode_any_files_dev(engine, data_t, ranges, fmt=nat.FMT_S16, errors=None, s
             got = decode(engine, data_t, rr, fmt, messages, kind_stats)
             return got, [(None, list(range(len(rr))), messages, kind_stats)]
         return run
-    decoders = (("flac", one(decode_flac_files_dev)), ("aac", one(decode_aac_files_dev)), ("vorbis", ogg), ("mpa", one(decode_mpeg_files_dev)))
+    decoders = (("flac", one(decode_flac_files_dev)), ("aac", one(decode_aac_files_dev)), ("vorbis", ogg), ("mpa", one(decode_mpeg_files_dev)),
+                ("alac", one(decode_alac_files_dev)))
     result, calls = [None] * n, []
     for kind, decode in decoders:
         mine = [i for i, k in enumerate(kinds) if k == kind]

@@ -261,6 +261,36 @@ class Engine:
                                                          n_groups, int(fmt), _dev_ptr(out_t), out_t.numel(), _dev_ptr(group_frames_t),
                                                          _dev_ptr(status_t)))
 
+    # -- ALAC ---------------------------------------------------------------------------------
+    def alac_decode_host(self, data, jobs, groups, out_cap, out=None, fmt=_native.FMT_S32):
+        """Device ALAC decoding of many files in one call: as flac_decode_host, with ALAC_GROUP_DTYPE groups (what each file's
+        magic cookie fixes) and FLAC_JOB_DTYPE jobs.  Returns (out, group_frames, status)."""
+        from ._native import ALAC_GROUP_DTYPE, FLAC_JOB_DTYPE
+        a = _byte_view(data)
+        jobs = np.ascontiguousarray(jobs, dtype=FLAC_JOB_DTYPE)
+        groups = np.ascontiguousarray(groups, dtype=ALAC_GROUP_DTYPE)
+        if out is None:
+            out = np.zeros(int(out_cap), dtype=FMT_NUMPY[fmt])
+        assert out.flags.c_contiguous and out.size >= out_cap and (fmt not in FMT_NUMPY or out.dtype == FMT_NUMPY[fmt])
+        group_frames = np.zeros(len(groups), dtype=np.uint64)
+        status = np.zeros(len(jobs), dtype=np.uint8)
+        self._check(self._lib.symgpu_alac_decode_fmt_host(self._ctx, _host_ptr(a), a.size, _host_ptr(jobs), len(jobs), _host_ptr(groups), len(groups),
+                                                          int(fmt), _host_ptr(out), int(out_cap), _host_ptr(group_frames), _host_ptr(status)))
+        return out, group_frames, status
+
+    def alac_decode_dev(self, data_t, jobs_t, groups_t, out_t, group_frames_t, status_t, fmt=_native.FMT_S32):
+        """Device-resident variant of alac_decode_host, with the tensors of flac_decode_dev; asynchronous on the engine's stream."""
+        from ._native import ALAC_GROUP_DTYPE, FLAC_JOB_DTYPE
+        ts = (data_t, jobs_t, groups_t, out_t, group_frames_t, status_t)
+        assert all(t.is_cuda and t.is_contiguous() for t in ts)
+        assert fmt not in FMT_NUMPY or out_t.element_size() == np.dtype(FMT_NUMPY[fmt]).itemsize
+        n_jobs = jobs_t.numel() * jobs_t.element_size() // FLAC_JOB_DTYPE.itemsize
+        n_groups = groups_t.numel() * groups_t.element_size() // ALAC_GROUP_DTYPE.itemsize
+        assert group_frames_t.numel() >= n_groups and group_frames_t.element_size() == 8 and status_t.numel() >= n_jobs
+        self._check(self._lib.symgpu_alac_decode_fmt_dev(self._ctx, _dev_ptr(data_t), data_t.numel(), _dev_ptr(jobs_t), n_jobs, _dev_ptr(groups_t),
+                                                         n_groups, int(fmt), _dev_ptr(out_t), out_t.numel(), _dev_ptr(group_frames_t),
+                                                         _dev_ptr(status_t)))
+
     # -- many files decoded on the device: one calling convention for MPEG Layer I / II, Layer III, AAC-LC and Vorbis -------------
     def _batch_decode_host(self, fn, lead, dtypes, counted, data, jobs, groups, fmt, out_samples, out):
         """fn(ctx, *lead, bytes, jobs, groups, fmt, out, results, status[, &count]) on host arrays; dtypes: (job, group, result).
@@ -423,6 +453,36 @@ class Engine:
         queue(data_t, r, cap, *kept, *read)
         self.sync()
         return (*kept, *(t.cpu().numpy().view(dt) for t, dt in zip(read, per_file)))
+
+    # -- CAF holding ALAC indexed on the device ----------------------------------------------------
+    def caf_index_dev(self, data_t, ranges):
+        """(infos, first_packet, packets_t, jobs_t, read_back_bytes) for the CAF files data_t[offset : offset + len] of `ranges`
+        (FILE_RANGE_DTYPE records, or (offset, len) pairs) in a uint8 CUDA tensor: infos the files' CAF_INFO_DTYPE records and
+        first_packet their uint64 starts, on the host; packets_t / jobs_t the uint8 bytes of CAF_PACKET_DTYPE / FLAC_JOB_DTYPE
+        records on the device, room for every file's table_packets.  File i's info and packets, [first_packet, first_packet +
+        n_packets), equal packetizer.caf_index of its bytes; its jobs are what alac_decode_dev takes (group i).  read_back_bytes
+        counts the two reads of the infos and the one of first_packet."""
+        import torch
+        from ._native import CAF_INFO_DTYPE, CAF_PACKET_DTYPE, FLAC_JOB_DTYPE
+        assert data_t.is_cuda and data_t.is_contiguous() and data_t.dtype == torch.uint8
+        r = file_ranges(ranges)
+        n, d = len(r), data_t.device
+        infos_t = torch.empty(n * CAF_INFO_DTYPE.itemsize, dtype=torch.uint8, device=d)
+        first_t = torch.empty(n * 8, dtype=torch.uint8, device=d)
+        torch.cuda.current_stream(d).synchronize()  # data_t and the outputs are torch's: written / allocated on its stream
+        self._check(self._lib.symgpu_caf_open_dev(self._ctx, _dev_ptr(data_t), data_t.numel(), _host_ptr(r), n, _dev_ptr(infos_t)))
+        self.sync()
+        heads = infos_t.cpu().numpy().view(CAF_INFO_DTYPE)
+        cap = int(heads["table_packets"][heads["open"] == 0].astype(np.int64).sum())
+        packets_t = torch.empty(max(cap, 1) * CAF_PACKET_DTYPE.itemsize, dtype=torch.uint8, device=d)
+        jobs_t = torch.empty(max(cap, 1) * FLAC_JOB_DTYPE.itemsize, dtype=torch.uint8, device=d)
+        torch.cuda.current_stream(d).synchronize()
+        self._check(self._lib.symgpu_caf_packets_dev(self._ctx, _dev_ptr(data_t), data_t.numel(), _host_ptr(r), n, _dev_ptr(infos_t),
+                                                     _dev_ptr(first_t), _dev_ptr(packets_t), _dev_ptr(jobs_t), cap))
+        self.sync()
+        infos = infos_t.cpu().numpy().view(CAF_INFO_DTYPE)
+        first = first_t.cpu().numpy().view(np.uint64)
+        return infos, first, packets_t, jobs_t, heads.nbytes + infos.nbytes + first.nbytes
 
     # -- ADTS frames indexed on the device ---------------------------------------------------------
     def adts_index_dev(self, data_t, ranges, cap=None):

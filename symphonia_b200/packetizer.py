@@ -118,6 +118,22 @@ def flac_index(data):
     return info[0], packets
 
 
+def caf_index(data):
+    """(info record, packets) of a CAF file holding ALAC: CAF_INFO_DTYPE and CAF_PACKET_DTYPE records.  SymgpuError status 2 for a
+    file that is not CAF, not ALAC or not in the packet layout ALAC uses, 1 for a malformed one; its message names the reason."""
+    L = nat.lib()
+    a, p = _buf(data)
+    info = np.zeros(1, dtype=nat.CAF_INFO_DTYPE)
+    n = ctypes.c_size_t(0)
+    rc = L.symgpu_caf_index(p, a.size, _vp(info.ctypes.data), None, 0, ctypes.byref(n))
+    if rc != 0:
+        raise SymgpuError(rc, f"symgpu_caf_index: {nat.CAF_REASONS.get(int(info['reason'][0]), 'refused')}")
+    packets = np.zeros(n.value, dtype=nat.CAF_PACKET_DTYPE)
+    if n.value:
+        _check(L.symgpu_caf_index(p, a.size, _vp(info.ctypes.data), _vp(packets.ctypes.data), n.value, ctypes.byref(n)), "symgpu_caf_index")
+    return info[0], packets
+
+
 def vorbis_setup_parse(packet, ident):
     """(info record, floors [n_floors] VORBIS_FLOOR1_DTYPE): the decoder's reading of a setup packet; floors of type 1 are ready for
     Engine.vorbis_floors_set."""
